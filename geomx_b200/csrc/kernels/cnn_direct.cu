@@ -1,24 +1,30 @@
 // Direct (fp32 FMA) convolution kernels for the small-batch regime of the reference's demo CNN
 //   Conv2D(16,k5,relu) -> MaxPool2 -> Conv2D(32,k5,relu) -> MaxPool2      (examples/cnn.py:56-60, input 1x28x28)
 // forward and backward, TWO launches in total:
-//   cnn_fwd_kernel      x -> a1 (+argmax) -> a2 (+argmax)          both convolutions, bias, ReLU and both max-pools; a1 stays in shared memory
-//   cnn_bwd_all_kernel  one heterogeneous grid: CTAs [0, 4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1 data gradient + pool/ReLU
-//                       backward of both layers + conv0 weight gradient), CTAs [4B, 4B+128)  da2, a1 -> dW1, db1  (conv1 weight gradient,
-//                       sparse: one non-zero per pooling window).  Both bodies resolve the programmatic grid dependency only AFTER the staging
-//                       that does not depend on the preceding kernel, so the CTAs become resident and stage while that kernel still runs.
-//                       (cnn_bwd_kernel / cnn_wgrad1_kernel: the same bodies as separate launches; cnn_bwd_exchange_kernel: the same grid
-//                       whose last CTAs also perform the conv keys' exchange — measured, no gain, opt-in.)
+//   cnn_fwd_kernel      x -> a1 (+argmax) -> a2 (+argmax)          both convolutions, bias, ReLU and both max-pools; one 4-CTA cluster per
+//                       image: each CTA computes a quarter of conv0 and shares it through distributed shared memory, so conv0 runs once
+//   cnn_bwd_all_kernel  one heterogeneous grid: CTAs [128, 128+4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1 data gradient gathered
+//                       from the non-zeros of dz2 + pool/ReLU backward of both layers + conv0 weight gradient), CTAs [0, 128)  da2, a1 -> dW1, db1
+//                       (conv1 weight gradient); both exploit the sparsity of dz2 (one non-zero per pooling window).  Both bodies resolve
+//                       the programmatic grid dependency only AFTER the staging that does not depend on the preceding kernel, so the CTAs
+//                       become resident and stage while that kernel still runs.
+//                       (cnn_bwd_kernel / cnn_wgrad1_kernel: the same bodies as separate launches; cnn_bwd_exchange_kernel: the same bodies
+//                       in one grid (data-gradient CTAs first) whose last CTAs also perform the conv keys' exchange — measured, no gain, opt-in.)
 //
 // Why not the tensor-core GEMM here: with a per-worker batch of 32 the conv1 products are M = 2048 x N = 32 x K = 400 — 16 tensor-core
 // tiles.  Forward + dgrad + wgrad + im2col/col2im traffic through the GEMM path is several launches of latency-bound work on 16 SMs, while
 // the same 78 MFLOP spread over 128 CTAs of plain FMAs finish in a few microseconds, in exact fp32 (the reference's cublasSgemmEx precision).  The max-pool makes
-// the backward pass 4x sparse (one non-zero per 2x2 window), which the weight-gradient kernel exploits.  Larger batches / other geometries use
+// the backward pass 4x sparse (one non-zero per 2x2 window), which both conv1 gradients exploit.  Larger batches / other geometries use
 // the wgmma GEMM path (ops/functional.py conv2d).
 //
 // Reference kernels replaced: im2col_gpu_kernel / col2im_gpu_kernel (src/operator/nn/im2col.cuh:79-187), per-image cublasSgemmEx
 // (convolution-inl.h:165-284), bias broadcast, ReLU (activation-inl.h:89-121), pool_max_2d / unpool (pool.cuh:128-165, 379-432).
 #include "common.cuh"
 #include "hips_ll.cuh"
+
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 namespace gx {
 
@@ -77,32 +83,36 @@ __device__ __forceinline__ float pool4(const float (&a)[4], float bias, int& bi)
 }
 
 // ------------------------------------------------------------------------------------------------------------------ forward
-// grid (B, 4), 256 threads.  CTA (b, g): conv0 of image b (all 16 channels, kept in shared memory) and conv1 for output channels [8g, 8g+8).
-__global__ void __launch_bounds__(256) cnn_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0,
-                                                       const float* __restrict__ w1, const float* __restrict__ b1, float* __restrict__ a1,
-                                                       unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2,
-                                                       const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
-                                                       unsigned long long* dbg) {
+// grid (B, 4), 256 threads, clusters of (1, 4, 1): the four CTAs of image b.  CTA (b, g) computes conv0 channels [4g, 4g+4) and stores them
+// into the conv0 map of all four CTAs of its cluster (distributed shared memory), then conv1 for output channels [8g, 8g+8) over all 16.
+__global__ void __cluster_dims__(1, 4, 1) __launch_bounds__(256)
+    cnn_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                   const float* __restrict__ b1, float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
+                   unsigned char* __restrict__ idx2, const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n,
+                   float* __restrict__ x_keep, unsigned long long* dbg) {
   __shared__ __align__(16) float sx[CD_H * CD_H];
-  __shared__ __align__(16) float sw0[CD_C1 * CD_W1PAD];
-  __shared__ float sb0[CD_C1];
+  __shared__ __align__(16) float sw0[4 * CD_W1PAD];
+  __shared__ float sb0[4];
   __shared__ __align__(16) float sa1[CD_C1 * CD_P1 * CD_P1];
   __shared__ __align__(16) float sw1[8 * CD_C1 * CD_W1PAD];
   __shared__ float sb1[8];
   __shared__ __align__(16) float spart[4 * 64 * 8];
+  cg::cluster_group cluster = cg::this_cluster();
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
   stamp(0);
+  // the conv0 stores below go into the other CTAs' shared memory, which must exist by then: arrive now, wait after the staging
+  cluster.barrier_arrive();
   pdl_wait();
   pdl_launch();
-  const int b = blockIdx.x, g = blockIdx.y, tid = threadIdx.x;
+  const int b = blockIdx.x, g = blockIdx.y, tid = threadIdx.x;     // g == cluster.block_rank()
   // look-ahead steps: this launch is the tail of the previous batch's step; it hands the labels that arrived with its image batch over to
   // the buffer the classifier head of the NEXT launch reads (a 128-byte side job instead of a copy node in the step graph)
   if (carry_n > 0 && b == 0 && g == 0) for (int i = tid; i < carry_n; i += 256) carry_dst[i] = carry_src[i];
   for (int i = tid; i < CD_H * CD_H / 4; i += 256) cpa16(sx + 4 * i, x + (long long)b * CD_H * CD_H + 4 * i);
-  for (int i = tid; i < CD_C1 * 25; i += 256) { const int ch = i / 25, t = i - ch * 25; cpa4(sw0 + ch * CD_W1PAD + t, w0 + i); }
-  for (int i = tid; i < CD_C1 * 3; i += 256) sw0[(i / 3) * CD_W1PAD + 25 + i % 3] = 0.f;          // pad taps 25..27
-  if (tid < CD_C1) sb0[tid] = b0[tid];
+  if (tid < 4 * 25) { const int cl = tid / 25, t = tid - cl * 25; cpa4(sw0 + cl * CD_W1PAD + t, w0 + 4 * g * 25 + tid); }
+  if (tid < 4 * 3) sw0[(tid / 3) * CD_W1PAD + 25 + tid % 3] = 0.f;                                   // pad taps 25..27
+  if (tid < 4) sb0[tid] = b0[4 * g + tid];
   {
     const float* wsrc = w1 + (long long)(8 * g) * CD_C1 * 25;      // the 8 output channels of this CTA: 3200 contiguous floats
     for (int i = tid; i < 8 * CD_C1 * 25; i += 256) { const int r = i / 25, t = i - r * 25; cpa4(sw1 + r * CD_W1PAD + t, wsrc + i); }
@@ -111,18 +121,19 @@ __global__ void __launch_bounds__(256) cnn_fwd_kernel(const float* __restrict__ 
   if (tid < 8) sb1[tid] = b1[8 * g + tid];
   cpa_wait_all();
   __syncthreads();
+  cluster.barrier_wait();
   stamp(1);
   // look-ahead steps: the backward pass of this batch runs in the NEXT launch, after the following batch has overwritten x — keep a copy
   if (x_keep != nullptr && g == 0) for (int i = tid; i < CD_H * CD_H / 4; i += 256)
     reinterpret_cast<float4*>(x_keep + (long long)b * CD_H * CD_H)[i] = reinterpret_cast<const float4*>(sx)[i];
-  // ---- conv0 + bias + ReLU + pool: thread -> channel tid/16, windows (tid%16) + 16 j
+  // ---- conv0 + bias + ReLU + pool of this CTA's 4 channels: thread -> channel 4g + tid/64, windows (tid%64) + 64 j
   {
-    const int ch = tid >> 4, sub = tid & 15;
+    const int cl = tid >> 6, sub = tid & 63, ch = 4 * g + cl;
     float w[28];
-    load_w28(sw0 + ch * CD_W1PAD, w);
-    const float bias = sb0[ch];
+    load_w28(sw0 + cl * CD_W1PAD, w);
+    const float bias = sb0[cl];
 #pragma unroll 1
-    for (int win = sub; win < CD_P1 * CD_P1; win += 16) {
+    for (int win = sub; win < CD_P1 * CD_P1; win += 64) {
       const int ph = win / CD_P1, pw = win - ph * CD_P1;
       float pt[6][6];
       load_patch(sx + (2 * ph) * CD_H + 2 * pw, CD_H, pt);
@@ -130,14 +141,13 @@ __global__ void __launch_bounds__(256) cnn_fwd_kernel(const float* __restrict__ 
       window_fma(pt, w, acc);
       int bi;
       const float v = pool4(acc, bias, bi);
-      sa1[ch * CD_P1 * CD_P1 + win] = v;
-      if (g == 0) {
-        const long long o = ((long long)b * CD_C1 + ch) * (CD_P1 * CD_P1) + win;
-        a1[o] = v; idx1[o] = (unsigned char)bi;
-      }
+#pragma unroll
+      for (int r = 0; r < 4; ++r) cluster.map_shared_rank(sa1, r)[ch * CD_P1 * CD_P1 + win] = v;
+      const long long o = ((long long)b * CD_C1 + ch) * (CD_P1 * CD_P1) + win;
+      a1[o] = v; idx1[o] = (unsigned char)bi;
     }
   }
-  __syncthreads();
+  cluster.sync();      // all 16 conv0 channels of image b are in every CTA's sa1
   stamp(2);
   // ---- conv1: thread -> input-channel quarter cq, output-channel pair op, pooling window win; 2 oc x 4 pixels accumulators
   {
@@ -177,21 +187,22 @@ __global__ void __launch_bounds__(256) cnn_fwd_kernel(const float* __restrict__ 
 
 // ------------------------------------------------------------------------------------------------------------------ backward (data + conv0)
 // grid (B, 4), 288 threads.  CTA (b, cg): conv1-input channels [4cg, 4cg+4) of image b.
-//   dz2 (32 x 8 x 8, one non-zero per pooling window where a2 > 0) is scattered into a zero-padded 32 x 16 x 16 plane in shared memory;
-//   da1 = full correlation with the flipped filters = the forward window routine on the padded plane; da1 never leaves shared memory:
-//   it is max-pool / ReLU routed straight into conv0's weight and bias gradient (the first layer needs no input gradient).
+//   dz2 (32 x 8 x 8) has at most one non-zero per 2x2 pooling window: at the window's arg-max, where a2 > 0.  Those non-zeros are listed per
+//   window position (16 lists of up to 32 output channels) and da1 is gathered from them: an output pixel (y, x) of the 12x12 map can only be
+//   reached by the 3x3 pooling windows around window (y/2 - 1, x/2 - 1), so it runs over those lists, i.e. over the non-zeros only.  The filter
+//   planes are zero-padded to 7x7, so that the one or two arg-max positions of a window that fall just outside a pixel's 5x5 footprint add 0
+//   instead of needing a test.  da1 never leaves shared memory: it is max-pool / ReLU routed straight into conv0's weight and bias gradient (the
+//   first layer needs no input gradient).
 struct CnnBwdSmem {
-  static constexpr int DZLD = 22;                                 // row stride of the padded dz2 plane: 16 + 6 floats keeps the 6x6 patch loads of a
-                                                                 // warp (6 windows per row pair, rows 2*ld apart) on distinct banks
-  static constexpr int DZPL = 16 * DZLD;                         // floats per plane
-  static constexpr int DZ = 0;                                   // [32][16][DZLD]
-  static constexpr int WT = DZ + CD_C2 * DZPL;                   // [4 cl][32 oc][28] flipped filters
-  static constexpr int X = WT + 4 * CD_C2 * CD_W1PAD;            // [28][28]
+  static constexpr int WT = 0;                                   // [2 cl pairs][32 oc][7][7] float2: W1[oc][4cg+2cp+{0,1}][r-1][s-1], 0 on the border
+  static constexpr int X = WT + 2 * CD_C2 * 49 * 2;              // [28][28]
   static constexpr int A1 = X + CD_H * CD_H;                     // [4][144] pooled conv0 activations (ReLU mask)
   static constexpr int DA1 = A1 + 4 * 144;                       // [4][144] -> routed gradient g
-  static constexpr int PART = DA1 + 4 * 144;                     // [4 ocq][72][8]
-  static constexpr int POS = PART + 4 * 72 * 8;                  // [4][144] int: top-left of the arg-max pixel in the 24x24 map (as x offset)
-  static constexpr int TOTAL = POS + 4 * 144;
+  static constexpr int POS = DA1 + 4 * 144;                      // [4][144] int: top-left of the arg-max pixel in the 24x24 map (as x offset)
+  static constexpr int NZ = POS + 4 * 144;                       // [16 windows][32] float2 {dz2 value, weight offset oc*49 - (iy*7 + ix)}
+  static constexpr int NZSRC = NZ + 16 * 32 * 2;                 // [16][32] int: oc*16 + window (index into the image's dz2 / da2)
+  static constexpr int NZCNT = NZSRC + 16 * 32;                  // [16] int: list lengths
+  static constexpr int TOTAL = NZCNT + 16;
   static constexpr int BYTES = TOTAL * 4;
 };
 
@@ -200,25 +211,49 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
                                              const unsigned char* __restrict__ idx2, const float* __restrict__ da2, float* __restrict__ dw0,
                                              float* __restrict__ db0, unsigned long long* dbg) {
   using L = CnnBwdSmem;
-  float* sdz = sm + L::DZ; float* swt = sm + L::WT; float* sx = sm + L::X; float* sa1 = sm + L::A1; float* sda1 = sm + L::DA1;
-  float* spart = sm + L::PART; int* spos = reinterpret_cast<int*>(sm + L::POS);
+  float* swt = sm + L::WT; float* sx = sm + L::X; float* sa1 = sm + L::A1; float* sda1 = sm + L::DA1;
+  int* spos = reinterpret_cast<int*>(sm + L::POS); float2* snz = reinterpret_cast<float2*>(sm + L::NZ);
+  int* snzsrc = reinterpret_cast<int*>(sm + L::NZSRC); int* snzcnt = reinterpret_cast<int*>(sm + L::NZCNT);
   const bool dbg_on = dbg != nullptr && b == 0 && cg == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
   stamp(8);
   const int tid = threadIdx.x;
-  for (int i = tid; i < CD_C2 * L::DZPL / 4; i += 288) reinterpret_cast<float4*>(sdz)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = tid; i < 4 * CD_C2 * 25; i += 288) {
-    // swt[(cl*32 + oc)*28 + t] = W1[oc][4cg+cl][4 - t/5][4 - t%5]   (t = flipped tap); source index runs over (oc, cl, tap) = 100 floats per oc
-    const int oc = i / 100, rem = i - oc * 100, cl = rem / 25, tap = rem - cl * 25;
-    cpa4(swt + (cl * CD_C2 + oc) * CD_W1PAD + (24 - tap), w1 + ((long long)oc * CD_C1 + 4 * cg) * 25 + rem);
+  // swt[((cp*32 + oc)*49 + r*7 + s)*2 + k] = W1[oc][4cg + 2cp + k][r-1][s-1] for r, s in 1..5, 0 on the border of the 7x7 plane.  The taps are
+  // copied in source order (100 contiguous floats per oc), so that a warp's loads are coalesced.
+  for (int i = tid; i < CD_C2 * 4 * 25; i += 288) {
+    const int oc = i / 100, rem = i - oc * 100, cl = rem / 25, tap = rem - cl * 25, r = tap / 5, t = tap - r * 5;
+    cpa4(swt + (((cl >> 1) * CD_C2 + oc) * 49 + (r + 1) * 7 + t + 1) * 2 + (cl & 1), w1 + ((long long)oc * CD_C1 + 4 * cg) * 25 + rem);
   }
-  for (int i = tid; i < 4 * CD_C2 * 3; i += 288) swt[(i / 3) * CD_W1PAD + 25 + i % 3] = 0.f;
+  for (int i = tid; i < 2 * CD_C2 * 24; i += 288) {          // the 24 border taps of every (cp, oc) plane: rows 0 and 6, then columns 0 and 6
+    const int plane = i / 24, j = i - plane * 24;
+    const int t7 = j < 7 ? j : j < 14 ? 42 + (j - 7) : j < 19 ? (j - 13) * 7 : (j - 18) * 7 + 6;
+    reinterpret_cast<float2*>(swt)[plane * 49 + t7] = make_float2(0.f, 0.f);
+  }
   for (int i = tid; i < CD_H * CD_H / 4; i += 288) cpa16(sx + 4 * i, x + (long long)b * CD_H * CD_H + 4 * i);
   for (int i = tid; i < 4 * 144 / 4; i += 288) cpa16(sa1 + 4 * i, a1 + ((long long)b * CD_C1 + 4 * cg) * 144 + 4 * i);
   for (int i = tid; i < 4 * 144; i += 288) {
     const long long o = ((long long)b * CD_C1 + 4 * cg) * 144 + i;
     const int win = i % 144, id = idx1[o];
     spos[i] = (2 * (win / CD_P1) + (id >> 1)) * CD_H + 2 * (win % CD_P1) + (id & 1);
+  }
+  // where dz2 can be non-zero (a2 > 0, at the arg-max idx2) is known from the forward pass: one warp per pooling window lists its output
+  // channels in ascending order, with the weight offset that places the arg-max pixel; only the values (da2) wait for the grid dependency
+  {
+    const int oc = tid & 31, wa = tid >> 5, wb = wa + 9;      // 9 warps: windows wa and wa + 9 (< 16); all loads issued before the first ballot
+    const long long oa = ((long long)b * CD_C2 + oc) * 16 + wa, ob = ((long long)b * CD_C2 + oc) * 16 + (wb < 16 ? wb : wa);
+    const float ava = a2[oa], avb = a2[ob];
+    const int ida = idx2[oa], idb = idx2[ob];
+    auto list = [&](int w, float av, int id) {
+      const unsigned m = __ballot_sync(0xffffffffu, av > 0.f);
+      if (av > 0.f) {
+        const int k = __popc(m & ((1u << oc) - 1u));
+        snz[w * 32 + k].y = __int_as_float(oc * 49 - ((id >> 1) * 7 + (id & 1)));
+        snzsrc[w * 32 + k] = oc * 16 + w;
+      }
+      if (oc == 0) snzcnt[w] = __popc(m);
+    };
+    list(wa, ava, ida);
+    if (wb < 16) list(wb, avb, idb);
   }
   cpa_wait_all();
   __syncthreads();
@@ -228,52 +263,42 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
   // dense-chain cluster leaves idle and finish their staging while it is still running.
   pdl_wait();
   pdl_launch();
-  // scatter the non-zeros of dz2 (pool + ReLU backward of conv1's output)
-  for (int e = tid; e < CD_C2 * 16; e += 288) {
-    const long long o = (long long)b * CD_C2 * 16 + e;
-    const int oc = e >> 4, win = e & 15, id = idx2[o];
-    const float gv = a2[o] > 0.f ? da2[o] : 0.f;
-    const int oh = 2 * (win >> 2) + (id >> 1), ow = 2 * (win & 3) + (id & 1);
-    sdz[oc * L::DZPL + (oh + 4) * L::DZLD + ow + 4] = gv;
-  }
+  // the non-zero values of dz2 (pool + ReLU backward of conv1's output)
+  for (int e = tid; e < 16 * 32; e += 288)
+    if ((e & 31) < snzcnt[e >> 5]) snz[e].x = da2[(long long)b * CD_C2 * 16 + snzsrc[e]];
   __syncthreads();
   stamp(10);
-  // ---- conv1 data gradient: thread -> oc quarter, channel pair, 2x2 output window of the 12x12 map
+  // ---- conv1 data gradient, routed through conv0's ReLU: thread -> channel pair cp, pixel (y, x) = (2py + qy, 2px + qx) of the 12x12 map
+  //   da1[c][y][x] = sum_{wh, ww} sum_{oc in list (wh, ww)} dz2 * W1[oc][c][y - oh][x - ow]   (windows and list entries in ascending order)
+  // a pixel whose a1 <= 0 gets no gradient (the ReLU routes it to 0), so its sum is skipped.  Pixels with the same (qy, qx) share a warp.
   {
-    const int ocq = tid / 72, t72 = tid % 72, cp = t72 / 36, win = t72 % 36, ph = win / 6, pw = win % 6;
-    float acc0[4] = {0.f, 0.f, 0.f, 0.f}, acc1[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-    for (int o8 = 0; o8 < 8; ++o8) {
-      const int oc = 8 * ocq + o8;
-      float pt[6][6], w[28];
-      load_patch(sdz + oc * L::DZPL + (2 * ph) * L::DZLD + 2 * pw, L::DZLD, pt);
-      load_w28(swt + ((2 * cp) * CD_C2 + oc) * CD_W1PAD, w);
-      window_fma(pt, w, acc0);
-      load_w28(swt + ((2 * cp + 1) * CD_C2 + oc) * CD_W1PAD, w);
-      window_fma(pt, w, acc1);
+    const int cp = tid / 144, p = tid - cp * 144, q = p / 36, r = p - q * 36, qy = q >> 1, qx = q & 1, py = r / 6, px = r - py * 6;
+    const int pix = (2 * py + qy) * CD_P1 + 2 * px + qx;
+    const float m0 = sa1[(2 * cp) * 144 + pix], m1 = sa1[(2 * cp + 1) * 144 + pix];
+    float acc0 = 0.f, acc1 = 0.f;
+    if (m0 > 0.f || m1 > 0.f) {
+      const float2* wcp = reinterpret_cast<const float2*>(swt) + cp * CD_C2 * 49;
+      for (int wh = max(py - 2, 0); wh <= min(py, 3); ++wh)
+        for (int ww = max(px - 2, 0); ww <= min(px, 3); ++ww) {
+          // 7x7 tap of the window's top-left pixel: (dy + 1, dx + 1) with dy = y - 2wh in 0..5; the entry's offset subtracts the arg-max shift
+          const float2* wp = wcp + (2 * (py - wh) + qy + 1) * 7 + 2 * (px - ww) + qx + 1;
+          const float2* nz = snz + (wh * 4 + ww) * 32;
+          const int n = snzcnt[wh * 4 + ww];
+#pragma unroll 4
+          for (int k = 0; k < n; ++k) {
+            const float2 e = nz[k];
+            const float2 wv = wp[__float_as_int(e.y)];
+            acc0 = fmaf(e.x, wv.x, acc0);
+            acc1 = fmaf(e.x, wv.y, acc1);
+          }
+        }
     }
-    float4* dst = reinterpret_cast<float4*>(spart + (ocq * 72 + t72) * 8);
-    dst[0] = make_float4(acc0[0], acc0[1], acc0[2], acc0[3]);
-    dst[1] = make_float4(acc1[0], acc1[1], acc1[2], acc1[3]);
+    sda1[(2 * cp) * 144 + pix] = m0 > 0.f ? acc0 : 0.f;
+    sda1[(2 * cp + 1) * 144 + pix] = m1 > 0.f ? acc1 : 0.f;
   }
   __syncthreads();
   stamp(11);
-  if (tid < 144) {
-    const int i72 = tid >> 1, which = tid & 1, cp = i72 / 36, win = i72 % 36, ph = win / 6, pw = win % 6, cl = 2 * cp + which;
-    float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 v = *reinterpret_cast<const float4*>(spart + (q * 72 + i72) * 8 + which * 4);
-      acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w;
-    }
-    // route through conv0's ReLU (+ pool: the value belongs to the arg-max pixel recorded in spos)
-    float* d = sda1 + cl * 144 + (2 * ph) * CD_P1 + 2 * pw;
-    const float* m = sa1 + cl * 144 + (2 * ph) * CD_P1 + 2 * pw;
-    d[0] = m[0] > 0.f ? acc[0] : 0.f; d[1] = m[1] > 0.f ? acc[1] : 0.f;
-    d[CD_P1] = m[CD_P1] > 0.f ? acc[2] : 0.f; d[CD_P1 + 1] = m[CD_P1 + 1] > 0.f ? acc[3] : 0.f;
-  }
-  __syncthreads();
-  stamp(12);
+  stamp(12);     // (the ReLU routing is part of the data-gradient phase)
   // ---- conv0 weight / bias gradient of this image (4 channels): dW0[ch][kh][kw] += sum_windows g * x[oh+kh][ow+kw]
   // 200 threads: (tap, channel) x 2 halves of the 144 windows; four independent accumulators break the FMA dependency chain
   if (tid < 200) {
@@ -370,8 +395,11 @@ __global__ void __launch_bounds__(256) cnn_wgrad1_kernel(const float* a1, const 
   extern __shared__ __align__(16) float sm[];
   cnn_wgrad1_body(sm, blockIdx.x, blockIdx.y, a1, a2, idx2, da2, dw1, db1, B, dbg);
 }
-// The whole convolution backward pass as ONE launch: CTAs [0, 4B) run the data-gradient / conv0 body, CTAs [4B, 4B + 128) the conv1
-// weight-gradient body (two independent jobs that read the same inputs; a single heterogeneous grid saves a stream fork / join in the step graph).
+// The whole convolution backward pass as ONE launch: CTAs [0, 128) run the conv1 weight-gradient body, CTAs [128, 128 + 4B) the data-gradient /
+// conv0 body (two independent jobs that read the same inputs; a single heterogeneous grid saves a stream fork / join in the step graph).
+// The weight-gradient CTAs come first: CTAs are dispatched in index order and, while the dense-chain cluster runs, only part of the grid
+// becomes resident; the weight-gradient body is the longer one after its grid dependency resolves, so it is the one that should be resident
+// and staged by then.
 __global__ void __launch_bounds__(288) cnn_bwd_all_kernel(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2,
                                                            const unsigned char* idx2, const float* da2, float* dw0, float* db0, float* dw1, float* db1,
                                                            int B, unsigned long long* dbg) {
@@ -380,11 +408,11 @@ __global__ void __launch_bounds__(288) cnn_bwd_all_kernel(const float* x, const 
   // debug: every CTA records (start, end, SM id) at dbg[64 + 3 i ..] so that tools/step_timeline.py can show how the grid packs onto the SMs
   unsigned long long t0 = 0;
   if (dbg != nullptr && threadIdx.x == 0) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t0));
-  if (i < 4 * B) {
-    cnn_bwd_body(sm, i >> 2, i & 3, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dbg);
+  if (i >= 4 * CD_C2) {
+    const int j = i - 4 * CD_C2;
+    cnn_bwd_body(sm, j >> 2, j & 3, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dbg);
   } else if (threadIdx.x < 256) {            // (no thread of this CTA takes the other branch, so its __syncthreads pair up among these 256)
-    const int j = i - 4 * B;
-    cnn_wgrad1_body(sm, j >> 2, j & 3, a1, a2, idx2, da2, dw1, db1, B, dbg);
+    cnn_wgrad1_body(sm, i >> 2, i & 3, a1, a2, idx2, da2, dw1, db1, B, dbg);
   }
   if (dbg != nullptr && threadIdx.x == 0) {
     unsigned long long t1; unsigned smid;
@@ -395,7 +423,8 @@ __global__ void __launch_bounds__(288) cnn_bwd_all_kernel(const float* x, const 
 }
 
 // The convolution backward pass AND the exchange of the four conv keys (push -> both server tiers -> optimizer -> pull, the replicated one-hop
-// mode of hips_fabric.cu's direct protocol) as ONE launch.  Grid and bodies are those of cnn_bwd_all_kernel.  Every CTA takes a ticket when its
+// mode of hips_fabric.cu's direct protocol) as ONE launch.  The bodies of cnn_bwd_all_kernel: CTAs [0, 4B) data gradient, [4B, 4B+128) conv1
+// weight gradient.  Every CTA takes a ticket when its
 // gradients are written; the CTAs that draw the last `n_active` tickets wait until the ticket counter shows that the whole grid has finished
 // and then each serve one 1024-float tile of the conv keys: gradient -> LL packets into every rank's slot, poll the packets of all ranks, sum
 // in the hierarchy's order (party sums, push_scale, sum over parties), optimizer on this rank's replica of the server state, fresh weights

@@ -19,6 +19,12 @@ import geomx_b200 as mx  # noqa: E402
 from geomx_b200.ops import native  # noqa: E402
 from geomx_b200.parallel import Topology  # noqa: E402
 
+# in-kernel %globaltimer stamps of the direct-convolution kernels (gx_cnn_set_debug slots, written by the first CTA of each body)
+CNN_PHASES = {"cnn_fwd": (0, 1, 2, 3, 4), "cnn_bwd": (8, 9, 10, 11, 12, 13), "cnn_wgrad1": (16, 17, 18)}
+CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
+                    "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
+                    "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
+
 
 def main():
     world, rank, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0))
@@ -66,6 +72,7 @@ def main():
             per = [(c[64 + 3 * i], c[65 + 3 * i], c[66 + 3 * i]) for i in range(256)]
             row["_cta"] = per
         row["_ms"] = ev[0].elapsed_time(ev[1])
+        row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in CNN_PHASES.items()}
         row["_ph"] = {k: [(v - st[k][0]) / 1e3 for v in st[k][:6]] for k in chans if st[k][0] > 0}
         rows.append(row)
     rows = rows[4:]
@@ -80,7 +87,7 @@ def main():
         # how the 256 CTAs of the convolution-backward grid pack onto the SMs (last sampled step)
         r = rows[-1]
         base = min(v[0] for kk, v in r.items() if not kk.startswith("_") and v[0] > 0)
-        for name, lo, hi in (("bwd CTAs  (0..127)", 0, 128), ("wgrad CTAs (128..255)", 128, 256)):
+        for name, lo, hi in (("wgrad CTAs (0..127)", 0, 128), ("bwd CTAs  (128..255)", 128, 256)):
             st = sorted((a - base) / 1e3 for a, b, sm_ in r["_cta"][lo:hi]); en = sorted((b - base) / 1e3 for a, b, sm_ in r["_cta"][lo:hi])
             du = sorted((b - a) / 1e3 for a, b, sm_ in r["_cta"][lo:hi])
             lines.append("  %-22s start min/med/max %.2f %.2f %.2f | end %.2f %.2f %.2f | duration %.2f %.2f %.2f" % (
@@ -93,9 +100,12 @@ def main():
         pair = {"bwd+bwd": 0, "bwd+wgrad": 0, "wgrad+wgrad": 0}
         for v in sms.values():
             if len(v) == 2:
-                k = sum(1 for i in v if i >= 128)
+                k = sum(1 for i in v if i < 128)
                 pair[["bwd+bwd", "bwd+wgrad", "wgrad+wgrad"][k]] += 1
         lines.append("  SM sharing: %s" % pair)
+    for name, labels in CNN_PHASE_LABELS.items():
+        lines.append("  %s phases of CTA 0 (us): %s" % (name, "  ".join("%s %.2f" % (lab, statistics.median(r["_cnn_ph"][name][i] for r in rows))
+                                                                      for i, lab in enumerate(labels))))
     if "_tail" in rows[0]:
         lines.append("  bwd tail (us since first tail ticket): ticket|grid done|sent|received|end %s" % ["%.2f" % statistics.median(r["_tail"][i] for r in rows) for i in range(5)])
     for k in rows[0]["_ph"]:
