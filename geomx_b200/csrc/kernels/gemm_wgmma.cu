@@ -455,12 +455,15 @@ GX_API int gx_gemm_get_precision() { return gemm_precision(); }
 GX_API int gx_gemm_set_debug(unsigned long long* p) { g_gemm_dbg = p; return 0; }
 
 // A: K-major -> [M][K] with row stride lda; MN-major -> [K][M] with row stride lda.  Same for B with N.
-// returns 0 on success, -1 if the operands do not satisfy TMA alignment (caller falls back to gx_gemm_simt).
+// returns 0 on success, -1 if the operands do not satisfy TMA alignment (caller falls back to gx_gemm_simt), -2 for a ReLU epilogue with
+// split_k > 1: every split applies the epilogue to its partial sum before the atomic add, which is right for the bias (split 0 only), the
+// mask and the column sum (linear), but would give sum(relu(partial)) instead of relu(sum).
 static int gemm_tf32_impl(const float* A, long long lda, int a_mn, const float* B, long long ldb, int b_mn, int M, int N, int K, float* D,
                           long long ldd, const float* bias, const float* mask, long long ldmask, float* colsum, int relu, int accumulate,
                           int store_mode, int hw, float alpha, int split_k,
                           int pool_w, unsigned char* pool_idx, cudaStream_t stream) {
   using namespace gx;
+  if (relu && split_k > 1) return -2;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if (store_mode == 2) {   // fused pooling: whole windows must live inside one warp's 32 rows, no split-K / accumulate
     if (pool_w < 2 || (pool_w & 1) || (32 % (2 * pool_w)) != 0 || hw % 32 != 0 || (hw % pool_w) != 0 || ((hw / pool_w) & 1) || M % 32 != 0 ||

@@ -48,7 +48,9 @@ def gemm_precision():
 
 def gemm(A, B, D, a_mn=False, b_mn=False, bias=None, mask=None, colsum=None, relu=False, accumulate=False,
          store_nchw_hw=0, alpha=1.0, split_k=1, M=None, N=None, K=None, lda=None, ldb=None, ldd=None, force_simt=False):
-    """D[M,N] = epi(alpha * A·Bᵀ).  A is [M,K] (K-major) or [K,M] (MN-major, ``a_mn``); B is [N,K] or [K,N] (``b_mn``)."""
+    """D[M,N] = epi(alpha * A·Bᵀ).  A is [M,K] (K-major) or [K,M] (MN-major, ``a_mn``); B is [N,K] or [K,N] (``b_mn``).
+    ``split_k > 1`` adds the partial products of K slices into D (so D must hold zeros, or the value to accumulate onto); it cannot be
+    combined with ``relu`` (raises RuntimeError)."""
     if M is None:
         M = A.shape[1] if a_mn else A.shape[0]
     if K is None:
