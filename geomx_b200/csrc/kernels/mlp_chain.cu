@@ -11,12 +11,14 @@
 //     so the 150 KB of weight traffic overlaps the tail of the convolution kernels) and reused by forward and backward;
 //   * products run on the fp32 FMA pipes (exact fp32, like the reference's SGEMM): 4x4 register tiles, K split over warps, operands read with
 //     conflict-free 128-bit shared loads from XOR-swizzled tiles, partial sums reduced through shared memory;
-//   * layer outputs are broadcast to all CTAs of the cluster with distributed-shared-memory stores (st.shared::cluster through
-//     cluster.map_shared_rank) followed by one hardware cluster barrier — no global round trip between layers;
+//   * layer outputs (a3, a4, dz4, dz3) are pushed to every CTA of the cluster with st.async into distributed shared memory; each store
+//     completes its bytes on a transaction mbarrier in the receiving CTA, and a consumer waits on its own barrier only.  Each receive buffer
+//     is written once per launch, so after start-up there is no cluster-wide barrier (and no GPU-scope fence, no L1 invalidation) between
+//     layers: a CTA starts a layer as soon as its own inputs have landed;
 //   * epilogues fused: bias, ReLU, ReLU masks of the backward pass, softmax / loss / dlogits, bias gradients (column sums).
 //   * 512 threads: the two warp-groups split K in the wide forward layer and run data-gradient and weight-gradient products side by side
 //     in the backward phases.
-// A handful of cluster barriers replace what used to be seven kernel launches (dense0, dense1, head, dW1, dz3, dW0, da2); tools/kernel_times.py
+// One cluster launch replaces what used to be seven kernel launches (dense0, dense1, head, dW1, dz3, dW0, da2); tools/kernel_times.py
 // times the whole chain with per-phase %globaltimer stamps.
 //
 // Shapes are compile-time (D0 -> D1 -> D2 -> C<=16, batch <= 32): the demo CNN's 512 -> 256 -> 128 -> 10.  Other shapes use the wgmma GEMMs.
@@ -57,6 +59,38 @@ __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---- point-to-point hand-offs between the CTAs of the cluster
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, int rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(local_smem_addr), "r"(rank));
+  return a;
+}
+// push v to float offset o of `buf` in the N CTAs of the cluster that follow rank cr (N = CS: every CTA including this one, this one last;
+// N = CS - 1: the peers only), so that the CTAs do not all hit rank 0 first; each store completes 16 bytes on the receiver's barrier `bar`
+template <int CS, int N = CS>
+__device__ __forceinline__ void push_all(const float* buf, int o, uint64_t* bar, int cr, float4 v) {
+  const uint32_t a = smem_u32(buf + o), m = smem_u32(bar);
+#pragma unroll 4   // a full unroll hoists all 2 N remote addresses and pushes the kernel past 96 registers (co-residency with cnn_fwd)
+  for (int i = 0; i < N; ++i) {
+    const int r = (cr + 1 + i) & (CS - 1);
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];"
+                 ::"r"(mapa_u32(a, r)), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(mapa_u32(m, r)) : "memory");
+  }
+}
+// wait until every byte announced on this CTA's (single-use) barrier has landed.  The acquire that makes the peers' stores visible is
+// restricted to shared::cluster memory: a plain acquire.cluster wait would also invalidate L1 after every layer, for no data the kernel
+// reads through it.
+__device__ __forceinline__ void wait_landed(uint64_t* bar) {
+  asm volatile(
+      "{\n\t.reg .pred P1;\n\t"
+      "WAIT_LANDED:\n\t"
+      "mbarrier.try_wait.parity.relaxed.cluster.shared::cta.b64 P1, [%0], 0;\n\t"
+      "@!P1 bra WAIT_LANDED;\n\t}\n"
+      "fence.acquire.sync_restrict::shared::cluster.cluster;" ::"r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // stage `rows` x K floats (global row stride ld) into a swizzled K-major tile
 __device__ __forceinline__ void stage_swizzled_async(float* dst, const float* src, int rows, int K, long long ld) {
@@ -174,13 +208,18 @@ struct MlpSmem {
   static constexpr int W0_SZ = (NS1 * D0 > D1 * KS0) ? NS1 * D0 : D1 * KS0;
   static constexpr int W1 = W0 + W0_SZ;                        // fwd: [NS2][D1] swizzled;  bwd: [D2][NS1] plain
   static constexpr int W1_SZ = (NS2 * D1 > D2 * NS1) ? NS2 * D1 : D2 * NS1;
+  // receive buffers: each is written by the peers exactly once per launch.  a3 is dead after this CTA's P2 products, which precede its a4
+  // push; no peer can produce dz3 before it has this CTA's a4 (and dz4), so dz3 lands in the same buffer without a write-after-read barrier
   static constexpr int A3 = W1 + W1_SZ;                        // [32][D1] swizzled  (later: dz3)
-  static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled  (later: scratch)
-  static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled  (earlier: scratch)
+  static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled  (earlier: P1 scratch; later: P4 / P5 scratch)
+  static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled  (earlier: P1 / P2 scratch)
   static constexpr int W2 = DZ4 + MC_B * D2;                   // [16][D2] plain
   static constexpr int DL = W2 + MC_CMAX * D2;                 // [32][16] dlogits
   static constexpr int MISC = DL + MC_B * MC_CMAX;             // b0 slice [NS1] | b1 slice [NS2] | b2 [16] | label [32]
-  static constexpr int TOTAL = MISC + NS1 + NS2 + 16 + 32;
+  static constexpr int A3OWN = MISC + NS1 + NS2 + 16 + 32;     // [32][NS1] plain: this CTA's a3 columns (ReLU mask of dz3, dW1)
+  static constexpr int A4OWN = A3OWN + MC_B * NS1;             // [32][NS2] plain: this CTA's a4 columns (ReLU mask of dz4, dW2)
+  static constexpr int BAR = A4OWN + MC_B * NS2;               // 4 mbarriers: a3, a4, dz4, dz3 landed
+  static constexpr int TOTAL = BAR + 4 * 2;
   static constexpr int BYTES = TOTAL * 4;
 };
 
@@ -189,15 +228,19 @@ template <int D0, int D1, int D2, int CS>
 __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_kernel(const MlpChainParams p) {
   using L = MlpSmem<D0, D1, D2, CS>;
   constexpr int NS1 = L::NS1, NS2 = L::NS2, KS0 = L::KS0;
-  constexpr int MC_CLUSTER = CS;
+  static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
   static_assert(D0 % 64 == 0 && D1 % 64 == 0 && D2 % 64 == 0, "layer widths must be multiples of 64");
   static_assert(NS1 % 8 == 0 && NS2 % 4 == 0 && KS0 % 4 == 0, "slices must hold whole register tiles");
   static_assert(MC_THREADS % (2 * NS1) == 0 && MC_HALF % (2 * NS2) == 0 && MC_HALF % (2 * NS1) == 0 && MC_HALF % (2 * KS0) == 0, "K splits");
   static_assert(MC_THREADS / (2 * NS1) * MC_B * NS1 <= 2 * MC_B * D2 && MC_HALF / (2 * KS0) * MC_B * KS0 <= MC_B * D2, "scratch sizes");
+  static_assert(MC_HALF % (NS1 / 4) == 0 && D2 % (MC_HALF / (NS1 / 4)) == 0, "dW1 tiles");
+  static_assert(L::BAR % 2 == 0, "mbarriers are 8-byte aligned");
   extern __shared__ __align__(16) float sm[];
   float* sX = sm + L::X; float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
-  float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL;
+  float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL; float* sA3own = sm + L::A3OWN; float* sA4own = sm + L::A4OWN;
   float* sB0 = sm + L::MISC; float* sB1 = sB0 + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + L::BAR);
+  uint64_t* bar_a3 = bar; uint64_t* bar_a4 = bar + 1; uint64_t* bar_dz4 = bar + 2; uint64_t* bar_dz3 = bar + 3;
   cg::cluster_group cluster = cg::this_cluster();
   const int cr = (int)cluster.block_rank();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -205,6 +248,18 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   const bool dbg_on = p.dbg != nullptr && cr == 0 && tid == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; } };
   stamp(0);
+
+  // ---------------- start-up: each receive barrier expects its whole buffer (dz3: all but this CTA's own columns, which are stored locally).
+  // The peers push into this CTA's shared memory only after the cluster barrier below, so the barriers are armed before any byte arrives.
+  if (tid == 0) {
+    for (int i = 0; i < 4; ++i) mbar_init(bar + i, 1);
+    mbar_arrive_expect_tx(bar_a3, MC_B * D1 * 4);
+    mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
+    mbar_arrive_expect_tx(bar_dz4, MC_B * D2 * 4);
+    mbar_arrive_expect_tx(bar_dz3, (CS - 1) * MC_B * NS1 * 4);
+    fence_barrier_init();      // (the release the peers need: nothing else this CTA wrote so far is read by them)
+  }
+  asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");   // waited for once the inputs are staged: the loads overlap the rendezvous
 
   // ---------------- prologue: weights do not depend on the preceding kernel (they were written by the previous step's exchange, which a
   // kernel further up the stream has already waited for) -> stage them before griddepcontrol.wait
@@ -233,7 +288,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  cluster.sync();      // every CTA of the cluster is running (DSMEM stores below need the target CTA's shared memory to exist)
+  cluster.barrier_wait();   // every CTA of the cluster is running with its barriers armed (the pushes below target its shared memory)
   stamp(3);
 
   // tile coordinates shared by the 32-row products: 8 row groups x (NC/4) column groups per K split
@@ -258,24 +313,24 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       v.x = fmaxf(v.x + sB0[4 * n4], 0.f); v.y = fmaxf(v.y + sB0[4 * n4 + 1], 0.f);
       v.z = fmaxf(v.z + sB0[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB0[4 * n4 + 3], 0.f);
       if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
-      const int o = sw_off(b, cr * NS1 + 4 * n4, D1);
-#pragma unroll
-      for (int r = 0; r < MC_CLUSTER; ++r) *reinterpret_cast<float4*>(cluster.map_shared_rank(sA3, r) + o) = v;
+      *reinterpret_cast<float4*>(sA3own + b * NS1 + 4 * n4) = v;
+      // the pushed value depends on this thread's scratch reads, so no peer can write a4 into the scratch before they are done
+      push_all<CS>(sA3, sw_off(b, cr * NS1 + 4 * n4, D1), bar_a3, cr, v);
     }
     stamp(13);
   }
-  cluster.sync();
-  stamp(4);
   // ---------------- P2: a4[:, slice] = relu(a3 * W1[slice]^T + b1)         NC = 16, K = D1, KS = 8
   {
     constexpr int PER = 2 * NS2, KS = MC_HALF / PER;     // this layer is small: warp-group 0 only
     if (tid < MC_HALF) {
+      wait_landed(bar_a3);
+      stamp(4);
       const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
       float acc[4][4] = {};
       prod_nt<D1, KS>(sA3, sW1, tb, tn, ks, acc);
       put_partial<NS2>(sDZ4, tb, tn, ks, acc);
     }
-    __syncthreads();
+    __syncthreads();     // from here on the full a3 buffer is dead: it receives dz3
     stage_plain_async(sW1, p.w1 + cr * NS1, D2, NS1, D1);   // W1[:, slice of D1] for dz3
     cp_async_commit();
     if (tid < MC_B * NS2 / 4) {
@@ -284,15 +339,14 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       v.x = fmaxf(v.x + sB1[4 * n4], 0.f); v.y = fmaxf(v.y + sB1[4 * n4 + 1], 0.f);
       v.z = fmaxf(v.z + sB1[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB1[4 * n4 + 3], 0.f);
       if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
-      const int o = sw_off(b, cr * NS2 + 4 * n4, D2);
-#pragma unroll
-      for (int r = 0; r < MC_CLUSTER; ++r) *reinterpret_cast<float4*>(cluster.map_shared_rank(sA4, r) + o) = v;
+      *reinterpret_cast<float4*>(sA4own + b * NS2 + 4 * n4) = v;
+      push_all<CS>(sA4, sw_off(b, cr * NS2 + 4 * n4, D2), bar_a4, cr, v);
     }
   }
-  cluster.sync();
-  stamp(5);
   // ---------------- P3: classifier + softmax-CE (every CTA redundantly: 32 x C logits), dz4 slice, dW2 slice, db2
   {
+    wait_landed(bar_a4);
+    stamp(5);
     for (int b = warp; b < MC_B; b += MC_THREADS / 32) {
       // all class dot products of this row at once: 16 independent partial sums per lane, then one butterfly over the whole vector
       // (a shuffle reduction per class would be a chain of 5 dependent ~25-cycle shuffles, ten times over)
@@ -324,37 +378,46 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
         if (p.logits != nullptr && lane < C) p.logits[(long long)b * C + lane] = mylogit;
       }
     }
-    __syncthreads();
-    // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m]   for m in this CTA's slice of D2; broadcast to the cluster
-    for (int e = tid; e < MC_B * NS2; e += MC_THREADS) {
-      const int b = e / NS2, m = cr * NS2 + e % NS2;
-      float s = 0.f;
-      for (int c = 0; c < C; ++c) s = fmaf(sDL[b * MC_CMAX + c], sW2[c * D2 + m], s);
-      const int o = sw_off(b, m, D2);
-      if (!(sA4[o] > 0.f)) s = 0.f;
-#pragma unroll
-      for (int r = 0; r < MC_CLUSTER; ++r) cluster.map_shared_rank(sDZ4, r)[o] = s;
-    }
-    // dW2[c][m] = sum_b dl[b][c] * a4[b][m] (this CTA's m slice), db2 (CTA 0)
-    for (int e = tid; e < C * NS2; e += MC_THREADS) {
-      const int c = e / NS2, m = cr * NS2 + e % NS2;
-      float s = 0.f;
-      for (int b = 0; b < MC_B; ++b) s = fmaf(sDL[b * MC_CMAX + c], sA4[sw_off(b, m, D2)], s);
-      p.dw2[(long long)c * D2 + m] = s;
-    }
-    if (cr == 0 && tid < C) {
-      float s = 0.f;
-      for (int b = 0; b < MC_B; ++b) s += sDL[b * MC_CMAX + tid];
-      p.db2[tid] = s;
+    cp_async_wait<0>();          // W1 column slice (and W0 column slice) landed
+    __syncthreads();             // dlogits complete, the staged slices visible; the full a4 buffer is dead from here on (P4 / P5 scratch)
+    if (tid < MC_HALF) {
+      // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m]   for m in this CTA's slice of D2, four columns per thread; pushed to the cluster
+      for (int e = tid; e < MC_B * NS2 / 4; e += MC_HALF) {
+        const int b = e / (NS2 / 4), m4 = 4 * (e % (NS2 / 4)), m = cr * NS2 + m4;
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int c = 0; c < C; ++c) {
+          const float d = sDL[b * MC_CMAX + c];
+          const float4 w = *reinterpret_cast<const float4*>(sW2 + c * D2 + m);
+          s.x = fmaf(d, w.x, s.x); s.y = fmaf(d, w.y, s.y); s.z = fmaf(d, w.z, s.z); s.w = fmaf(d, w.w, s.w);
+        }
+        const float4 a = *reinterpret_cast<const float4*>(sA4own + b * NS2 + m4);
+        if (!(a.x > 0.f)) s.x = 0.f;
+        if (!(a.y > 0.f)) s.y = 0.f;
+        if (!(a.z > 0.f)) s.z = 0.f;
+        if (!(a.w > 0.f)) s.w = 0.f;
+        push_all<CS>(sDZ4, sw_off(b, m, D2), bar_dz4, cr, s);
+      }
+    } else {
+      // warp-group 1, off the critical path: dW2[c][m] = sum_b dl[b][c] * a4[b][m] (this CTA's m slice), db2 (CTA 0)
+      const int t = tid - MC_HALF;
+      for (int e = t; e < C * NS2; e += MC_HALF) {
+        const int c = e / NS2, m = e % NS2;
+        float s = 0.f;
+        for (int b = 0; b < MC_B; ++b) s = fmaf(sDL[b * MC_CMAX + c], sA4own[b * NS2 + m], s);
+        p.dw2[(long long)c * D2 + cr * NS2 + m] = s;
+      }
+      if (cr == 0 && t < C) {
+        float s = 0.f;
+        for (int b = 0; b < MC_B; ++b) s += sDL[b * MC_CMAX + t];
+        p.db2[t] = s;
+      }
     }
   }
-  cluster.sync();
-  stamp(6);
-  // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice]);  dW1[slice of D2 rows] = dz4[:, rows]^T * a3;  db1
-  float4 dz3v;   // this thread's float4 of the dz3 slice (kept in registers across the barrier that protects a3)
+  // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice]);  dW1[:, slice of D1 columns] = dz4^T * a3[:, slice];  db1
+  float* sDZ3 = sA3;
   {
-    cp_async_wait<0>();          // W1 column slice (and W0 column slice) landed
-    __syncthreads();
+    wait_landed(bar_dz4);
+    stamp(6);
     if (tid < MC_HALF) {
       // warp-group 0: the data gradient dz3 (critical path)
       constexpr int PER = 2 * NS1, KS = MC_HALF / PER;   // K = D2
@@ -365,17 +428,35 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       named_bar_sync(1, MC_HALF);
       if (tid < MC_B * NS1 / 4) {
         const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);
-        dz3v = sum_partials<NS1, KS>(sA4, b, n4);
-        const float4 a3 = *reinterpret_cast<const float4*>(sA3 + sw_off(b, cr * NS1 + 4 * n4, D1));
+        float4 dz3v = sum_partials<NS1, KS>(sA4, b, n4);
+        const float4 a3 = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * n4);
         dz3v.x = a3.x > 0.f ? dz3v.x : 0.f; dz3v.y = a3.y > 0.f ? dz3v.y : 0.f; dz3v.z = a3.z > 0.f ? dz3v.z : 0.f; dz3v.w = a3.w > 0.f ? dz3v.w : 0.f;
+        const int o = sw_off(b, cr * NS1 + 4 * n4, D1);
+        push_all<CS, CS - 1>(sDZ3, o, bar_dz3, cr, dz3v);
+        *reinterpret_cast<float4*>(sDZ3 + o) = dz3v;   // own columns: stored locally (warp-group 1 reads them without waiting for the peers)
       }
+      named_bar_arrive(2, MC_THREADS);                   // own dz3 columns stored -> warp-group 1 may start dW0
+      stamp(7);
     } else {
-      // warp-group 1, concurrently: dW1 rows [cr*NS2, +NS2) as 4 x 4 tiles (4 x D1/4 = 256 of them) and the db1 slice
-      const int t = tid - MC_HALF;
-      if (t < (NS2 / 4) * (D1 / 4)) {
-        const int tnw = t / (D1 / 4), tk = t % (D1 / 4);
-        wgrad_tile<D2, D1, 4>(sDZ4, sA3, cr * NS2, 4 * tnw, tk, p.dw1 + (long long)cr * NS2 * D1);
+      // warp-group 1, concurrently: dW1 columns [cr*NS1, +NS1) of all D2 rows as TN x 4 tiles, and the db1 slice
+      constexpr int CG = NS1 / 4, TN = D2 / (MC_HALF / CG);
+      const int t = tid - MC_HALF, tk = t % CG, n0 = (t / CG) * TN;
+      float acc[TN][4];
+#pragma unroll
+      for (int i = 0; i < TN; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
+#pragma unroll 4
+      for (int b = 0; b < MC_B; ++b) {
+        const float4 a = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * tk);
+#pragma unroll
+        for (int i = 0; i < TN; ++i) {
+          const float d = sDZ4[sw_off(b, n0 + i, D2)];
+          acc[i][0] = fmaf(d, a.x, acc[i][0]); acc[i][1] = fmaf(d, a.y, acc[i][1]);
+          acc[i][2] = fmaf(d, a.z, acc[i][2]); acc[i][3] = fmaf(d, a.w, acc[i][3]);
+        }
       }
+#pragma unroll
+      for (int i = 0; i < TN; ++i)
+        *reinterpret_cast<float4*>(p.dw1 + (long long)(n0 + i) * D1 + cr * NS1 + 4 * tk) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
       if (t < NS2) {
         float s = 0.f;
         for (int bb = 0; bb < MC_B; ++bb) s += sDZ4[sw_off(bb, cr * NS2 + t, D2)];
@@ -383,34 +464,28 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       }
     }
   }
-  stamp(7);
-  cluster.sync();      // everybody is done reading a3 -> its buffer becomes dz3
-  if (tid < MC_B * NS1 / 4) {
-    const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);
-    const int o = sw_off(b, cr * NS1 + 4 * n4, D1);
-#pragma unroll
-    for (int r = 0; r < MC_CLUSTER; ++r) *reinterpret_cast<float4*>(cluster.map_shared_rank(sA3, r) + o) = dz3v;
-  }
-  cluster.sync();
-  stamp(8);
   // ---------------- P5: dx[:, slice of D0] = dz3 * W0[:, slice];  dW0[slice of D1 rows] = dz3[:, rows]^T * x;  db0
   {
-    float* sDZ3 = sA3;
     if (tid < MC_HALF) {
       // warp-group 0: the input gradient (what the convolution backward pass is waiting for)
       constexpr int PER = 2 * KS0, KS = MC_HALF / PER;   // K = D1
+      named_bar_sync(1, MC_HALF);                        // own dz3 columns stored, P4 scratch read
+      wait_landed(bar_dz3);                              // the peers' columns
+      stamp(8);
       const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
       float acc[4][4] = {};
       prod_nn<D1, KS0, KS>(sDZ3, sW0, tb, tn, ks, acc);
       stamp(14);
-      put_partial<KS0>(sDZ4, tb, tn, ks, acc);          // scratch = dz4 buffer (dead after P4): KS x 32 x KS0 floats = 16 KB
+      put_partial<KS0>(sA4, tb, tn, ks, acc);           // scratch = a4 buffer again (warp-group 0 only): KS x 32 x KS0 floats = 16 KB
       named_bar_sync(1, MC_HALF);
       for (int e = tid; e < MC_B * KS0 / 4; e += MC_HALF) {
         const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
-        if (b < B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(sDZ4, b, n4);
+        if (b < B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(sA4, b, n4);
       }
     } else {
-      // warp-group 1, concurrently: dW0 rows [cr*NS1, +NS1) as 8 x 4 tiles (4 x D0/4 = 512 tiles, two per thread) and the db0 slice
+      // warp-group 1, concurrently: dW0 rows [cr*NS1, +NS1) as 8 x 4 tiles (4 x D0/4 = 512 tiles, two per thread) and the db0 slice.
+      // It needs only this CTA's own dz3 columns, so it does not wait for the peers.
+      named_bar_sync(2, MC_THREADS);
       const int t0 = tid - MC_HALF;
       for (int t = t0; t < (NS1 / 8) * (D0 / 4); t += MC_HALF) {
         const int tnw = t / (D0 / 4), tk = t % (D0 / 4);

@@ -47,8 +47,9 @@ if eng.fused_mlp:
     for rep in range(3):
         eng._body(); torch.cuda.synchronize()
         st = dbg.cpu().tolist()
-        print("mlp chain phases (us since kernel start): 0 start|1 prologue issued|2 pdl wait done|3 inputs landed+sync|4 P1|5 P2|6 P3|7 P4 compute|8 dz3 bcast|9 end:",
-              ["%.2f" % ((v - st[0]) / 1e3) for v in st[:10]], "| P1: 10 products done|11 partials synced|12 W0 prefetch issued|13 a3 broadcast:",
+        print("mlp chain phases (us since kernel start): 0 start|1 prologue issued|2 pdl wait done|3 inputs landed+sync|4 a3 landed|5 a4 landed|"
+              "6 dz4 landed|7 dz3 pushed|8 dz3 landed|9 end:",
+              ["%.2f" % ((v - st[0]) / 1e3) for v in st[:10]], "| P1: 10 products done|11 partials synced|12 W0 prefetch issued|13 a3 pushed:",
               ["%.2f" % ((v - st[0]) / 1e3) for v in st[10:14]], "| P5: 14 da2 products done:", "%.2f" % ((st[14] - st[0]) / 1e3))
     lib.gx_mlp_chain_set_debug(ctypes.c_void_p(0))
 if eng.direct_conv:

@@ -24,6 +24,9 @@ CNN_PHASES = {"cnn_fwd": (0, 1, 2, 3, 4), "cnn_bwd": (8, 9, 10, 11, 12, 13), "cn
 CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
                     "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
                     "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
+# the same for the dense-chain cluster kernel (gx_mlp_chain_set_debug slots of cluster CTA 0); each phase ends when its input has landed
+MLP_PHASES = (0, 3, 4, 5, 6, 7, 8, 9)
+MLP_PHASE_LABELS = ("staging+pdl-wait", "dense0 -> a3", "dense1 -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
 
 
 def main():
@@ -73,6 +76,7 @@ def main():
             row["_cta"] = per
         row["_ms"] = ev[0].elapsed_time(ev[1])
         row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in CNN_PHASES.items()}
+        row["_mlp_ph"] = [(m[s1] - m[s0]) / 1e3 for s0, s1 in zip(MLP_PHASES, MLP_PHASES[1:])]
         row["_ph"] = {k: [(v - st[k][0]) / 1e3 for v in st[k][:6]] for k in chans if st[k][0] > 0}
         rows.append(row)
     rows = rows[4:]
@@ -106,6 +110,8 @@ def main():
     for name, labels in CNN_PHASE_LABELS.items():
         lines.append("  %s phases of CTA 0 (us): %s" % (name, "  ".join("%s %.2f" % (lab, statistics.median(r["_cnn_ph"][name][i] for r in rows))
                                                                       for i, lab in enumerate(labels))))
+    lines.append("  mlp_chain phases of CTA 0 (us): %s" % "  ".join("%s %.2f" % (lab, statistics.median(r["_mlp_ph"][i] for r in rows))
+                                                                    for i, lab in enumerate(MLP_PHASE_LABELS)))
     if "_tail" in rows[0]:
         lines.append("  bwd tail (us since first tail ticket): ticket|grid done|sent|received|end %s" % ["%.2f" % statistics.median(r["_tail"][i] for r in rows) for i in range(5)])
     for k in rows[0]["_ph"]:
