@@ -11,10 +11,11 @@
 //     so the 150 KB of weight traffic overlaps the tail of the convolution kernels) and reused by forward and backward;
 //   * products run on the fp32 FMA pipes (exact fp32, like the reference's SGEMM): 4x4 register tiles, K split over warps, operands read with
 //     conflict-free 128-bit shared loads from XOR-swizzled tiles, partial sums reduced through shared memory;
-//   * layer outputs (a3, a4, dz4, dz3) are pushed to every CTA of the cluster with st.async into distributed shared memory; each store
+//   * layer outputs (a3, a4, dz3) are pushed to every CTA of the cluster with st.async into distributed shared memory; each store
 //     completes its bytes on a transaction mbarrier in the receiving CTA, and a consumer waits on its own barrier only.  Each receive buffer
 //     is written once per launch, so after start-up there is no cluster-wide barrier (and no GPU-scope fence, no L1 invalidation) between
-//     layers: a CTA starts a layer as soon as its own inputs have landed;
+//     layers: a CTA starts a layer as soon as its own inputs have landed.  dz4 is not handed off: once a4 has landed every CTA holds all
+//     of its inputs (a4, W2, dlogits) and computes the whole of it;
 //   * epilogues fused: bias, ReLU, ReLU masks of the backward pass, softmax / loss / dlogits, bias gradients (column sums).
 //   * 512 threads: the two warp-groups split K in the wide forward layer and run data-gradient and weight-gradient products side by side
 //     in the backward phases.
@@ -208,18 +209,17 @@ struct MlpSmem {
   static constexpr int W0_SZ = (NS1 * D0 > D1 * KS0) ? NS1 * D0 : D1 * KS0;
   static constexpr int W1 = W0 + W0_SZ;                        // fwd: [NS2][D1] swizzled;  bwd: [D2][NS1] plain
   static constexpr int W1_SZ = (NS2 * D1 > D2 * NS1) ? NS2 * D1 : D2 * NS1;
-  // receive buffers: each is written by the peers exactly once per launch.  a3 is dead after this CTA's P2 products, which precede its a4
-  // push; no peer can produce dz3 before it has this CTA's a4 (and dz4), so dz3 lands in the same buffer without a write-after-read barrier
+  // receive buffers: each is written by the peers exactly once per launch.  No peer can produce dz3 before it holds this CTA's a4, and
+  // this CTA pushes a4 only after its P2 products have finished reading a3, so dz3 lands in the a3 buffer without a write-after-read barrier
   static constexpr int A3 = W1 + W1_SZ;                        // [32][D1] swizzled  (later: dz3)
   static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled  (earlier: P1 scratch; later: P4 / P5 scratch)
-  static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled  (earlier: P1 / P2 scratch)
-  static constexpr int W2 = DZ4 + MC_B * D2;                   // [16][D2] plain
+  static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled, computed locally  (earlier: P1 / P2 / logit scratch)
+  static constexpr int W2 = DZ4 + MC_B * D2;                   // [16][D2] swizzled, rows >= C zero
   static constexpr int DL = W2 + MC_CMAX * D2;                 // [32][16] dlogits
   static constexpr int MISC = DL + MC_B * MC_CMAX;             // b0 slice [NS1] | b1 slice [NS2] | b2 [16] | label [32]
   static constexpr int A3OWN = MISC + NS1 + NS2 + 16 + 32;     // [32][NS1] plain: this CTA's a3 columns (ReLU mask of dz3, dW1)
-  static constexpr int A4OWN = A3OWN + MC_B * NS1;             // [32][NS2] plain: this CTA's a4 columns (ReLU mask of dz4, dW2)
-  static constexpr int BAR = A4OWN + MC_B * NS2;               // 4 mbarriers: a3, a4, dz4, dz3 landed
-  static constexpr int TOTAL = BAR + 4 * 2;
+  static constexpr int BAR = A3OWN + MC_B * NS1;               // 3 mbarriers: a3, a4, dz3 landed
+  static constexpr int TOTAL = BAR + 3 * 2;
   static constexpr int BYTES = TOTAL * 4;
 };
 
@@ -237,25 +237,26 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   static_assert(L::BAR % 2 == 0, "mbarriers are 8-byte aligned");
   extern __shared__ __align__(16) float sm[];
   float* sX = sm + L::X; float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
-  float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL; float* sA3own = sm + L::A3OWN; float* sA4own = sm + L::A4OWN;
+  float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL; float* sA3own = sm + L::A3OWN;
   float* sB0 = sm + L::MISC; float* sB1 = sB0 + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
   uint64_t* bar = reinterpret_cast<uint64_t*>(sm + L::BAR);
-  uint64_t* bar_a3 = bar; uint64_t* bar_a4 = bar + 1; uint64_t* bar_dz4 = bar + 2; uint64_t* bar_dz3 = bar + 3;
+  uint64_t* bar_a3 = bar; uint64_t* bar_a4 = bar + 1; uint64_t* bar_dz3 = bar + 2;
   cg::cluster_group cluster = cg::this_cluster();
   const int cr = (int)cluster.block_rank();
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int B = p.B, C = p.C;
-  const bool dbg_on = p.dbg != nullptr && cr == 0 && tid == 0;
-  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; } };
+  // stamp by thread `by` of cluster CTA 0 (thread 0 unless a slot marks the end of warp-group 1's work)
+  auto stamp = [&](int slot, int by = 0) {
+    if (p.dbg != nullptr && cr == 0 && tid == by) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
+  };
   stamp(0);
 
   // ---------------- start-up: each receive barrier expects its whole buffer (dz3: all but this CTA's own columns, which are stored locally).
   // The peers push into this CTA's shared memory only after the cluster barrier below, so the barriers are armed before any byte arrives.
   if (tid == 0) {
-    for (int i = 0; i < 4; ++i) mbar_init(bar + i, 1);
+    for (int i = 0; i < 3; ++i) mbar_init(bar + i, 1);
     mbar_arrive_expect_tx(bar_a3, MC_B * D1 * 4);
     mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
-    mbar_arrive_expect_tx(bar_dz4, MC_B * D2 * 4);
     mbar_arrive_expect_tx(bar_dz3, (CS - 1) * MC_B * NS1 * 4);
     fence_barrier_init();      // (the release the peers need: nothing else this CTA wrote so far is read by them)
   }
@@ -267,8 +268,9 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   stage_swizzled_async(sW1, p.w1 + (long long)cr * NS2 * D1, NS2, D1, D1);
   for (int c = tid; c < MC_CMAX * (D2 >> 2); c += MC_THREADS) {
     const int r = c / (D2 >> 2), q = c - r * (D2 >> 2);
-    if (r < C) cp_async16(sW2 + r * D2 + (q << 2), p.w2 + (long long)r * D2 + (q << 2));
-    else *reinterpret_cast<float4*>(sW2 + r * D2 + (q << 2)) = make_float4(0.f, 0.f, 0.f, 0.f);
+    float* dst = sW2 + sw_off(r, q << 2, D2);
+    if (r < C) cp_async16(dst, p.w2 + (long long)r * D2 + (q << 2));
+    else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   if (tid < NS1) sB0[tid] = p.b0[cr * NS1 + tid];
   if (tid < NS2) sB1[tid] = p.b1[cr * NS2 + tid];
@@ -339,71 +341,90 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       v.x = fmaxf(v.x + sB1[4 * n4], 0.f); v.y = fmaxf(v.y + sB1[4 * n4 + 1], 0.f);
       v.z = fmaxf(v.z + sB1[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB1[4 * n4 + 3], 0.f);
       if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
-      *reinterpret_cast<float4*>(sA4own + b * NS2 + 4 * n4) = v;
       push_all<CS>(sA4, sw_off(b, cr * NS2 + 4 * n4, D2), bar_a4, cr, v);
     }
   }
-  // ---------------- P3: classifier + softmax-CE (every CTA redundantly: 32 x C logits), dz4 slice, dW2 slice, db2
+  // ---------------- P3: classifier + softmax-CE (every CTA redundantly: 32 x C logits), the whole dz4, dW2 slice, db2
   {
     wait_landed(bar_a4);
     stamp(5);
-    for (int b = warp; b < MC_B; b += MC_THREADS / 32) {
-      // all class dot products of this row at once: 16 independent partial sums per lane, then one butterfly over the whole vector
-      // (a shuffle reduction per class would be a chain of 5 dependent ~25-cycle shuffles, ten times over)
-      float part[MC_CMAX];
+    constexpr int PER = 8 * (MC_CMAX / 4), KS = MC_HALF / PER;   // 32 logit tiles x 8 K splits on warp-group 0: NC = 16, K = D2
+    static_assert(KS * MC_B * MC_CMAX <= MC_B * D2, "logit partials fit the dz4 buffer");
+    if (tid < MC_HALF) {
+      // The dz4 buffer still holds P2's partials, but every one of them was read before this CTA's own a4 slice was pushed (the pushed
+      // values depend on those reads), and bar_a4 has counted that slice.  Rows >= C of W2 are zero, so their logits are just b2.
+      const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
+      float acc[4][4] = {};
+      prod_nt<D2, KS>(sA4, sW2, tb, tn, ks, acc);
+      put_partial<MC_CMAX>(sDZ4, tb, tn, ks, acc);
+    }
+    __syncthreads();
+    if (tid < MC_B * MC_CMAX / 4) {
+      // softmax-CE: four consecutive lanes hold one row, lane n4 of the four its classes 4 n4 .. 4 n4 + 3
+      const int b = tid >> 2, n4 = tid & 3, c0 = 4 * n4;
+      const float4 s4 = sum_partials<MC_CMAX, KS>(sDZ4, b, n4);
+      const float lg[4] = {s4.x + sB2[c0], s4.y + sB2[c0 + 1], s4.z + sB2[c0 + 2], s4.w + sB2[c0 + 3]};
+      float mx = -INFINITY;
 #pragma unroll
-      for (int c = 0; c < MC_CMAX; ++c) part[c] = 0.f;
+      for (int j = 0; j < 4; ++j) if (c0 + j < C) mx = fmaxf(mx, lg[j]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      float e[4], s = 0.f;
 #pragma unroll
-      for (int k = lane; k < D2; k += 32) {
-        const float av = sA4[sw_off(b, k, D2)];
-#pragma unroll
-        for (int c = 0; c < MC_CMAX; ++c) part[c] = fmaf(av, sW2[c * D2 + k], part[c]);      // rows >= C of sW2 are zero
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-        for (int c = 0; c < MC_CMAX; ++c) part[c] += __shfl_xor_sync(0xffffffffu, part[c], o);
-      float mylogit = 0.f;
-#pragma unroll
-      for (int c = 0; c < MC_CMAX; ++c) if (lane == c) mylogit = part[c] + sB2[c];
-      float mx = lane < C ? mylogit : -INFINITY;
-      mx = warp_max(mx);
-      const float e = lane < C ? __expf(mylogit - mx) : 0.f;
-      const float s = warp_sum(e);
+      for (int j = 0; j < 4; ++j) { e[j] = c0 + j < C ? __expf(lg[j] - mx) : 0.f; s += e[j]; }
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      s += __shfl_xor_sync(0xffffffffu, s, 2);
       const int l = (int)sLab[b];
-      if (lane < MC_CMAX) sDL[b * MC_CMAX + lane] = (lane < C && b < B) ? e / s - (lane == l ? 1.f : 0.f) : 0.f;
-      const float picked = __shfl_sync(0xffffffffu, mylogit, l & 31);
+      float dl[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) dl[j] = (c0 + j < C && b < B) ? e[j] / s - (c0 + j == l ? 1.f : 0.f) : 0.f;
+      *reinterpret_cast<float4*>(sDL + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
+      const int q = l & 3;
+      const float mine = q == 0 ? lg[0] : q == 1 ? lg[1] : q == 2 ? lg[2] : lg[3];
+      const float picked = __shfl_sync(0xffffffffu, mine, (lane & ~3) | ((l >> 2) & 3));
       if (cr == 0 && b < B) {
-        if (lane == 0) p.loss[b] = -(picked - mx - __logf(s));
-        if (p.logits != nullptr && lane < C) p.logits[(long long)b * C + lane] = mylogit;
+        if (n4 == 0) p.loss[b] = -(picked - mx - __logf(s));
+        if (p.logits != nullptr)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) if (c0 + j < C) p.logits[(long long)b * C + c0 + j] = lg[j];
       }
     }
-    cp_async_wait<0>();          // W1 column slice (and W0 column slice) landed
-    __syncthreads();             // dlogits complete, the staged slices visible; the full a4 buffer is dead from here on (P4 / P5 scratch)
+    __syncthreads();             // dlogits complete, the logit partials read
     if (tid < MC_HALF) {
-      // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m]   for m in this CTA's slice of D2, four columns per thread; pushed to the cluster
-      for (int e = tid; e < MC_B * NS2 / 4; e += MC_HALF) {
-        const int b = e / (NS2 / 4), m4 = 4 * (e % (NS2 / 4)), m = cr * NS2 + m4;
-        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int c = 0; c < C; ++c) {
-          const float d = sDL[b * MC_CMAX + c];
-          const float4 w = *reinterpret_cast<const float4*>(sW2 + c * D2 + m);
-          s.x = fmaf(d, w.x, s.x); s.y = fmaf(d, w.y, s.y); s.z = fmaf(d, w.z, s.z); s.w = fmaf(d, w.w, s.w);
+      // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m] over all of D2: four columns m of the rows b0, b0 + 8, b0 + 16, b0 + 24
+      // per thread, which share each W2 load.  Every CTA runs the same loop over c on the same data, so all of them hold the same bits.
+      constexpr int RSTEP = MC_HALF / (D2 / 4), NR = MC_B / RSTEP;
+      static_assert(MC_HALF % (D2 / 4) == 0 && MC_B % RSTEP == 0, "dz4 rows split evenly over warp-group 0");
+      const int b0 = tid / (D2 / 4), m = 4 * (tid % (D2 / 4));
+      float4 s[NR];
+#pragma unroll
+      for (int r = 0; r < NR; ++r) s[r] = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int c = 0; c < C; ++c) {
+        const float4 w = *reinterpret_cast<const float4*>(sW2 + sw_off(c, m, D2));
+#pragma unroll
+        for (int r = 0; r < NR; ++r) {
+          const float d = sDL[(b0 + r * RSTEP) * MC_CMAX + c];
+          s[r].x = fmaf(d, w.x, s[r].x); s[r].y = fmaf(d, w.y, s[r].y); s[r].z = fmaf(d, w.z, s[r].z); s[r].w = fmaf(d, w.w, s[r].w);
         }
-        const float4 a = *reinterpret_cast<const float4*>(sA4own + b * NS2 + m4);
-        if (!(a.x > 0.f)) s.x = 0.f;
-        if (!(a.y > 0.f)) s.y = 0.f;
-        if (!(a.z > 0.f)) s.z = 0.f;
-        if (!(a.w > 0.f)) s.w = 0.f;
-        push_all<CS>(sDZ4, sw_off(b, m, D2), bar_dz4, cr, s);
+      }
+#pragma unroll
+      for (int r = 0; r < NR; ++r) {
+        const int o = sw_off(b0 + r * RSTEP, m, D2);
+        const float4 a = *reinterpret_cast<const float4*>(sA4 + o);
+        float4 v = s[r];
+        if (!(a.x > 0.f)) v.x = 0.f;
+        if (!(a.y > 0.f)) v.y = 0.f;
+        if (!(a.z > 0.f)) v.z = 0.f;
+        if (!(a.w > 0.f)) v.w = 0.f;
+        *reinterpret_cast<float4*>(sDZ4 + o) = v;
       }
     } else {
-      // warp-group 1, off the critical path: dW2[c][m] = sum_b dl[b][c] * a4[b][m] (this CTA's m slice), db2 (CTA 0)
+      // warp-group 1: dW2[c][m] = sum_b dl[b][c] * a4[b][m] (this CTA's m slice), db2 (CTA 0)
       const int t = tid - MC_HALF;
       for (int e = t; e < C * NS2; e += MC_HALF) {
         const int c = e / NS2, m = e % NS2;
         float s = 0.f;
-        for (int b = 0; b < MC_B; ++b) s = fmaf(sDL[b * MC_CMAX + c], sA4own[b * NS2 + m], s);
+        for (int b = 0; b < MC_B; ++b) s = fmaf(sDL[b * MC_CMAX + c], sA4[sw_off(b, cr * NS2 + m, D2)], s);
         p.dw2[(long long)c * D2 + cr * NS2 + m] = s;
       }
       if (cr == 0 && t < C) {
@@ -412,12 +433,13 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
         p.db2[t] = s;
       }
     }
+    cp_async_wait<0>();          // W1 column slice (and W0 column slice) landed: first read in P4, so the head does not wait for them
+    __syncthreads();             // dz4 complete, the staged slices visible; the full a4 buffer is dead from here on (P4 / P5 scratch)
+    stamp(6);
   }
   // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice]);  dW1[:, slice of D1 columns] = dz4^T * a3[:, slice];  db1
   float* sDZ3 = sA3;
   {
-    wait_landed(bar_dz4);
-    stamp(6);
     if (tid < MC_HALF) {
       // warp-group 0: the data gradient dz3 (critical path)
       constexpr int PER = 2 * NS1, KS = MC_HALF / PER;   // K = D2
@@ -496,6 +518,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
         for (int bb = 0; bb < MC_B; ++bb) s += sDZ3[sw_off(bb, cr * NS1 + t0, D1)];
         p.db0[cr * NS1 + t0] = s;
       }
+      stamp(15, MC_HALF);   // warp-group 1's end: the kernel's tail when dW0 outlasts dx
     }
   }
   stamp(9);
