@@ -16,11 +16,13 @@
 //     is written once per launch, so after start-up there is no cluster-wide barrier (and no GPU-scope fence, no L1 invalidation) between
 //     layers: a CTA starts a layer as soon as its own inputs have landed.  dz4 is not handed off: once a4 has landed every CTA holds all
 //     of its inputs (a4, W2, dlogits) and computes the whole of it;
-//   * epilogues fused: bias, ReLU, ReLU masks of the backward pass, softmax / loss / dlogits, bias gradients (column sums).
-//   * 512 threads: the two warp-groups split K in the wide forward layer and run data-gradient and weight-gradient products side by side
-//     in the backward phases.
-// One cluster launch replaces what used to be seven kernel launches (dense0, dense1, head, dW1, dz3, dW0, da2); tools/kernel_times.py
-// times the whole chain with per-phase %globaltimer stamps.
+//   * epilogues fused: bias, ReLU, ReLU masks of the backward pass, softmax / loss / dlogits.
+//   * 512 threads: all of them on dense0, dz4 and dx; dense1, the logits and dz3 are too small for a deeper K split to pay.
+// The cluster kernel computes only what the convolution backward pass waits for (loss, logits, da2).  Nothing in the step reads the dense
+// weight gradients before the dense keys' exchange, so they are a second, ordinary grid (dense_wgrad_kernel) on a parallel branch: the
+// cluster kernel stores what they need (a3, a4, dz4, dz3, dlogits; about 50 KB) and the weight-gradient kernel turns them into dW0 / dW1 /
+// dW2 and the bias gradients.  Two launches replace what used to be seven (dense0, dense1, head, dW1, dz3, dW0, da2); tools/kernel_times.py
+// times the chain with per-phase %globaltimer stamps.
 //
 // Shapes are compile-time (D0 -> D1 -> D2 -> C<=16, batch <= 32): the demo CNN's 512 -> 256 -> 128 -> 10.  Other shapes use the wgmma GEMMs.
 #include <cooperative_groups.h>
@@ -31,8 +33,8 @@ namespace cg = cooperative_groups;
 
 namespace gx {
 
-constexpr int MC_THREADS = 512;   // 16 warps: two warp-groups of 256 that either split K (P1) or run data- and weight-gradient side by side (P4, P5)
-constexpr int MC_HALF = 256;
+constexpr int MC_THREADS = 512;   // 16 warps
+constexpr int MC_HALF = 256;      // warp-group 0: dense1, the logits and dz3
 constexpr int MC_B = 32;      // batch rows held (rows >= B are zero)
 constexpr int MC_CMAX = 16;   // classes (padded)
 
@@ -44,8 +46,9 @@ struct MlpChainParams {
   const float* label;   // [B] class index as float
   float* loss;          // [B]
   float* logits;        // [B][C] or nullptr
-  float* dw0; float* db0; float* dw1; float* db1; float* dw2; float* db2;
   float* dx;            // [B][D0]   gradient w.r.t. x
+  // what the weight gradients need (rows b < B): a3 [B][D1], a4 [B][D2], dz4 [B][D2], dz3 [B][D1], dlogits [B][16] (classes >= C zero)
+  float* a3; float* a4; float* dz4; float* dz3; float* dl;
   int B, C;
   unsigned long long* dbg;   // optional %globaltimer stamps of cluster CTA 0 (tools/kernel_times.py)
 };
@@ -91,7 +94,6 @@ __device__ __forceinline__ void wait_landed(uint64_t* bar) {
       "fence.acquire.sync_restrict::shared::cluster.cluster;" ::"r"(smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // stage `rows` x K floats (global row stride ld) into a swizzled K-major tile
 __device__ __forceinline__ void stage_swizzled_async(float* dst, const float* src, int rows, int K, long long ld) {
@@ -171,40 +173,42 @@ __device__ __forceinline__ float4 sum_partials(const float* scratch, int b, int 
   }
   return s;
 }
-// wgrad: dW[n][k] = sum_b DZ[b][nbase+n] * X[b][k]   (DZ: swizzled [32][ND], X: swizzled [32][KD]); thread tile TN x 4, coalesced global store
-template <int ND, int KD, int TN>
-__device__ __forceinline__ void wgrad_tile(const float* __restrict__ sDZ, const float* __restrict__ sX, int nbase, int n0, int tk, float* __restrict__ out_row0) {
-  float acc[TN][4];
-#pragma unroll
-  for (int i = 0; i < TN; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
+// wgrad: dW[n][k] = sum_{b < B} DZ[b][n] * X[b][k] for rows n0 .. n0+3 (those < nrows are stored) and columns k0 .. k0+3, read from global
+// memory (DZ: [B][LDZ], X and dW: [.][LDX]).  One fmaf chain per output over b ascending.
+template <int LDZ, int LDX>
+__device__ __forceinline__ void wgrad_4x4(const float* __restrict__ dz, const float* __restrict__ x, int B, int n0, int k0, int nrows,
+                                          float* __restrict__ out) {
+  float acc[4][4] = {};
 #pragma unroll 4
-  for (int b = 0; b < MC_B; ++b) {
-    const int key = (b >> 2) & 7;
-    const float4 x = *reinterpret_cast<const float4*>(sX + b * KD + ((tk ^ key) << 2));
-    float dz[TN];
+  for (int b = 0; b < B; ++b) {
+    const float4 d = *reinterpret_cast<const float4*>(dz + b * LDZ + n0);
+    const float4 v = *reinterpret_cast<const float4*>(x + b * LDX + k0);
+    const float dd[4] = {d.x, d.y, d.z, d.w};
 #pragma unroll
-    for (int q = 0; q < TN / 4; ++q) {
-      const float4 d = *reinterpret_cast<const float4*>(sDZ + b * ND + ((((nbase + n0) >> 2) + q) ^ key) * 4);
-      dz[4 * q] = d.x; dz[4 * q + 1] = d.y; dz[4 * q + 2] = d.z; dz[4 * q + 3] = d.w;
-    }
-#pragma unroll
-    for (int i = 0; i < TN; ++i) {
-      acc[i][0] = fmaf(dz[i], x.x, acc[i][0]);
-      acc[i][1] = fmaf(dz[i], x.y, acc[i][1]);
-      acc[i][2] = fmaf(dz[i], x.z, acc[i][2]);
-      acc[i][3] = fmaf(dz[i], x.w, acc[i][3]);
+    for (int i = 0; i < 4; ++i) {
+      acc[i][0] = fmaf(dd[i], v.x, acc[i][0]);
+      acc[i][1] = fmaf(dd[i], v.y, acc[i][1]);
+      acc[i][2] = fmaf(dd[i], v.z, acc[i][2]);
+      acc[i][3] = fmaf(dd[i], v.w, acc[i][3]);
     }
   }
 #pragma unroll
-  for (int i = 0; i < TN; ++i)
-    *reinterpret_cast<float4*>(out_row0 + (long long)(n0 + i) * KD + 4 * tk) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+  for (int i = 0; i < 4; ++i)
+    if (n0 + i < nrows) *reinterpret_cast<float4*>(out + (n0 + i) * LDX + k0) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+}
+// bias gradient: db[n] = sum_{b < B} DZ[b][n], b ascending
+template <int LDZ>
+__device__ __forceinline__ float colsum(const float* __restrict__ dz, int B, int n) {
+  float s = 0.f;
+  for (int b = 0; b < B; ++b) s += dz[b * LDZ + n];
+  return s;
 }
 
 template <int D0, int D1, int D2, int CS>
 struct MlpSmem {
   static constexpr int NS1 = D1 / CS, NS2 = D2 / CS, KS0 = D0 / CS;
   // float offsets
-  static constexpr int X = 0;                                  // [32][D0] swizzled
+  static constexpr int X = 0;                                  // [32][D0] swizzled  (dead after P1: P4 / P5 scratch)
   static constexpr int W0 = X + MC_B * D0;                     // fwd: [NS1][D0] swizzled;  bwd: [D1][KS0] plain
   static constexpr int W0_SZ = (NS1 * D0 > D1 * KS0) ? NS1 * D0 : D1 * KS0;
   static constexpr int W1 = W0 + W0_SZ;                        // fwd: [NS2][D1] swizzled;  bwd: [D2][NS1] plain
@@ -212,12 +216,12 @@ struct MlpSmem {
   // receive buffers: each is written by the peers exactly once per launch.  No peer can produce dz3 before it holds this CTA's a4, and
   // this CTA pushes a4 only after its P2 products have finished reading a3, so dz3 lands in the a3 buffer without a write-after-read barrier
   static constexpr int A3 = W1 + W1_SZ;                        // [32][D1] swizzled  (later: dz3)
-  static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled  (earlier: P1 scratch; later: P4 / P5 scratch)
+  static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled  (earlier: P1 scratch)
   static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled, computed locally  (earlier: P1 / P2 / logit scratch)
   static constexpr int W2 = DZ4 + MC_B * D2;                   // [16][D2] swizzled, rows >= C zero
   static constexpr int DL = W2 + MC_CMAX * D2;                 // [32][16] dlogits
   static constexpr int MISC = DL + MC_B * MC_CMAX;             // b0 slice [NS1] | b1 slice [NS2] | b2 [16] | label [32]
-  static constexpr int A3OWN = MISC + NS1 + NS2 + 16 + 32;     // [32][NS1] plain: this CTA's a3 columns (ReLU mask of dz3, dW1)
+  static constexpr int A3OWN = MISC + NS1 + NS2 + 16 + 32;     // [32][NS1] plain: this CTA's a3 columns (ReLU mask of dz3)
   static constexpr int BAR = A3OWN + MC_B * NS1;               // 3 mbarriers: a3, a4, dz3 landed
   static constexpr int TOTAL = BAR + 3 * 2;
   static constexpr int BYTES = TOTAL * 4;
@@ -231,9 +235,10 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
   static_assert(D0 % 64 == 0 && D1 % 64 == 0 && D2 % 64 == 0, "layer widths must be multiples of 64");
   static_assert(NS1 % 8 == 0 && NS2 % 4 == 0 && KS0 % 4 == 0, "slices must hold whole register tiles");
-  static_assert(MC_THREADS % (2 * NS1) == 0 && MC_HALF % (2 * NS2) == 0 && MC_HALF % (2 * NS1) == 0 && MC_HALF % (2 * KS0) == 0, "K splits");
-  static_assert(MC_THREADS / (2 * NS1) * MC_B * NS1 <= 2 * MC_B * D2 && MC_HALF / (2 * KS0) * MC_B * KS0 <= MC_B * D2, "scratch sizes");
-  static_assert(MC_HALF % (NS1 / 4) == 0 && D2 % (MC_HALF / (NS1 / 4)) == 0, "dW1 tiles");
+  static_assert(MC_HALF % (2 * NS1) == 0 && MC_HALF % (2 * NS2) == 0 && MC_THREADS % (2 * KS0) == 0, "K splits");
+  static_assert(MC_THREADS / (2 * NS1) * MC_B * NS1 <= 2 * MC_B * D2, "P1 scratch fits the a4 and dz4 buffers");
+  static_assert(MC_HALF / (2 * NS1) * MC_B * NS1 <= MC_B * D0 && MC_THREADS / (2 * KS0) * MC_B * KS0 <= MC_B * D0, "P4 / P5 scratch fits x");
+  static_assert(MC_B * NS1 / 4 <= MC_HALF && MC_B * NS2 / 4 <= MC_HALF, "one thread per float4 of a3 / a4");
   static_assert(L::BAR % 2 == 0, "mbarriers are 8-byte aligned");
   extern __shared__ __align__(16) float sm[];
   float* sX = sm + L::X; float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
@@ -245,9 +250,9 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   const int cr = (int)cluster.block_rank();
   const int tid = threadIdx.x, lane = tid & 31;
   const int B = p.B, C = p.C;
-  // stamp by thread `by` of cluster CTA 0 (thread 0 unless a slot marks the end of warp-group 1's work)
-  auto stamp = [&](int slot, int by = 0) {
-    if (p.dbg != nullptr && cr == 0 && tid == by) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
+  // stamp by thread 0 of cluster CTA 0
+  auto stamp = [&](int slot) {
+    if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
   };
   stamp(0);
 
@@ -342,6 +347,11 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       v.z = fmaxf(v.z + sB1[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB1[4 * n4 + 3], 0.f);
       if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
       push_all<CS>(sA4, sw_off(b, cr * NS2 + 4 * n4, D2), bar_a4, cr, v);
+      if (b < B) *reinterpret_cast<float4*>(p.a4 + b * D2 + cr * NS2 + 4 * n4) = v;
+    } else if (tid >= MC_HALF && tid - MC_HALF < MC_B * NS1 / 4) {
+      // warp-group 1 is idle in P2: it stores this CTA's a3 columns for the weight-gradient kernel
+      const int b = (tid - MC_HALF) / (NS1 / 4), n4 = (tid - MC_HALF) % (NS1 / 4);
+      if (b < B) *reinterpret_cast<float4*>(p.a3 + b * D1 + cr * NS1 + 4 * n4) = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * n4);
     }
   }
   // ---------------- P3: classifier + softmax-CE (every CTA redundantly: 32 x C logits), the whole dz4, dW2 slice, db2
@@ -383,6 +393,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       const float mine = q == 0 ? lg[0] : q == 1 ? lg[1] : q == 2 ? lg[2] : lg[3];
       const float picked = __shfl_sync(0xffffffffu, mine, (lane & ~3) | ((l >> 2) & 3));
       if (cr == 0 && b < B) {
+        *reinterpret_cast<float4*>(p.dl + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
         if (n4 == 0) p.loss[b] = -(picked - mx - __logf(s));
         if (p.logits != nullptr)
 #pragma unroll
@@ -390,11 +401,11 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       }
     }
     __syncthreads();             // dlogits complete, the logit partials read
-    if (tid < MC_HALF) {
-      // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m] over all of D2: four columns m of the rows b0, b0 + 8, b0 + 16, b0 + 24
-      // per thread, which share each W2 load.  Every CTA runs the same loop over c on the same data, so all of them hold the same bits.
-      constexpr int RSTEP = MC_HALF / (D2 / 4), NR = MC_B / RSTEP;
-      static_assert(MC_HALF % (D2 / 4) == 0 && MC_B % RSTEP == 0, "dz4 rows split evenly over warp-group 0");
+    {
+      // dz4[b][m] = relu'(a4[b][m]) * sum_c dl[b][c] * W2[c][m] over all of D2: four columns m of the rows b0, b0 + 16 per thread, which
+      // share each W2 load.  Every CTA runs the same loop over c on the same data, so all of them hold the same bits.
+      constexpr int RSTEP = MC_THREADS / (D2 / 4), NR = MC_B / RSTEP;
+      static_assert(MC_THREADS % (D2 / 4) == 0 && MC_B % RSTEP == 0, "dz4 rows split evenly over the threads");
       const int b0 = tid / (D2 / 4), m = 4 * (tid % (D2 / 4));
       float4 s[NR];
 #pragma unroll
@@ -417,111 +428,103 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
         if (!(a.z > 0.f)) v.z = 0.f;
         if (!(a.w > 0.f)) v.w = 0.f;
         *reinterpret_cast<float4*>(sDZ4 + o) = v;
-      }
-    } else {
-      // warp-group 1: dW2[c][m] = sum_b dl[b][c] * a4[b][m] (this CTA's m slice), db2 (CTA 0)
-      const int t = tid - MC_HALF;
-      for (int e = t; e < C * NS2; e += MC_HALF) {
-        const int c = e / NS2, m = e % NS2;
-        float s = 0.f;
-        for (int b = 0; b < MC_B; ++b) s = fmaf(sDL[b * MC_CMAX + c], sA4[sw_off(b, cr * NS2 + m, D2)], s);
-        p.dw2[(long long)c * D2 + cr * NS2 + m] = s;
-      }
-      if (cr == 0 && t < C) {
-        float s = 0.f;
-        for (int b = 0; b < MC_B; ++b) s += sDL[b * MC_CMAX + t];
-        p.db2[t] = s;
+        if (b0 + r * RSTEP < B && m / NS2 == cr)     // this CTA's column slice, for the weight-gradient kernel
+          *reinterpret_cast<float4*>(p.dz4 + (b0 + r * RSTEP) * D2 + m) = v;
       }
     }
     cp_async_wait<0>();          // W1 column slice (and W0 column slice) landed: first read in P4, so the head does not wait for them
-    __syncthreads();             // dz4 complete, the staged slices visible; the full a4 buffer is dead from here on (P4 / P5 scratch)
+    __syncthreads();             // dz4 complete, the staged slices visible
     stamp(6);
   }
-  // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice]);  dW1[:, slice of D1 columns] = dz4^T * a3[:, slice];  db1
+  // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice])          NC = NS1, K = D2, split over warp-group 0
+  // (split over all 16 warps, the deeper reduction made "dz3 pushed" slower: 2.4 us instead of 2.0)
   float* sDZ3 = sA3;
+  float* scratch = sX;                                   // x is dead after P1: P4 / P5 partials
   {
+    constexpr int PER = 2 * NS1, KS = MC_HALF / PER;
     if (tid < MC_HALF) {
-      // warp-group 0: the data gradient dz3 (critical path)
-      constexpr int PER = 2 * NS1, KS = MC_HALF / PER;   // K = D2
       const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
       float acc[4][4] = {};
       prod_nn<D2, NS1, KS>(sDZ4, sW1, tb, tn, ks, acc);
-      put_partial<NS1>(sA4, tb, tn, ks, acc);           // scratch = a4 buffer (dead after P3)
-      named_bar_sync(1, MC_HALF);
-      if (tid < MC_B * NS1 / 4) {
-        const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);
-        float4 dz3v = sum_partials<NS1, KS>(sA4, b, n4);
-        const float4 a3 = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * n4);
-        dz3v.x = a3.x > 0.f ? dz3v.x : 0.f; dz3v.y = a3.y > 0.f ? dz3v.y : 0.f; dz3v.z = a3.z > 0.f ? dz3v.z : 0.f; dz3v.w = a3.w > 0.f ? dz3v.w : 0.f;
-        const int o = sw_off(b, cr * NS1 + 4 * n4, D1);
-        push_all<CS, CS - 1>(sDZ3, o, bar_dz3, cr, dz3v);
-        *reinterpret_cast<float4*>(sDZ3 + o) = dz3v;   // own columns: stored locally (warp-group 1 reads them without waiting for the peers)
-      }
-      named_bar_arrive(2, MC_THREADS);                   // own dz3 columns stored -> warp-group 1 may start dW0
-      stamp(7);
-    } else {
-      // warp-group 1, concurrently: dW1 columns [cr*NS1, +NS1) of all D2 rows as TN x 4 tiles, and the db1 slice
-      constexpr int CG = NS1 / 4, TN = D2 / (MC_HALF / CG);
-      const int t = tid - MC_HALF, tk = t % CG, n0 = (t / CG) * TN;
-      float acc[TN][4];
-#pragma unroll
-      for (int i = 0; i < TN; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
-#pragma unroll 4
-      for (int b = 0; b < MC_B; ++b) {
-        const float4 a = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * tk);
-#pragma unroll
-        for (int i = 0; i < TN; ++i) {
-          const float d = sDZ4[sw_off(b, n0 + i, D2)];
-          acc[i][0] = fmaf(d, a.x, acc[i][0]); acc[i][1] = fmaf(d, a.y, acc[i][1]);
-          acc[i][2] = fmaf(d, a.z, acc[i][2]); acc[i][3] = fmaf(d, a.w, acc[i][3]);
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < TN; ++i)
-        *reinterpret_cast<float4*>(p.dw1 + (long long)(n0 + i) * D1 + cr * NS1 + 4 * tk) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-      if (t < NS2) {
-        float s = 0.f;
-        for (int bb = 0; bb < MC_B; ++bb) s += sDZ4[sw_off(bb, cr * NS2 + t, D2)];
-        p.db1[cr * NS2 + t] = s;
-      }
+      put_partial<NS1>(scratch, tb, tn, ks, acc);
     }
+    __syncthreads();
+    if (tid < MC_B * NS1 / 4) {
+      const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);
+      float4 dz3v = sum_partials<NS1, KS>(scratch, b, n4);
+      const float4 a3 = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * n4);
+      dz3v.x = a3.x > 0.f ? dz3v.x : 0.f; dz3v.y = a3.y > 0.f ? dz3v.y : 0.f; dz3v.z = a3.z > 0.f ? dz3v.z : 0.f; dz3v.w = a3.w > 0.f ? dz3v.w : 0.f;
+      const int o = sw_off(b, cr * NS1 + 4 * n4, D1);
+      push_all<CS, CS - 1>(sDZ3, o, bar_dz3, cr, dz3v);
+      *reinterpret_cast<float4*>(sDZ3 + o) = dz3v;   // own columns: stored locally
+      if (b < B) *reinterpret_cast<float4*>(p.dz3 + b * D1 + cr * NS1 + 4 * n4) = dz3v;
+    }
+    stamp(7);
+    __syncthreads();                                     // own dz3 columns stored, the P4 partials read
   }
-  // ---------------- P5: dx[:, slice of D0] = dz3 * W0[:, slice];  dW0[slice of D1 rows] = dz3[:, rows]^T * x;  db0
+  // ---------------- P5: dx[:, slice of D0] = dz3 * W0[:, slice]                      NC = KS0, K = D1, split over all 16 warps
   {
-    if (tid < MC_HALF) {
-      // warp-group 0: the input gradient (what the convolution backward pass is waiting for)
-      constexpr int PER = 2 * KS0, KS = MC_HALF / PER;   // K = D1
-      named_bar_sync(1, MC_HALF);                        // own dz3 columns stored, P4 scratch read
-      wait_landed(bar_dz3);                              // the peers' columns
-      stamp(8);
-      const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
-      float acc[4][4] = {};
-      prod_nn<D1, KS0, KS>(sDZ3, sW0, tb, tn, ks, acc);
-      stamp(14);
-      put_partial<KS0>(sA4, tb, tn, ks, acc);           // scratch = a4 buffer again (warp-group 0 only): KS x 32 x KS0 floats = 16 KB
-      named_bar_sync(1, MC_HALF);
-      for (int e = tid; e < MC_B * KS0 / 4; e += MC_HALF) {
-        const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
-        if (b < B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(sA4, b, n4);
-      }
-    } else {
-      // warp-group 1, concurrently: dW0 rows [cr*NS1, +NS1) as 8 x 4 tiles (4 x D0/4 = 512 tiles, two per thread) and the db0 slice.
-      // It needs only this CTA's own dz3 columns, so it does not wait for the peers.
-      named_bar_sync(2, MC_THREADS);
-      const int t0 = tid - MC_HALF;
-      for (int t = t0; t < (NS1 / 8) * (D0 / 4); t += MC_HALF) {
-        const int tnw = t / (D0 / 4), tk = t % (D0 / 4);
-        wgrad_tile<D1, D0, 8>(sDZ3, sX, cr * NS1, 8 * tnw, tk, p.dw0 + (long long)cr * NS1 * D0);
-      }
-      if (t0 < NS1) {
-        float s = 0.f;
-        for (int bb = 0; bb < MC_B; ++bb) s += sDZ3[sw_off(bb, cr * NS1 + t0, D1)];
-        p.db0[cr * NS1 + t0] = s;
-      }
-      stamp(15, MC_HALF);   // warp-group 1's end: the kernel's tail when dW0 outlasts dx
+    wait_landed(bar_dz3);                                // the peers' columns
+    stamp(8);
+    constexpr int PER = 2 * KS0, KS = MC_THREADS / PER;
+    const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
+    float acc[4][4] = {};
+    prod_nn<D1, KS0, KS>(sDZ3, sW0, tb, tn, ks, acc);
+    stamp(14);
+    put_partial<KS0>(scratch, tb, tn, ks, acc);
+    __syncthreads();
+    for (int e = tid; e < MC_B * KS0 / 4; e += MC_THREADS) {
+      const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
+      if (b < B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(scratch, b, n4);
     }
   }
   stamp(9);
+}
+
+// ---- the dense weight gradients, from what mlp_chain_kernel stored: dW0 = dz3^T x, dW1 = dz4^T a3, dW2 = dl^T a4, and the bias gradients
+// as column sums.  K = B <= 32, so every output is one register-held fmaf chain over b; one thread per 4 x 4 tile (or per bias element).
+struct DenseWgradParams {
+  const float* x; const float* a3; const float* a4; const float* dz4; const float* dz3; const float* dl;   // rows b < B
+  float* dw0; float* db0; float* dw1; float* db1; float* dw2; float* db2;
+  int B, C;
+  unsigned long long* dbg;   // optional: 16 start of CTA 0 | 17 its grid dependency resolved | 18 end of the last CTA
+};
+constexpr int WG_THREADS = 256;
+template <int D0, int D1, int D2>
+struct DenseWgradGrid {
+  static constexpr int T0 = (D1 / 4) * (D0 / 4), T1 = (D2 / 4) * (D1 / 4), T2 = (MC_CMAX / 4) * (D2 / 4);   // 4 x 4 tiles of dW0, dW1, dW2
+  static constexpr int THREADS = T0 + T1 + T2 + D1 + D2 + MC_CMAX;                                            // + db0, db1, db2
+  static constexpr int CTAS = (THREADS + WG_THREADS - 1) / WG_THREADS;
+};
+
+template <int D0, int D1, int D2>
+__global__ void __launch_bounds__(WG_THREADS) dense_wgrad_kernel(const DenseWgradParams p) {
+  using G = DenseWgradGrid<D0, D1, D2>;
+  const bool stamps = p.dbg != nullptr && threadIdx.x == 0;
+  auto now = [] { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; };
+  if (stamps && blockIdx.x == 0) p.dbg[16] = now();
+  pdl_launch();   // the dense keys' exchange behind this kernel may become resident and stage; its own griddepcontrol.wait covers this grid
+  pdl_wait();
+  if (stamps && blockIdx.x == 0) p.dbg[17] = now();
+  const int B = p.B;
+  int t = blockIdx.x * WG_THREADS + threadIdx.x;
+  if (t < G::T0) {
+    wgrad_4x4<D1, D0>(p.dz3, p.x, B, 4 * (t / (D0 / 4)), 4 * (t % (D0 / 4)), D1, p.dw0);
+  } else if ((t -= G::T0) < G::T1) {
+    wgrad_4x4<D2, D1>(p.dz4, p.a3, B, 4 * (t / (D1 / 4)), 4 * (t % (D1 / 4)), D2, p.dw1);
+  } else if ((t -= G::T1) < G::T2) {
+    wgrad_4x4<MC_CMAX, D2>(p.dl, p.a4, B, 4 * (t / (D2 / 4)), 4 * (t % (D2 / 4)), p.C, p.dw2);
+  } else if ((t -= G::T2) < D1) {
+    p.db0[t] = colsum<D1>(p.dz3, B, t);
+  } else if ((t -= D1) < D2) {
+    p.db1[t] = colsum<D2>(p.dz4, B, t);
+  } else if ((t -= D2) < p.C) {
+    p.db2[t] = colsum<MC_CMAX>(p.dl, B, t);
+  }
+  if (p.dbg != nullptr) {
+    __syncthreads();
+    if (threadIdx.x == 0) atomicMax(p.dbg + 18, now());
+  }
 }
 
 }  // namespace gx
@@ -559,13 +562,14 @@ static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
 static unsigned long long* g_mlp_dbg = nullptr;
 GX_API int gx_mlp_chain_set_debug(unsigned long long* p) { g_mlp_dbg = p; return 0; }
 
-GX_API int gx_mlp_chain_fwd_bwd(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
-                                const float* label, float* loss, float* logits, float* dw0, float* db0, float* dw1, float* db1, float* dw2,
-                                float* db2, float* dx, int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
+// the data path: loss, logits, dx; stores a3, a4, dz4, dz3 and the dlogits (rows b < B) for gx_dense_wgrad
+GX_API int gx_mlp_chain(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
+                        const float* label, float* loss, float* logits, float* dx, float* a3, float* a4, float* dz4, float* dz3, float* dl,
+                        int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
   if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
   MlpChainParams p;
-  p.x = x; p.w0 = w0; p.b0 = b0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits;
-  p.dw0 = dw0; p.db0 = db0; p.dw1 = dw1; p.db1 = db1; p.dw2 = dw2; p.db2 = db2; p.dx = dx; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
+  p.x = x; p.w0 = w0; p.b0 = b0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
+  p.a3 = a3; p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
   // cluster of 16 CTAs (one GPC) halves every slice; fall back to the portable size 8 when the device cannot co-schedule 16
   static int want = -1;
   if (want < 0) { const char* e = getenv("GEOMX_MLP_CLUSTER"); want = e ? atoi(e) : 16; }
@@ -575,5 +579,16 @@ GX_API int gx_mlp_chain_fwd_bwd(const float* x, const float* w0, const float* b0
     want = 8;
   }
   return mlp_launch<8>(p, stream);
+}
+
+// dW0 / db0, dW1 / db1, dW2 / db2 (overwritten) from what gx_mlp_chain stored; x has exactly B rows, dl rows hold 16 floats
+GX_API int gx_dense_wgrad(const float* x, const float* a3, const float* a4, const float* dz4, const float* dz3, const float* dl, float* dw0,
+                          float* db0, float* dw1, float* db1, float* dw2, float* db2, int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
+  if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
+  DenseWgradParams p;
+  p.x = x; p.a3 = a3; p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl;
+  p.dw0 = dw0; p.db0 = db0; p.dw1 = dw1; p.db1 = db1; p.dw2 = dw2; p.db2 = db2; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
+  launch_pdl(dense_wgrad_kernel<512, 256, 128>, dim3(DenseWgradGrid<512, 256, 128>::CTAS), dim3(WG_THREADS), 0, stream, p);
+  return GX_CHECK_LAUNCH();
 }
 GX_API int gx_mlp_chain_smem_bytes() { return MlpSmem<512, 256, 128, 8>::BYTES; }

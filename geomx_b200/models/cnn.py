@@ -5,10 +5,12 @@
 
 ``HipsCNNTrainStep`` is the flagship hot path: one *training step* = forward + backward of that network for a per-worker batch
 plus the HiPS push/pull of all 10 keys (``dist_sync``: party aggregation → global aggregation + optimizer → broadcast), captured ONCE
-into a CUDA graph and replayed per step.  At the reference's batch size (32 per worker) the step is 4-5 hand-written sm_90a launches:
+into a CUDA graph and replayed per step.  At the reference's batch size (32 per worker) the step is 5-6 hand-written sm_90a launches:
 
   cnn_fwd      conv0+bias+ReLU+pool → conv1+bias+ReLU+pool, fp32 FMA, the conv0 map never leaves shared memory      (csrc/kernels/cnn_direct.cu)
-  mlp_chain    dense0 → dense1 → classifier → softmax-CE forward AND backward in one 16-CTA cluster                  (csrc/kernels/mlp_chain.cu)
+  mlp_chain    dense0 → dense1 → classifier → softmax-CE forward and the data gradients down to da2, one 16-CTA cluster (csrc/kernels/mlp_chain.cu)
+  dense_wgrad  the three dense weight gradients and bias gradients, on a parallel branch: in the dense channel's step on the
+               high-priority stream when there is one, otherwise on the side stream, joined before the exchange   (csrc/kernels/mlp_chain.cu)
   cnn_bwd_all  conv1 data gradient + pool/ReLU routing + conv0 weight gradient ‖ conv1 weight gradient, one grid      (csrc/kernels/cnn_direct.cu)
   exchange     one LL kernel for all keys after the backward pass (several ranks), or key-group channels: the dense keys' exchange on
                a high-priority stream underneath cnn_bwd_all, the conv keys' one-hop exchange after it (one rank / GEOMX_STEP_OVERLAP=1)
@@ -177,6 +179,7 @@ class HipsCNNTrainStep:
         self.a3, self.a4 = e(B, 256), e(B, 128)
         self.loss, self.logits = e(B), e(B, 10)
         self.dz4, self.dz3, self.da2 = e(B, 128), e(B, 256), e(B, 512)
+        self.dl = e(B, 16)          # dlogits, classes padded to 16 (cluster kernel -> dense weight-gradient kernel)
         self.dz2rows, self.dcol1, self.da1 = e(B * 64, 32), e(B * 64, 400), e(B, 16, 12, 12)
         self.loss_host = torch.empty(B, dtype=f32).pin_memory()
         self.lookahead = bool(lookahead) and mode == "dist_sync" and not self.hfa
@@ -275,9 +278,19 @@ class HipsCNNTrainStep:
             ("da2 gemm", "main", lambda: n.gemm(self.dz3, P[4], self.da2, b_mn=True)),
         ]
         if self.fused_mlp:
-            # dense0 -> dense1 -> classifier -> softmax-CE forward and backward: ONE 8-CTA cluster launch instead of the seven above
-            head = [("mlp chain fwd+bwd (cluster)", "main", lambda: n.mlp_chain(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits,
-                                                                              G[4], G[5], G[6], G[7], G[8], G[9], self.da2))]
+            # dense0 -> dense1 -> classifier -> softmax-CE forward and backward: one cluster launch for the data path (what the convolution
+            # backward pass waits for) and one weight-gradient launch on a parallel branch, instead of the seven above
+            head = [("mlp chain fwd+bwd (cluster)", "main", lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss,
+                                                                                   self.logits, self.da2, self.a3, self.a4, self.dz4, self.dz3, self.dl))]
+            wgrad = lambda: n.dense_wgrad(a2f, self.a3, self.a4, self.dz4, self.dz3, self.dl, G[4], G[5], G[6], G[7], G[8], G[9])
+            if kv_dense and not self.lookahead:
+                # the dense channel reads these gradients: issued in the same comm-stream step, only a programmatic edge separates the two
+                name, _, chan = kv_dense[0]
+                kv_dense = [("dense weight gradients + " + name, "comm", lambda: (wgrad(), chan()))]
+            else:
+                # side stream, joined before the exchange (a dense channel's comm step waits for it too).  A look-ahead launch ends with
+                # the next batch's forward convolutions, which overwrite the x this kernel reads: _body joins the side branch before them
+                head.append(("dense weight gradients", "side", wgrad))
         # number of leading steps that only need the batch and the conv weights (the part a look-ahead launch runs for the NEXT batch)
         self._n_fwd = 1 if self.direct_conv else 2
         carry = (self.label, self.label_cur) if self.lookahead else None
@@ -336,7 +349,9 @@ class HipsCNNTrainStep:
         forked = comm_forked = False
         steps = self._steps()
         nf = self._n_fwd
-        steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": steps[nf:] + steps[:nf]}[part]
+        # rotated: the next batch's forward convolutions overwrite a2, which the side branch (dense weight gradients) may still be reading
+        rotated = steps[nf:] + [(name, "join" if where == "main" else where, fn) for name, where, fn in steps[:nf]]
+        steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": rotated}[part]
         for i, (name, where, fn) in enumerate(steps):
             if stop_after is not None and i >= stop_after:
                 break

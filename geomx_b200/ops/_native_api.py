@@ -91,16 +91,41 @@ def gemm_pool(A, B, pooled, idx, OH, OW, bias=None, relu=True, a_mn=False, b_mn=
 
 
 def mlp_chain(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dw0, db0, dw1, db1, dw2, db2, dx):
-    """Dense(D1,relu) -> Dense(D2,relu) -> Dense(C) -> softmax-CE, forward and backward, in ONE cluster launch (csrc/kernels/mlp_chain.cu).
+    """Dense(D1,relu) -> Dense(D2,relu) -> Dense(C) -> softmax-CE, forward and backward (csrc/kernels/mlp_chain.cu): the cluster launch of
+    :func:`mlp_chain_data`, then :func:`dense_wgrad`, both on the current stream, with scratch tensors of their own.
     Returns False when the shapes are not the compiled 512 -> 256 -> 128 -> C<=16, batch <= 32 (callers then use the per-layer kernels)."""
+    B = x.shape[0]
+    e = lambda *s: torch.empty(*s, dtype=torch.float32, device=x.device)
+    a3, a4, dz4, dz3, dl = e(B, w0.shape[0]), e(B, w1.shape[0]), e(B, w1.shape[0]), e(B, w0.shape[0]), e(B, 16)
+    if not mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, dz4, dz3, dl):
+        return False
+    dense_wgrad(x, a3, a4, dz4, dz3, dl, dw0, db0, dw1, db1, dw2, db2)
+    return True
+
+
+def mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, dz4, dz3, dl):
+    """The data path of the dense chain in ONE cluster launch: per-sample loss, logits and dx; it also stores what :func:`dense_wgrad` reads:
+    a3 [B,D1], a4 [B,D2], dz4 [B,D2], dz3 [B,D1] and the dlogits dl [B,16].  Returns False for shapes other than 512 -> 256 -> 128 -> C<=16,
+    batch <= 32."""
     B, D0 = x.shape
     D1, D2, C = w0.shape[0], w1.shape[0], w2.shape[0]
-    rc = _lib().gx_mlp_chain_fwd_bwd(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dw0), _p(db0),
-                                     _p(dw1), _p(db1), _p(dw2), _p(db2), _p(dx), B, D0, D1, D2, C, _s())
+    rc = _lib().gx_mlp_chain(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dx),
+                             _p(a3), _p(a4), _p(dz4), _p(dz3), _p(dl), B, D0, D1, D2, C, _s())
     if rc == -1:
         return False
     _ck(rc, "mlp_chain")
     return True
+
+
+def dense_wgrad(x, a3, a4, dz4, dz3, dl, dw0, db0, dw1, db1, dw2, db2):
+    """The dense chain's weight and bias gradients (overwritten) from what :func:`mlp_chain_data` stored: dW0 = dz3ᵀ·x, dW1 = dz4ᵀ·a3,
+    dW2 = dlᵀ·a4 and their column sums, one launch."""
+    B, D0 = x.shape
+    D1, D2, C = a3.shape[1], a4.shape[1], dw2.shape[0]
+    assert dl.shape == (B, 16) and all(t.shape[0] == B for t in (a3, a4, dz4, dz3))
+    rc = _lib().gx_dense_wgrad(_p(x), _p(a3), _p(a4), _p(dz4), _p(dz3), _p(dl), _p(dw0), _p(db0), _p(dw1), _p(db1), _p(dw2), _p(db2),
+                               B, D0, D1, D2, C, _s())
+    _ck(rc, "dense_wgrad")
 
 
 # --------------------------------------------------------------------------------------------------------------- demo-CNN direct convolutions

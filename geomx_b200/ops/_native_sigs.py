@@ -7,7 +7,8 @@ SIGS = {
     # gemm_wgmma.cu
     "gx_gemm_tf32": [P, L, I, P, L, I, I, I, I, P, L, P, P, L, P, I, I, I, I, F, I, P],
     "gx_gemm_tf32_pool": [P, L, I, P, L, I, I, I, I, P, P, I, I, I, P, F, P],
-    "gx_mlp_chain_fwd_bwd": [P] * 17 + [I] * 5 + [P],
+    "gx_mlp_chain": [P] * 16 + [I] * 5 + [P],
+    "gx_dense_wgrad": [P] * 12 + [I] * 5 + [P],
     "gx_cnn_fwd": [P] * 11 + [I, P, I, P],
     "gx_cnn_bwd": [P] * 9 + [I, P],
     "gx_cnn_wgrad1": [P] * 6 + [I, P],

@@ -1,6 +1,6 @@
 """Per-kernel cost of the flagship step (1 GPU): every launch of HipsCNNTrainStep is captured alone, REP times back to back, in a CUDA graph
 (PDL edges, L2 warm) and timed with CUDA events -> steady-state us per launch; plus in-kernel %globaltimer phase stamps of the fused MLP
-cluster kernel and of the conv1 wgmma GEMM.  Usage: python tools/kernel_times.py [--fast]"""
+cluster kernel, of the dense weight-gradient kernel behind it and of the conv1 wgmma GEMM.  Usage: python tools/kernel_times.py [--fast]"""
 import ctypes
 import os
 import sys
@@ -48,10 +48,10 @@ if eng.fused_mlp:
         eng._body(); torch.cuda.synchronize()
         st = dbg.cpu().tolist()
         print("mlp chain phases (us since kernel start): 0 start|1 prologue issued|2 pdl wait done|3 inputs landed+sync|4 a3 landed|5 a4 landed|"
-              "6 dz4 computed|7 dz3 pushed|8 dz3 landed|9 end of warp-group 0:",
+              "6 dz4 computed|7 dz3 pushed|8 dz3 landed|9 end (da2 stored):",
               ["%.2f" % ((v - st[0]) / 1e3) for v in st[:10]], "| P1: 10 products done|11 partials synced|12 W0 prefetch issued|13 a3 pushed:",
-              ["%.2f" % ((v - st[0]) / 1e3) for v in st[10:14]], "| P5: 14 da2 products done|15 dW0/db0 done (warp-group 1):",
-              ["%.2f" % ((v - st[0]) / 1e3) for v in st[14:16]])
+              ["%.2f" % ((v - st[0]) / 1e3) for v in st[10:14]], "| P5: 14 da2 products done:", "%.2f" % ((st[14] - st[0]) / 1e3),
+              "| dense_wgrad: 16 start|17 dependency resolved|18 last CTA done:", ["%.2f" % ((v - st[0]) / 1e3) for v in st[16:19]])
     lib.gx_mlp_chain_set_debug(ctypes.c_void_p(0))
 if eng.direct_conv:
     dbg = torch.zeros(1024, dtype=torch.int64, device="cuda")

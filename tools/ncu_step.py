@@ -1,6 +1,6 @@
 """Driver for `ncu --set full`: a few EAGER flagship steps (one launch per kernel, no CUDA graph) so that every kernel of the step can be
-captured on its own.  Launch order per step: cnn_fwd, mlp_chain, dense-key channel, cnn_bwd_all, conv-key channel (5 launches; with
-GEOMX_FUSED_EXCHANGE=1: 4).  Then one BatchNorm forward/backward and the large GEMM in both precisions.
+captured on its own.  Launch order per step: cnn_fwd, mlp_chain, dense_wgrad, dense-key channel, cnn_bwd_all, conv-key channel
+(6 launches; with GEOMX_FUSED_EXCHANGE=1: 5).  Then one BatchNorm forward/backward and the large GEMM in both precisions.
 
   ncu --set full --clock-control none --import-source on --launch-skip 15 --launch-count 9 -o gpurun_out/r2_step python tools/ncu_step.py
 """

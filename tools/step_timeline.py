@@ -25,10 +25,10 @@ CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
                     "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
                     "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
 # the same for the dense-chain cluster kernel (gx_mlp_chain_set_debug slots of cluster CTA 0): 0 start | 3 inputs landed | 4 a3 landed |
-# 5 a4 landed | 6 dz4 computed | 7 dz3 pushed | 8 dz3 landed | 9 end of warp-group 0 (da2) | 15 end of warp-group 1 (dW0 / db0)
+# 5 a4 landed | 6 dz4 computed | 7 dz3 pushed | 8 dz3 landed | 9 end (da2 stored); and of the dense weight-gradient kernel: 16 start of its
+# CTA 0 | 17 its grid dependency resolved | 18 end of its last CTA
 MLP_PHASES = (0, 3, 4, 5, 6, 7, 8, 9)
 MLP_PHASE_LABELS = ("staging+pdl-wait", "dense0 -> a3", "dense1 -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
-MLP_END = (9, 15)
 
 
 def main():
@@ -66,8 +66,9 @@ def main():
         torch.cuda.synchronize()
         c, m = cdbg.tolist(), mdbg.tolist()
         st = {k: fab.state[k][8:8 + 12].view(torch.int64).tolist() for k in chans}
-        mlp_end = max(m[s] for s in MLP_END)            # whichever warp-group finishes last
-        row = {"cnn_fwd": (c[0], c[4]), "mlp_chain": (m[0], mlp_end), "cnn_bwd": (c[8], c[13]), "cnn_wgrad1": (c[16], c[18])}
+        row = {"cnn_fwd": (c[0], c[4]), "mlp_chain": (m[0], m[9]), "cnn_bwd": (c[8], c[13]), "cnn_wgrad1": (c[16], c[18])}
+        if m[16] > 0:
+            row["dense_wgrad"] = (m[17], m[18])         # from its grid dependency (the cluster kernel's end) to its last CTA
         for k in chans:
             if st[k][0] > 0:
                 row["chan:" + k] = (st[k][0], st[k][5])
@@ -80,7 +81,9 @@ def main():
         row["_ms"] = ev[0].elapsed_time(ev[1])
         row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in CNN_PHASES.items()}
         row["_mlp_ph"] = [(m[s1] - m[s0]) / 1e3 for s0, s1 in zip(MLP_PHASES, MLP_PHASES[1:])]
-        row["_mlp_wg1"] = (m[15] - m[9]) / 1e3 if m[15] > 0 else float("nan")
+        if "chan:dense" in row and "chan:conv" in row:
+            # the dense branch (weight gradients + dense channel) must end before the conv-key exchange does, or it is exposed
+            row["_dense_vs_conv"] = (row["chan:dense"][1] - row["chan:conv"][1]) / 1e3
         row["_ph"] = {k: [(v - st[k][0]) / 1e3 for v in st[k][:6]] for k in chans if st[k][0] > 0}
         rows.append(row)
     rows = rows[4:]
@@ -115,8 +118,10 @@ def main():
         lines.append("  %s phases of CTA 0 (us): %s" % (name, "  ".join("%s %.2f" % (lab, statistics.median(r["_cnn_ph"][name][i] for r in rows))
                                                                       for i, lab in enumerate(labels))))
     lines.append("  mlp_chain phases of CTA 0 (us): %s" % "  ".join("%s %.2f" % (lab, statistics.median(r["_mlp_ph"][i] for r in rows))
-                                                                    for i, lab in enumerate(MLP_PHASE_LABELS)) +
-                 "  | warp-group 1 (dW0) ends %.2f after warp-group 0" % statistics.median(r["_mlp_wg1"] for r in rows))
+                                                                    for i, lab in enumerate(MLP_PHASE_LABELS)))
+    if "_dense_vs_conv" in rows[0]:
+        d = statistics.median(r["_dense_vs_conv"] for r in rows)
+        lines.append("  dense branch (weight gradients + dense channel) ends %.2f us %s the end of the conv-key exchange" % (abs(d), "after" if d > 0 else "before"))
     if "_tail" in rows[0]:
         lines.append("  bwd tail (us since first tail ticket): ticket|grid done|sent|received|end %s" % ["%.2f" % statistics.median(r["_tail"][i] for r in rows) for i in range(5)])
     for k in rows[0]["_ph"]:
