@@ -3,6 +3,8 @@
 // forward and backward, TWO launches in total:
 //   cnn_fwd_kernel      x -> a1 (+argmax) -> a2 (+argmax)          both convolutions, bias, ReLU and both max-pools; one 4-CTA cluster per
 //                       image: each CTA computes a quarter of conv0 and shares it through distributed shared memory, so conv0 runs once
+//                       (cnn_fwd_dense0_kernel, even batches <= 32: the same, in clusters of two images, followed by the first dense
+//                       layer a2 -> a3, so that the dense-chain cluster kernel starts from a3)
 //   cnn_bwd_all_kernel  one heterogeneous grid: CTAs [128, 128+4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1 data gradient gathered
 //                       from the non-zeros of dz2 + pool/ReLU backward of both layers + conv0 weight gradient), CTAs [0, 128)  da2, a1 -> dW1, db1
 //                       (conv1 weight gradient); both exploit the sparsity of dz2 (one non-zero per pooling window).  Both bodies resolve
@@ -83,29 +85,36 @@ __device__ __forceinline__ float pool4(const float (&a)[4], float bias, int& bi)
 }
 
 // ------------------------------------------------------------------------------------------------------------------ forward
-// grid (B, 4), 256 threads, clusters of (1, 4, 1): the four CTAs of image b.  CTA (b, g) computes conv0 channels [4g, 4g+4) and stores them
-// into the conv0 map of all four CTAs of its cluster (distributed shared memory), then conv1 for output channels [8g, 8g+8) over all 16.
-__global__ void __cluster_dims__(1, 4, 1) __launch_bounds__(256)
-    cnn_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
-                   const float* __restrict__ b1, float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
-                   unsigned char* __restrict__ idx2, const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n,
-                   float* __restrict__ x_keep, unsigned long long* dbg) {
-  __shared__ __align__(16) float sx[CD_H * CD_H];
-  __shared__ __align__(16) float sw0[4 * CD_W1PAD];
-  __shared__ float sb0[4];
-  __shared__ __align__(16) float sa1[CD_C1 * CD_P1 * CD_P1];
-  __shared__ __align__(16) float sw1[8 * CD_C1 * CD_W1PAD];
-  __shared__ float sb1[8];
-  __shared__ __align__(16) float spart[4 * 64 * 8];
+struct CnnFwdSmem {
+  __align__(16) float sx[CD_H * CD_H];
+  __align__(16) float sw0[4 * CD_W1PAD];
+  float sb0[4];
+  __align__(16) float sa1[CD_C1 * CD_P1 * CD_P1];
+  __align__(16) float sw1[8 * CD_C1 * CD_W1PAD];
+  float sb1[8];
+  __align__(16) float spart[4 * 64 * 8];
+};
+
+// Both convolutions of image b in CTA g of its four, IMGS images per cluster (the four CTAs of image b are cluster ranks bl + IMGS r,
+// bl = b % IMGS).  CTA (b, g) computes conv0 channels [4g, 4g+4) and stores them into the conv0 map of all four CTAs of its image
+// (distributed shared memory), then conv1 for output channels [8g, 8g+8) over all 16.  Returns, in threads tid < 128, the pooled conv1
+// value that thread stored to a2 and its offset within the image's 512 (channel * 16 + window).  The kernel arms whatever its cluster
+// needs before this body's start-up cluster barrier.
+template <int IMGS>
+__device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __restrict__ x, const float* __restrict__ w0,
+                                               const float* __restrict__ b0, const float* __restrict__ w1, const float* __restrict__ b1,
+                                               float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
+                                               unsigned char* __restrict__ idx2, const float* __restrict__ carry_src, float* __restrict__ carry_dst,
+                                               int carry_n, float* __restrict__ x_keep, unsigned long long* dbg, int& a2_off) {
+  float* sx = s.sx; float* sw0 = s.sw0; float* sb0 = s.sb0; float* sa1 = s.sa1; float* sw1 = s.sw1; float* sb1 = s.sb1; float* spart = s.spart;
   cg::cluster_group cluster = cg::this_cluster();
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
-  stamp(0);
   // the conv0 stores below go into the other CTAs' shared memory, which must exist by then: arrive now, wait after the staging
   cluster.barrier_arrive();
   pdl_wait();
   pdl_launch();
-  const int b = blockIdx.x, g = blockIdx.y, tid = threadIdx.x;     // g == cluster.block_rank()
+  const int b = blockIdx.x, g = blockIdx.y, tid = threadIdx.x, bl = b % IMGS;     // g == the image's rank among its four CTAs
   // look-ahead steps: this launch is the tail of the previous batch's step; it hands the labels that arrived with its image batch over to
   // the buffer the classifier head of the NEXT launch reads (a 128-byte side job instead of a copy node in the step graph)
   if (carry_n > 0 && b == 0 && g == 0) for (int i = tid; i < carry_n; i += 256) carry_dst[i] = carry_src[i];
@@ -142,7 +151,7 @@ __global__ void __cluster_dims__(1, 4, 1) __launch_bounds__(256)
       int bi;
       const float v = pool4(acc, bias, bi);
 #pragma unroll
-      for (int r = 0; r < 4; ++r) cluster.map_shared_rank(sa1, r)[ch * CD_P1 * CD_P1 + win] = v;
+      for (int r = 0; r < 4; ++r) cluster.map_shared_rank(sa1, r * IMGS + bl)[ch * CD_P1 * CD_P1 + win] = v;
       const long long o = ((long long)b * CD_C1 + ch) * (CD_P1 * CD_P1) + win;
       a1[o] = v; idx1[o] = (unsigned char)bi;
     }
@@ -169,20 +178,122 @@ __global__ void __cluster_dims__(1, 4, 1) __launch_bounds__(256)
   }
   __syncthreads();
   stamp(3);
+  float v = 0.f;
+  a2_off = 0;
   if (tid < 128) {
     const int i64 = tid >> 1, which = tid & 1, op = i64 >> 4, win = i64 & 15, ol = 2 * op + which;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
     for (int cq = 0; cq < 4; ++cq) {
-      const float4 v = *reinterpret_cast<const float4*>(spart + (cq * 64 + i64) * 8 + which * 4);
-      acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w;
+      const float4 t = *reinterpret_cast<const float4*>(spart + (cq * 64 + i64) * 8 + which * 4);
+      acc[0] += t.x; acc[1] += t.y; acc[2] += t.z; acc[3] += t.w;
     }
     int bi;
-    const float v = pool4(acc, sb1[ol], bi);
-    const long long o = ((long long)b * CD_C2 + 8 * g + ol) * (CD_P2 * CD_P2) + win;
+    v = pool4(acc, sb1[ol], bi);
+    a2_off = (8 * g + ol) * (CD_P2 * CD_P2) + win;
+    const long long o = (long long)b * CD_C2 * (CD_P2 * CD_P2) + a2_off;
     a2[o] = v; idx2[o] = (unsigned char)bi;
   }
+  return v;
+}
+
+// grid (B, 4), 256 threads, clusters of (1, 4, 1): the four CTAs of image b
+__global__ void __cluster_dims__(1, 4, 1) __launch_bounds__(256)
+    cnn_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                   const float* __restrict__ b1, float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
+                   unsigned char* __restrict__ idx2, const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n,
+                   float* __restrict__ x_keep, unsigned long long* dbg) {
+  __shared__ CnnFwdSmem s;
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  stamp(0);
+  int a2_off;
+  cnn_fwd_convs<1>(s, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
   stamp(4);
+}
+
+// ---- the same convolutions, followed by the first dense layer of the head: a3 = relu(a2 Wd^T + bd), Wd [256][512].  dense0 is
+// row-separable (a3[b] needs only a2[b]), so it runs on the forward grid instead of the 16 SMs of the dense-chain cluster.
+// grid (B, 4), B even, 256 threads, clusters of (2, 4, 1): the four CTAs of images b0 and b0 + 1 (b0 even; conv0 is shared within each
+// image's four).  After the conv1 epilogue every CTA pushes its 128 a2 values (st.async, transaction mbarrier) into the a2 buffer of all 8
+// CTAs; cluster rank r then computes a3[b0 .. b0+1][32 r .. 32 r + 32]: 8 threads per output column, each over every 8th float4 of the
+// column's W0 row (its K-segment; 8 neighbouring lanes read 128 contiguous bytes of the row, and distinct 16-byte chunks of a2 in shared
+// memory), every W0 load used for both images; the 8 partials are summed in a fixed shuffle order.
+struct CnnFwdDense0Smem {
+  CnnFwdSmem conv;
+  __align__(16) float a2[2 * CD_C2 * CD_P2 * CD_P2];   // both images' a2, as pushed by the 8 CTAs
+  uint64_t bar_a2;
+};
+static_assert(sizeof(CnnFwdDense0Smem) == CNN_FWD_DENSE0_SMEM_BYTES, "CNN_FWD_DENSE0_SMEM_BYTES (common.cuh) must match");
+constexpr int CD_D1 = 256, CD_D0 = CD_C2 * CD_P2 * CD_P2;    // dense0: 512 -> 256
+
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
+    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
+                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
+                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
+                          unsigned long long* dbg) {
+  __shared__ CnnFwdDense0Smem s;
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  stamp(0);
+  if (threadIdx.x == 0) {
+    // the a2 buffer expects all 1024 floats; the peers push only after the body's start-up cluster barrier, so it is armed in time
+    mbar_init(&s.bar_a2, 1);
+    mbar_arrive_expect_tx(&s.bar_a2, 2 * CD_D0 * 4);
+    fence_barrier_init();
+    // W0 into L2 now: it is read at the very end of the kernel, and the step may start with L2 cold.  The first cluster prefetches it (each
+    // CTA its 64 KB, rows 32 r .. 32 r + 31) and every cluster reads it from L2.  (Every cluster prefetching its own copy was measured
+    // 0.4 us slower per step: 8 MiB of prefetch traffic at B = 32 slowed the staging of the images.)
+    if (blockIdx.x < 2) {
+      const float* slice = wd + (long long)32 * cg::this_cluster().block_rank() * CD_D0;
+      for (int k = 0; k < 4; ++k)
+        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(slice + k * 8 * CD_D0), "r"(8 * CD_D0 * 4) : "memory");
+    }
+  }
+  int a2_off;
+  const float v = cnn_fwd_convs<2>(s.conv, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
+  // (computed after the convolutions, which need every register they can get)
+  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), bl = blockIdx.x & 1, bpair = blockIdx.x - bl;
+  const float* wrow = wd + (long long)(32 * cr + (tid >> 3)) * CD_D0;   // the W0 row of this thread's output column
+  // ---- a2 hand-off: lane 2 win + which holds window win of channel 8g + 2 op + which (op = warp); lanes 8k + which + {0, 2, 4, 6} hold
+  // windows 4k .. 4k + 3 of one channel, gathered into one float4 push
+  if (tid < 128) {
+    const float v1 = __shfl_down_sync(0xffffffffu, v, 2), v2 = __shfl_down_sync(0xffffffffu, v, 4), v3 = __shfl_down_sync(0xffffffffu, v, 6);
+    if ((tid & 6) == 0) push_all<8>(s.a2, bl * CD_D0 + a2_off, &s.bar_a2, cr, make_float4(v, v1, v2, v3));
+  }
+  // ---- dense0: thread -> column n = 32 r + tid / 8, K-segment j = tid % 8: float4 chunks j, j + 8, ... of the row (k = 32 q + 4 j)
+  const int j = tid & 7;
+  const float bias = __ldg(bd + 32 * cr + (tid >> 3));
+  constexpr int NB = 8;   // float4 of W0 in flight per thread: two batches cover the row segment (16 float4), in 32 of the 64 registers
+  float4 w[NB];
+#pragma unroll
+  for (int i = 0; i < NB; ++i) w[i] = __ldg(reinterpret_cast<const float4*>(wrow) + 8 * i + j);   // first batch: in flight while a2 lands
+  wait_landed(&s.bar_a2);
+  stamp(5);
+  float acc0 = 0.f, acc1 = 0.f;
+#pragma unroll 1
+  for (int q0 = 0; q0 < CD_D0 / 32; q0 += NB) {
+    if (q0 > 0) {
+#pragma unroll
+      for (int i = 0; i < NB; ++i) w[i] = __ldg(reinterpret_cast<const float4*>(wrow) + 8 * (q0 + i) + j);
+    }
+#pragma unroll
+    for (int i = 0; i < NB; ++i) {
+      const float4 x0 = reinterpret_cast<const float4*>(s.a2)[8 * (q0 + i) + j];
+      const float4 x1 = reinterpret_cast<const float4*>(s.a2 + CD_D0)[8 * (q0 + i) + j];
+      acc0 = fmaf(w[i].x, x0.x, acc0); acc0 = fmaf(w[i].y, x0.y, acc0); acc0 = fmaf(w[i].z, x0.z, acc0); acc0 = fmaf(w[i].w, x0.w, acc0);
+      acc1 = fmaf(w[i].x, x1.x, acc1); acc1 = fmaf(w[i].y, x1.y, acc1); acc1 = fmaf(w[i].z, x1.z, acc1); acc1 = fmaf(w[i].w, x1.w, acc1);
+    }
+  }
+#pragma unroll
+  for (int o = 4; o > 0; o >>= 1) {
+    acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
+    acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
+  }
+  if (j < 2) a3[(long long)(bpair + j) * CD_D1 + 32 * cr + (tid >> 3)] = fmaxf((j == 0 ? acc0 : acc1) + bias, 0.f);
+  stamp(6);
+  stamp(4);      // (slot 4 stays the end of the forward kernel)
 }
 
 // ------------------------------------------------------------------------------------------------------------------ backward (data + conv0)
@@ -522,7 +633,7 @@ __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, c
 
 using namespace gx;
 
-static unsigned long long* g_cnn_dbg = nullptr;      // optional %globaltimer stamps of CTA (0,0): fwd 0-4, bwd 8-13, wgrad1 16-18
+static unsigned long long* g_cnn_dbg = nullptr;      // optional %globaltimer stamps of CTA (0,0): fwd 0-6, bwd 8-13, wgrad1 16-18
 GX_API int gx_cnn_set_debug(unsigned long long* p) { g_cnn_dbg = p; return 0; }
 
 // x [B,1,28,28]; w0 [16,1,5,5]; w1 [32,16,5,5]; writes a1 [B,16,12,12] + idx1, a2 [B,32,4,4] + idx2
@@ -530,6 +641,16 @@ GX_API int gx_cnn_fwd(const float* x, const float* w0, const float* b0, const fl
                       unsigned char* idx2, const float* carry_src, float* carry_dst, int carry_n, float* x_keep, int B, cudaStream_t s) {
   if (B < 1) return 0;
   launch_pdl(cnn_fwd_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, g_cnn_dbg);
+  return GX_CHECK_LAUNCH();
+}
+// the same, plus the first dense layer: a3 [B,256] = relu(a2 [B,512] · wd [256,512]^T + bd).  Only for even B <= 32 (clusters of two images);
+// returns -1 without launching otherwise.
+GX_API int gx_cnn_fwd_dense0(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* wd, const float* bd,
+                             float* a1, unsigned char* idx1, float* a2, unsigned char* idx2, float* a3, const float* carry_src, float* carry_dst,
+                             int carry_n, float* x_keep, int B, cudaStream_t s) {
+  if (B < 2 || (B & 1) || B > 32) return -1;
+  launch_pdl(cnn_fwd_dense0_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n,
+             x_keep, g_cnn_dbg);
   return GX_CHECK_LAUNCH();
 }
 // accumulates into dw0 [16,25] / db0 [16] (atomics: zero them first)

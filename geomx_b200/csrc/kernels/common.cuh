@@ -110,6 +110,42 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ------------------------------------------------------------------------------------------------ point-to-point cluster hand-offs
+// A producer pushes its slice into the receive buffer of every CTA of the cluster with st.async; each store completes its bytes on a
+// transaction mbarrier in the receiving CTA, which waits on its own barrier only (no cluster-wide barrier, no GPU-scope fence).
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, int rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(local_smem_addr), "r"(rank));
+  return a;
+}
+// push v to float offset o of `buf` in the N CTAs of the cluster that follow rank cr (N = CS: every CTA including this one, this one last;
+// N = CS - 1: the peers only), so that the CTAs do not all hit rank 0 first; each store completes 16 bytes on the receiver's barrier `bar`
+template <int CS, int N = CS>
+__device__ __forceinline__ void push_all(const float* buf, int o, uint64_t* bar, int cr, float4 v) {
+  const uint32_t a = smem_u32(buf + o), m = smem_u32(bar);
+#pragma unroll 4   // a full unroll hoists all 2 N remote addresses and pushes mlp_chain_kernel past 96 registers (co-residency with cnn_fwd)
+  for (int i = 0; i < N; ++i) {
+    const int r = (cr + 1 + i) & (CS - 1);
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];"
+                 ::"r"(mapa_u32(a, r)), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(mapa_u32(m, r)) : "memory");
+  }
+}
+// wait until every byte announced on this CTA's (single-use) barrier has landed.  The acquire that makes the peers' stores visible is
+// restricted to shared::cluster memory: a plain acquire.cluster wait would also invalidate L1, for no data the kernels read through it.
+__device__ __forceinline__ void wait_landed(uint64_t* bar) {
+  asm volatile(
+      "{\n\t.reg .pred P1;\n\t"
+      "WAIT_LANDED:\n\t"
+      "mbarrier.try_wait.parity.relaxed.cluster.shared::cta.b64 P1, [%0], 0;\n\t"
+      "@!P1 bra WAIT_LANDED;\n\t}\n"
+      "fence.acquire.sync_restrict::shared::cluster.cluster;" ::"r"(smem_u32(bar))
+      : "memory");
+}
+
+// Static shared memory of cnn_fwd_dense0_kernel (cnn_direct.cu asserts it).  Its successor in the step, dense_tail_kernel (mlp_chain.cu),
+// stages its weights while the forward kernel runs, on the SMs beside its CTAs: mlp_chain.cu checks that both fit into one SM.
+constexpr int CNN_FWD_DENSE0_SMEM_BYTES = 39488;
+
 // ------------------------------------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");

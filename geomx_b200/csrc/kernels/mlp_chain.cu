@@ -23,6 +23,9 @@
 // cluster kernel stores what they need (a3, a4, dz4, dz3, dlogits; about 50 KB) and the weight-gradient kernel turns them into dW0 / dW1 /
 // dW2 and the bias gradients.  Two launches replace what used to be seven (dense0, dense1, head, dW1, dz3, dW0, da2); tools/kernel_times.py
 // times the chain with per-phase %globaltimer stamps.
+// dense0 is row-separable (a3[b] needs only the pooled conv output of image b), so where the direct forward kernel runs (even batches <= 32)
+// it computes a3 on its 128 SMs (cnn_fwd_dense0_kernel, cnn_direct.cu) and the cluster kernel is dense_tail_kernel: the same chain from a3
+// on, through the same body (dense_chain_body), with no x tile, no dense0 phase and no a3 hand-off.
 //
 // Shapes are compile-time (D0 -> D1 -> D2 -> C<=16, batch <= 32): the demo CNN's 512 -> 256 -> 128 -> 10.  Other shapes use the wgmma GEMMs.
 #include <cooperative_groups.h>
@@ -48,6 +51,7 @@ struct MlpChainParams {
   float* logits;        // [B][C] or nullptr
   float* dx;            // [B][D0]   gradient w.r.t. x
   // what the weight gradients need (rows b < B): a3 [B][D1], a4 [B][D2], dz4 [B][D2], dz3 [B][D1], dlogits [B][16] (classes >= C zero)
+  // (dense_tail_kernel: a3 is its input, x and b0 are unused)
   float* a3; float* a4; float* dz4; float* dz3; float* dl;
   int B, C;
   unsigned long long* dbg;   // optional %globaltimer stamps of cluster CTA 0 (tools/kernel_times.py)
@@ -64,36 +68,7 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// ---- point-to-point hand-offs between the CTAs of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, int rank) {
-  uint32_t a;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(local_smem_addr), "r"(rank));
-  return a;
-}
-// push v to float offset o of `buf` in the N CTAs of the cluster that follow rank cr (N = CS: every CTA including this one, this one last;
-// N = CS - 1: the peers only), so that the CTAs do not all hit rank 0 first; each store completes 16 bytes on the receiver's barrier `bar`
-template <int CS, int N = CS>
-__device__ __forceinline__ void push_all(const float* buf, int o, uint64_t* bar, int cr, float4 v) {
-  const uint32_t a = smem_u32(buf + o), m = smem_u32(bar);
-#pragma unroll 4   // a full unroll hoists all 2 N remote addresses and pushes the kernel past 96 registers (co-residency with cnn_fwd)
-  for (int i = 0; i < N; ++i) {
-    const int r = (cr + 1 + i) & (CS - 1);
-    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];"
-                 ::"r"(mapa_u32(a, r)), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(mapa_u32(m, r)) : "memory");
-  }
-}
-// wait until every byte announced on this CTA's (single-use) barrier has landed.  The acquire that makes the peers' stores visible is
-// restricted to shared::cluster memory: a plain acquire.cluster wait would also invalidate L1 after every layer, for no data the kernel
-// reads through it.
-__device__ __forceinline__ void wait_landed(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "WAIT_LANDED:\n\t"
-      "mbarrier.try_wait.parity.relaxed.cluster.shared::cta.b64 P1, [%0], 0;\n\t"
-      "@!P1 bra WAIT_LANDED;\n\t}\n"
-      "fence.acquire.sync_restrict::shared::cluster.cluster;" ::"r"(smem_u32(bar))
-      : "memory");
-}
+// (the point-to-point hand-offs between the CTAs of the cluster, push_all / wait_landed, are in common.cuh)
 
 // stage `rows` x K floats (global row stride ld) into a swizzled K-major tile
 __device__ __forceinline__ void stage_swizzled_async(float* dst, const float* src, int rows, int K, long long ld) {
@@ -204,11 +179,29 @@ __device__ __forceinline__ float colsum(const float* __restrict__ dz, int B, int
   return s;
 }
 
+// W2 as a swizzled K-major tile [16][D2] (rows >= C zero), b1 slice, b2 (classes >= C zero)
+template <int D2, int NS2>
+__device__ __forceinline__ void stage_head_async(float* sW2, float* sB1, float* sB2, const float* w2, const float* b1, const float* b2, int cr,
+                                                 int C) {
+  const int tid = threadIdx.x;
+  for (int c = tid; c < MC_CMAX * (D2 >> 2); c += MC_THREADS) {
+    const int r = c / (D2 >> 2), q = c - r * (D2 >> 2);
+    float* dst = sW2 + sw_off(r, q << 2, D2);
+    if (r < C) cp_async16(dst, w2 + (long long)r * D2 + (q << 2));
+    else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (tid < NS2) sB1[tid] = b1[cr * NS2 + tid];
+  if (tid < 16) sB2[tid] = tid < C ? b2[tid] : 0.f;
+}
+
+// Shared-memory layout of mlp_chain_kernel (starts from x and computes dense0 itself).  Both kernels name the same buffers (W0, W1, A3, A4,
+// DZ4, W2, DL, MISC, A3OWN, SCRATCH, BAR) so that dense_chain_body serves both.
 template <int D0, int D1, int D2, int CS>
 struct MlpSmem {
   static constexpr int NS1 = D1 / CS, NS2 = D2 / CS, KS0 = D0 / CS;
   // float offsets
   static constexpr int X = 0;                                  // [32][D0] swizzled  (dead after P1: P4 / P5 scratch)
+  static constexpr int SCRATCH = X, SCRATCH_SZ = MC_B * D0;
   static constexpr int W0 = X + MC_B * D0;                     // fwd: [NS1][D0] swizzled;  bwd: [D1][KS0] plain
   static constexpr int W0_SZ = (NS1 * D0 > D1 * KS0) ? NS1 * D0 : D1 * KS0;
   static constexpr int W1 = W0 + W0_SZ;                        // fwd: [NS2][D1] swizzled;  bwd: [D2][NS1] plain
@@ -226,112 +219,56 @@ struct MlpSmem {
   static constexpr int TOTAL = BAR + 3 * 2;
   static constexpr int BYTES = TOTAL * 4;
 };
-
-// CS = CTAs per cluster: 8 (portable) or 16 (non-portable size, one GPC): every layer is cut into CS column slices
+// Shared-memory layout of dense_tail_kernel (starts from a3, which the forward kernel computed): no x tile, W0 only as the column slice of
+// the backward pass, and a scratch of its own for the P4 / P5 partials.  The A3 buffer is staged from global memory and later receives dz3,
+// the only hand-off into it (write-once as in MlpSmem: no peer can push dz3 before it holds this CTA's a4).
 template <int D0, int D1, int D2, int CS>
-__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_kernel(const MlpChainParams p) {
-  using L = MlpSmem<D0, D1, D2, CS>;
+struct TailSmem {
+  static constexpr int NS1 = D1 / CS, NS2 = D2 / CS, KS0 = D0 / CS;
+  static constexpr int W0 = 0;                                 // [D1][KS0] plain
+  static constexpr int W1 = W0 + D1 * KS0;                     // fwd: [NS2][D1] swizzled;  bwd: [D2][NS1] plain
+  static constexpr int W1_SZ = (NS2 * D1 > D2 * NS1) ? NS2 * D1 : D2 * NS1;
+  static constexpr int A3 = W1 + W1_SZ;                        // [32][D1] swizzled, rows >= B zero  (later: dz3)
+  static constexpr int A4 = A3 + MC_B * D1;                    // [32][D2] swizzled
+  static constexpr int DZ4 = A4 + MC_B * D2;                   // [32][D2] swizzled, computed locally  (earlier: P2 / logit scratch)
+  static constexpr int W2 = DZ4 + MC_B * D2;                   // [16][D2] swizzled, rows >= C zero
+  static constexpr int DL = W2 + MC_CMAX * D2;                 // [32][16] dlogits
+  static constexpr int MISC = DL + MC_B * MC_CMAX;             // (unused) [NS1] | b1 slice [NS2] | b2 [16] | label [32]
+  static constexpr int A3OWN = MISC + NS1 + NS2 + 16 + 32;     // [32][NS1] plain: this CTA's a3 columns (ReLU mask of dz3)
+  static constexpr int SCRATCH = A3OWN + MC_B * NS1;           // P4 / P5 partials
+  static constexpr int SCRATCH_SZ = (MC_THREADS / (2 * KS0)) * MC_B * KS0;
+  static constexpr int BAR = SCRATCH + SCRATCH_SZ;             // 2 mbarriers: a4, dz3 landed
+  static constexpr int TOTAL = BAR + 2 * 2;
+  static constexpr int BYTES = TOTAL * 4;
+};
+// the tail's CTAs stage their weights on the SMs beside the forward kernel's CTAs (one each: 256 x 64 + 512 x 96 = 65,536 registers), so
+// both kernels' shared memory, with the 1 KB the runtime reserves per CTA, has to fit into the SM's 228 KB
+static_assert(TailSmem<512, 256, 128, 16>::BYTES + CNN_FWD_DENSE0_SMEM_BYTES + 2048 <= 233472, "dense_tail_kernel fits beside cnn_fwd_dense0_kernel");
+
+// P2 .. P5 of the chain, the part both cluster kernels share: a4 = relu(a3 W1^T + b1) with the a4 hand-off, the classifier, softmax-CE and
+// the whole dz4, dz3 with its hand-off, and dx.  On entry the weights are staged (W0 as the column slice for dx still in flight, W1 as the
+// row slice), a3 is in the A3 buffer (FROM_X: as it lands from the peers) and in A3OWN (this CTA's columns), the labels and biases are
+// staged and the cluster has met once.  FROM_X (mlp_chain_kernel) also waits for a3 and stores this CTA's a3 columns.
+template <class L, int D0, int D1, int D2, int CS, bool FROM_X, class Stamp>
+__device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams& p, const int cr, uint64_t* bar_a3, uint64_t* bar_a4,
+                                                 uint64_t* bar_dz3, Stamp&& stamp) {
   constexpr int NS1 = L::NS1, NS2 = L::NS2, KS0 = L::KS0;
-  static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
-  static_assert(D0 % 64 == 0 && D1 % 64 == 0 && D2 % 64 == 0, "layer widths must be multiples of 64");
-  static_assert(NS1 % 8 == 0 && NS2 % 4 == 0 && KS0 % 4 == 0, "slices must hold whole register tiles");
   static_assert(MC_HALF % (2 * NS1) == 0 && MC_HALF % (2 * NS2) == 0 && MC_THREADS % (2 * KS0) == 0, "K splits");
-  static_assert(MC_THREADS / (2 * NS1) * MC_B * NS1 <= 2 * MC_B * D2, "P1 scratch fits the a4 and dz4 buffers");
-  static_assert(MC_HALF / (2 * NS1) * MC_B * NS1 <= MC_B * D0 && MC_THREADS / (2 * KS0) * MC_B * KS0 <= MC_B * D0, "P4 / P5 scratch fits x");
+  static_assert(MC_HALF / (2 * NS1) * MC_B * NS1 <= L::SCRATCH_SZ && MC_THREADS / (2 * KS0) * MC_B * KS0 <= L::SCRATCH_SZ, "P4 / P5 scratch");
   static_assert(MC_B * NS1 / 4 <= MC_HALF && MC_B * NS2 / 4 <= MC_HALF, "one thread per float4 of a3 / a4");
-  static_assert(L::BAR % 2 == 0, "mbarriers are 8-byte aligned");
-  extern __shared__ __align__(16) float sm[];
-  float* sX = sm + L::X; float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
+  float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
   float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL; float* sA3own = sm + L::A3OWN;
-  float* sB0 = sm + L::MISC; float* sB1 = sB0 + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + L::BAR);
-  uint64_t* bar_a3 = bar; uint64_t* bar_a4 = bar + 1; uint64_t* bar_dz3 = bar + 2;
-  cg::cluster_group cluster = cg::this_cluster();
-  const int cr = (int)cluster.block_rank();
+  float* sB1 = sm + L::MISC + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
   const int tid = threadIdx.x, lane = tid & 31;
   const int B = p.B, C = p.C;
-  // stamp by thread 0 of cluster CTA 0
-  auto stamp = [&](int slot) {
-    if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
-  };
-  stamp(0);
-
-  // ---------------- start-up: each receive barrier expects its whole buffer (dz3: all but this CTA's own columns, which are stored locally).
-  // The peers push into this CTA's shared memory only after the cluster barrier below, so the barriers are armed before any byte arrives.
-  if (tid == 0) {
-    for (int i = 0; i < 3; ++i) mbar_init(bar + i, 1);
-    mbar_arrive_expect_tx(bar_a3, MC_B * D1 * 4);
-    mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
-    mbar_arrive_expect_tx(bar_dz3, (CS - 1) * MC_B * NS1 * 4);
-    fence_barrier_init();      // (the release the peers need: nothing else this CTA wrote so far is read by them)
-  }
-  asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");   // waited for once the inputs are staged: the loads overlap the rendezvous
-
-  // ---------------- prologue: weights do not depend on the preceding kernel (they were written by the previous step's exchange, which a
-  // kernel further up the stream has already waited for) -> stage them before griddepcontrol.wait
-  stage_swizzled_async(sW0, p.w0 + (long long)cr * NS1 * D0, NS1, D0, D0);
-  stage_swizzled_async(sW1, p.w1 + (long long)cr * NS2 * D1, NS2, D1, D1);
-  for (int c = tid; c < MC_CMAX * (D2 >> 2); c += MC_THREADS) {
-    const int r = c / (D2 >> 2), q = c - r * (D2 >> 2);
-    float* dst = sW2 + sw_off(r, q << 2, D2);
-    if (r < C) cp_async16(dst, p.w2 + (long long)r * D2 + (q << 2));
-    else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (tid < NS1) sB0[tid] = p.b0[cr * NS1 + tid];
-  if (tid < NS2) sB1[tid] = p.b1[cr * NS2 + tid];
-  if (tid < 16) sB2[tid] = tid < C ? p.b2[tid] : 0.f;
-  cp_async_commit();
-  stamp(1);
-  pdl_wait();
-  pdl_launch();
-  stamp(2);
-  // input activations (full copy per CTA) + labels
-  for (int c = tid; c < MC_B * (D0 >> 2); c += MC_THREADS) {
-    const int r = c / (D0 >> 2), q = c - r * (D0 >> 2);
-    if (r < B) cp_async16(sX + sw_off(r, q << 2, D0), p.x + (long long)r * D0 + (q << 2));
-    else *reinterpret_cast<float4*>(sX + sw_off(r, q << 2, D0)) = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (tid < MC_B) sLab[tid] = tid < B ? p.label[tid] : 0.f;
-  cp_async_commit();
-  cp_async_wait<0>();
-  __syncthreads();
-  cluster.barrier_wait();   // every CTA of the cluster is running with its barriers armed (the pushes below target its shared memory)
-  stamp(3);
-
-  // tile coordinates shared by the 32-row products: 8 row groups x (NC/4) column groups per K split
-  // ---------------- P1: a3[:, slice] = relu(x * W0[slice]^T + b0)          NC = 32, K = D0, KS = 4
-  {
-    constexpr int PER = 2 * NS1, KS = MC_THREADS / PER;  // 8 row groups x NS1/4 column groups per split; K split over all 16 warps
-    const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
-    float acc[4][4] = {};
-    prod_nt<D0, KS>(sX, sW0, tb, tn, ks, acc);
-    stamp(10);
-    float* scratch = sA4;                                // [sA4 | sDZ4] = 32 KB contiguous, both unused until the end of P2 / P3
-    put_partial<NS1>(scratch, tb, tn, ks, acc);
-    __syncthreads();
-    // W0's row slice is no longer needed: start fetching the COLUMN slice W0[:, cr*KS0 ...] for the backward pass (da2) underneath P2..P4
-    stamp(11);
-    stage_plain_async(sW0, p.w0 + cr * KS0, D1, KS0, D0);
-    cp_async_commit();
-    stamp(12);
-    if (tid < MC_B * NS1 / 4) {
-      const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);   // 32 x NS1/4 float4 outputs
-      float4 v = sum_partials<NS1, KS>(scratch, b, n4);
-      v.x = fmaxf(v.x + sB0[4 * n4], 0.f); v.y = fmaxf(v.y + sB0[4 * n4 + 1], 0.f);
-      v.z = fmaxf(v.z + sB0[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB0[4 * n4 + 3], 0.f);
-      if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
-      *reinterpret_cast<float4*>(sA3own + b * NS1 + 4 * n4) = v;
-      // the pushed value depends on this thread's scratch reads, so no peer can write a4 into the scratch before they are done
-      push_all<CS>(sA3, sw_off(b, cr * NS1 + 4 * n4, D1), bar_a3, cr, v);
-    }
-    stamp(13);
-  }
   // ---------------- P2: a4[:, slice] = relu(a3 * W1[slice]^T + b1)         NC = 16, K = D1, KS = 8
   {
     constexpr int PER = 2 * NS2, KS = MC_HALF / PER;     // this layer is small: warp-group 0 only
     if (tid < MC_HALF) {
-      wait_landed(bar_a3);
-      stamp(4);
+      if (FROM_X) {
+        wait_landed(bar_a3);
+        stamp(4);
+      }
       const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
       float acc[4][4] = {};
       prod_nt<D1, KS>(sA3, sW1, tb, tn, ks, acc);
@@ -348,7 +285,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
       if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
       push_all<CS>(sA4, sw_off(b, cr * NS2 + 4 * n4, D2), bar_a4, cr, v);
       if (b < B) *reinterpret_cast<float4*>(p.a4 + b * D2 + cr * NS2 + 4 * n4) = v;
-    } else if (tid >= MC_HALF && tid - MC_HALF < MC_B * NS1 / 4) {
+    } else if (FROM_X && tid >= MC_HALF && tid - MC_HALF < MC_B * NS1 / 4) {
       // warp-group 1 is idle in P2: it stores this CTA's a3 columns for the weight-gradient kernel
       const int b = (tid - MC_HALF) / (NS1 / 4), n4 = (tid - MC_HALF) % (NS1 / 4);
       if (b < B) *reinterpret_cast<float4*>(p.a3 + b * D1 + cr * NS1 + 4 * n4) = *reinterpret_cast<const float4*>(sA3own + b * NS1 + 4 * n4);
@@ -439,7 +376,7 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
   // ---------------- P4: dz3[:, slice] = relu'(a3) * (dz4 * W1[:, slice])          NC = NS1, K = D2, split over warp-group 0
   // (split over all 16 warps, the deeper reduction made "dz3 pushed" slower: 2.4 us instead of 2.0)
   float* sDZ3 = sA3;
-  float* scratch = sX;                                   // x is dead after P1: P4 / P5 partials
+  float* scratch = sm + L::SCRATCH;                      // P4 / P5 partials
   {
     constexpr int PER = 2 * NS1, KS = MC_HALF / PER;
     if (tid < MC_HALF) {
@@ -479,6 +416,157 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
     }
   }
   stamp(9);
+}
+
+// CS = CTAs per cluster: 8 (portable) or 16 (non-portable size, one GPC): every layer is cut into CS column slices
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_kernel(const MlpChainParams p) {
+  using L = MlpSmem<D0, D1, D2, CS>;
+  constexpr int NS1 = L::NS1, NS2 = L::NS2;
+  static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
+  static_assert(D0 % 64 == 0 && D1 % 64 == 0 && D2 % 64 == 0, "layer widths must be multiples of 64");
+  static_assert(NS1 % 8 == 0 && NS2 % 4 == 0 && L::KS0 % 4 == 0, "slices must hold whole register tiles");
+  static_assert(MC_THREADS / (2 * NS1) * MC_B * NS1 <= 2 * MC_B * D2, "P1 scratch fits the a4 and dz4 buffers");
+  static_assert(L::BAR % 2 == 0, "mbarriers are 8-byte aligned");
+  extern __shared__ __align__(16) float sm[];
+  float* sX = sm + L::X; float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
+  float* sW2 = sm + L::W2; float* sA3own = sm + L::A3OWN;
+  float* sB0 = sm + L::MISC; float* sB1 = sB0 + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + L::BAR);
+  uint64_t* bar_a3 = bar; uint64_t* bar_a4 = bar + 1; uint64_t* bar_dz3 = bar + 2;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int cr = (int)cluster.block_rank();
+  const int tid = threadIdx.x;
+  const int B = p.B, C = p.C;
+  // stamp by thread 0 of cluster CTA 0
+  auto stamp = [&](int slot) {
+    if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
+  };
+  stamp(0);
+
+  // ---------------- start-up: each receive barrier expects its whole buffer (dz3: all but this CTA's own columns, which are stored locally).
+  // The peers push into this CTA's shared memory only after the cluster barrier below, so the barriers are armed before any byte arrives.
+  if (tid == 0) {
+    for (int i = 0; i < 3; ++i) mbar_init(bar + i, 1);
+    mbar_arrive_expect_tx(bar_a3, MC_B * D1 * 4);
+    mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
+    mbar_arrive_expect_tx(bar_dz3, (CS - 1) * MC_B * NS1 * 4);
+    fence_barrier_init();      // (the release the peers need: nothing else this CTA wrote so far is read by them)
+  }
+  asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");   // waited for once the inputs are staged: the loads overlap the rendezvous
+
+  // ---------------- prologue: weights do not depend on the preceding kernel (they were written by the previous step's exchange, which a
+  // kernel further up the stream has already waited for) -> stage them before griddepcontrol.wait
+  stage_swizzled_async(sW0, p.w0 + (long long)cr * NS1 * D0, NS1, D0, D0);
+  stage_swizzled_async(sW1, p.w1 + (long long)cr * NS2 * D1, NS2, D1, D1);
+  stage_head_async<D2, NS2>(sW2, sB1, sB2, p.w2, p.b1, p.b2, cr, C);
+  if (tid < NS1) sB0[tid] = p.b0[cr * NS1 + tid];
+  cp_async_commit();
+  stamp(1);
+  pdl_wait();
+  pdl_launch();
+  stamp(2);
+  // input activations (full copy per CTA) + labels
+  for (int c = tid; c < MC_B * (D0 >> 2); c += MC_THREADS) {
+    const int r = c / (D0 >> 2), q = c - r * (D0 >> 2);
+    if (r < B) cp_async16(sX + sw_off(r, q << 2, D0), p.x + (long long)r * D0 + (q << 2));
+    else *reinterpret_cast<float4*>(sX + sw_off(r, q << 2, D0)) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (tid < MC_B) sLab[tid] = tid < B ? p.label[tid] : 0.f;
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();
+  cluster.barrier_wait();   // every CTA of the cluster is running with its barriers armed (the pushes below target its shared memory)
+  stamp(3);
+
+  // tile coordinates shared by the 32-row products: 8 row groups x (NC/4) column groups per K split
+  // ---------------- P1: a3[:, slice] = relu(x * W0[slice]^T + b0)          NC = 32, K = D0, KS = 4
+  {
+    constexpr int PER = 2 * NS1, KS = MC_THREADS / PER;  // 8 row groups x NS1/4 column groups per split; K split over all 16 warps
+    const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
+    float acc[4][4] = {};
+    prod_nt<D0, KS>(sX, sW0, tb, tn, ks, acc);
+    stamp(10);
+    float* scratch = sA4;                                // [sA4 | sDZ4] = 32 KB contiguous, both unused until the end of P2 / P3
+    put_partial<NS1>(scratch, tb, tn, ks, acc);
+    __syncthreads();
+    // W0's row slice is no longer needed: start fetching the COLUMN slice W0[:, cr*KS0 ...] for the backward pass (da2) underneath P2..P4
+    stamp(11);
+    stage_plain_async(sW0, p.w0 + cr * L::KS0, D1, L::KS0, D0);
+    cp_async_commit();
+    stamp(12);
+    if (tid < MC_B * NS1 / 4) {
+      const int b = tid / (NS1 / 4), n4 = tid % (NS1 / 4);   // 32 x NS1/4 float4 outputs
+      float4 v = sum_partials<NS1, KS>(scratch, b, n4);
+      v.x = fmaxf(v.x + sB0[4 * n4], 0.f); v.y = fmaxf(v.y + sB0[4 * n4 + 1], 0.f);
+      v.z = fmaxf(v.z + sB0[4 * n4 + 2], 0.f); v.w = fmaxf(v.w + sB0[4 * n4 + 3], 0.f);
+      if (b >= B) v = make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(sA3own + b * NS1 + 4 * n4) = v;
+      // the pushed value depends on this thread's scratch reads, so no peer can write a4 into the scratch before they are done
+      push_all<CS>(sA3, sw_off(b, cr * NS1 + 4 * n4, D1), bar_a3, cr, v);
+    }
+    stamp(13);
+  }
+  dense_chain_body<L, D0, D1, D2, CS, true>(sm, p, cr, bar_a3, bar_a4, bar_dz3, stamp);
+}
+
+// The chain from a3 on, for a step whose forward kernel (cnn_fwd_dense0_kernel) has already computed a3 = relu(x W0^T + b0): P2 .. P5 of
+// mlp_chain_kernel, unchanged, on the same cluster.  Everything but a3 and the labels (the W1 row slice, W2, the biases and the W0 column
+// slice of dx) is staged before griddepcontrol.wait, i.e. while the forward kernel still runs; then a3 (32 KB) is the only input left.
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dense_tail_kernel(const MlpChainParams p) {
+  using L = TailSmem<D0, D1, D2, CS>;
+  constexpr int NS1 = L::NS1, NS2 = L::NS2;
+  static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
+  static_assert(NS1 % 8 == 0 && NS2 % 4 == 0 && L::KS0 % 4 == 0, "slices must hold whole register tiles");
+  static_assert(L::BAR % 2 == 0 && L::SCRATCH % 4 == 0, "mbarriers are 8-byte aligned, the scratch 16-byte aligned");
+  extern __shared__ __align__(16) float sm[];
+  float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sW2 = sm + L::W2; float* sA3own = sm + L::A3OWN;
+  float* sB1 = sm + L::MISC + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + L::BAR);
+  uint64_t* bar_a4 = bar; uint64_t* bar_dz3 = bar + 1;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int cr = (int)cluster.block_rank();
+  const int tid = threadIdx.x;
+  const int B = p.B, C = p.C;
+  auto stamp = [&](int slot) {
+    if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
+  };
+  stamp(0);
+  if (tid == 0) {
+    for (int i = 0; i < 2; ++i) mbar_init(bar + i, 1);
+    mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
+    mbar_arrive_expect_tx(bar_dz3, (CS - 1) * MC_B * NS1 * 4);
+    fence_barrier_init();
+  }
+  asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
+  // ---------------- prologue (independent of the forward kernel)
+  stage_swizzled_async(sW1, p.w1 + (long long)cr * NS2 * D1, NS2, D1, D1);
+  stage_head_async<D2, NS2>(sW2, sB1, sB2, p.w2, p.b1, p.b2, cr, C);
+  stage_plain_async(sW0, p.w0 + cr * L::KS0, D1, L::KS0, D0);
+  cp_async_commit();
+  stamp(1);
+  pdl_wait();
+  pdl_launch();
+  stamp(2);
+  // a3 (rows >= B zero), this CTA's own a3 columns, the labels
+  for (int c = tid; c < MC_B * (D1 >> 2); c += MC_THREADS) {
+    const int r = c / (D1 >> 2), q = c - r * (D1 >> 2);
+    if (r < B) cp_async16(sA3 + sw_off(r, q << 2, D1), p.a3 + (long long)r * D1 + (q << 2));
+    else *reinterpret_cast<float4*>(sA3 + sw_off(r, q << 2, D1)) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  for (int c = tid; c < MC_B * (NS1 >> 2); c += MC_THREADS) {
+    const int r = c / (NS1 >> 2), q = c - r * (NS1 >> 2);
+    if (r < B) cp_async16(sA3own + r * NS1 + (q << 2), p.a3 + (long long)r * D1 + cr * NS1 + (q << 2));
+    else *reinterpret_cast<float4*>(sA3own + r * NS1 + (q << 2)) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (tid < MC_B) sLab[tid] = tid < B ? p.label[tid] : 0.f;
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();
+  cluster.barrier_wait();
+  stamp(3);
+  dense_chain_body<L, D0, D1, D2, CS, false>(sm, p, cr, nullptr, bar_a4, bar_dz3, stamp);
 }
 
 // ---- the dense weight gradients, from what mlp_chain_kernel stored: dW0 = dz3^T x, dW1 = dz4^T a3, dW2 = dl^T a4, and the bias gradients
@@ -531,18 +619,19 @@ __global__ void __launch_bounds__(WG_THREADS) dense_wgrad_kernel(const DenseWgra
 
 using namespace gx;
 
-// 512 -> 256 -> 128 -> C (C <= 16), B <= 32.  Returns -1 for unsupported shapes (caller uses the per-layer kernels).
-template <int CS>
+// 512 -> 256 -> 128 -> C (C <= 16), B <= 32.  TAIL: dense_tail_kernel, else mlp_chain_kernel.  Returns -2 when this cluster size cannot be
+// scheduled on this device.
+template <bool TAIL, int CS>
 static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
-  using L = MlpSmem<512, 256, 128, CS>;
-  auto kern = mlp_chain_kernel<512, 256, 128, CS>;
+  constexpr int BYTES = TAIL ? TailSmem<512, 256, 128, CS>::BYTES : MlpSmem<512, 256, 128, CS>::BYTES;
+  auto kern = TAIL ? dense_tail_kernel<512, 256, 128, CS> : mlp_chain_kernel<512, 256, 128, CS>;
   static int ready = 0;      // 0 = not configured, 1 = ok, -1 = this cluster size cannot be scheduled on this device
   if (ready == 0) {
     ready = -1;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::BYTES) == cudaSuccess &&
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES) == cudaSuccess &&
         (CS <= 8 || cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess)) {
       cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(CS); cfg.blockDim = dim3(MC_THREADS); cfg.dynamicSmemBytes = L::BYTES;
+      cfg.gridDim = dim3(CS); cfg.blockDim = dim3(MC_THREADS); cfg.dynamicSmemBytes = BYTES;
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
       cfg.attrs = at; cfg.numAttrs = 1;
@@ -554,15 +643,28 @@ static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
   if (ready < 0) return -2;
   static int use_pdl = -1;
   if (use_pdl < 0) { const char* e = getenv("GEOMX_MLP_PDL"); use_pdl = (e && e[0] == '0') ? 0 : 1; }
-  if (use_pdl) launch_pdl(kern, dim3(CS), dim3(MC_THREADS), (size_t)L::BYTES, stream, p);
-  else kern<<<dim3(CS), dim3(MC_THREADS), (size_t)L::BYTES, stream>>>(p);
+  if (use_pdl) launch_pdl(kern, dim3(CS), dim3(MC_THREADS), (size_t)BYTES, stream, p);
+  else kern<<<dim3(CS), dim3(MC_THREADS), (size_t)BYTES, stream>>>(p);
   return GX_CHECK_LAUNCH();
+}
+// cluster of 16 CTAs (one GPC) halves every slice; fall back to the portable size 8 when the device cannot co-schedule 16
+template <bool TAIL>
+static int mlp_launch_any(const MlpChainParams& p, cudaStream_t stream) {
+  static int want = -1;
+  if (want < 0) { const char* e = getenv("GEOMX_MLP_CLUSTER"); want = e ? atoi(e) : 16; }
+  if (want >= 16) {
+    const int rc = mlp_launch<TAIL, 16>(p, stream);
+    if (rc != -2) return rc;
+    want = 8;
+  }
+  return mlp_launch<TAIL, 8>(p, stream);
 }
 
 static unsigned long long* g_mlp_dbg = nullptr;
 GX_API int gx_mlp_chain_set_debug(unsigned long long* p) { g_mlp_dbg = p; return 0; }
 
-// the data path: loss, logits, dx; stores a3, a4, dz4, dz3 and the dlogits (rows b < B) for gx_dense_wgrad
+// the data path: loss, logits, dx; stores a3, a4, dz4, dz3 and the dlogits (rows b < B) for gx_dense_wgrad.  Returns -1 for unsupported
+// shapes (caller uses the per-layer kernels).
 GX_API int gx_mlp_chain(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
                         const float* label, float* loss, float* logits, float* dx, float* a3, float* a4, float* dz4, float* dz3, float* dl,
                         int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
@@ -570,15 +672,19 @@ GX_API int gx_mlp_chain(const float* x, const float* w0, const float* b0, const 
   MlpChainParams p;
   p.x = x; p.w0 = w0; p.b0 = b0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
   p.a3 = a3; p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
-  // cluster of 16 CTAs (one GPC) halves every slice; fall back to the portable size 8 when the device cannot co-schedule 16
-  static int want = -1;
-  if (want < 0) { const char* e = getenv("GEOMX_MLP_CLUSTER"); want = e ? atoi(e) : 16; }
-  if (want >= 16) {
-    const int rc = mlp_launch<16>(p, stream);
-    if (rc != -2) return rc;
-    want = 8;
-  }
-  return mlp_launch<8>(p, stream);
+  return mlp_launch_any<false>(p, stream);
+}
+
+// the same data path from a3 [B][D1] (computed by gx_cnn_fwd_dense0): loss, logits, dx; stores a4, dz4, dz3 and the dlogits for
+// gx_dense_wgrad.  w0 is read only as the column slices of dx.  Returns -1 for unsupported shapes.
+GX_API int gx_dense_tail(const float* a3, const float* w0, const float* w1, const float* b1, const float* w2, const float* b2, const float* label,
+                         float* loss, float* logits, float* dx, float* a4, float* dz4, float* dz3, float* dl, int B, int D0, int D1, int D2, int C,
+                         cudaStream_t stream) {
+  if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
+  MlpChainParams p = {};
+  p.w0 = w0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
+  p.a3 = const_cast<float*>(a3); p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
+  return mlp_launch_any<true>(p, stream);
 }
 
 // dW0 / db0, dW1 / db1, dW2 / db2 (overwritten) from what gx_mlp_chain stored; x has exactly B rows, dl rows hold 16 floats
@@ -592,3 +698,4 @@ GX_API int gx_dense_wgrad(const float* x, const float* a3, const float* a4, cons
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_mlp_chain_smem_bytes() { return MlpSmem<512, 256, 128, 8>::BYTES; }
+GX_API int gx_dense_tail_smem_bytes() { return TailSmem<512, 256, 128, 16>::BYTES; }

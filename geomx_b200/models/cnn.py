@@ -7,8 +7,10 @@
 plus the HiPS push/pull of all 10 keys (``dist_sync``: party aggregation → global aggregation + optimizer → broadcast), captured ONCE
 into a CUDA graph and replayed per step.  At the reference's batch size (32 per worker) the step is 5-6 hand-written sm_90a launches:
 
-  cnn_fwd      conv0+bias+ReLU+pool → conv1+bias+ReLU+pool, fp32 FMA, the conv0 map never leaves shared memory      (csrc/kernels/cnn_direct.cu)
-  mlp_chain    dense0 → dense1 → classifier → softmax-CE forward and the data gradients down to da2, one 16-CTA cluster (csrc/kernels/mlp_chain.cu)
+  cnn_fwd      conv0+bias+ReLU+pool → conv1+bias+ReLU+pool → dense0+bias+ReLU, fp32 FMA, the conv0 map never leaves shared memory; clusters
+               of two images, whose 8 CTAs exchange a2 and compute a3 (cnn_fwd_dense0_kernel, csrc/kernels/cnn_direct.cu)
+  mlp_chain    dense1 → classifier → softmax-CE forward and the data gradients down to da2, from a3, one 16-CTA cluster
+               (dense_tail_kernel, csrc/kernels/mlp_chain.cu)
   dense_wgrad  the three dense weight gradients and bias gradients, on a parallel branch: in the dense channel's step on the
                high-priority stream when there is one, otherwise on the side stream, joined before the exchange   (csrc/kernels/mlp_chain.cu)
   cnn_bwd_all  conv1 data gradient + pool/ReLU routing + conv0 weight gradient ‖ conv1 weight gradient, one grid      (csrc/kernels/cnn_direct.cu)
@@ -16,7 +18,8 @@ into a CUDA graph and replayed per step.  At the reference's batch size (32 per 
                a high-priority stream underneath cnn_bwd_all, the conv keys' one-hop exchange after it (one rank / GEOMX_STEP_OVERLAP=1)
                                                                                                                       (csrc/kernels/hips_fabric.cu)
 
-Larger batches (and ``GEOMX_DIRECT_CONV=0`` / ``GEOMX_FUSED_MLP=0``) use the generic kernels: direct conv0 + im2col, wgmma GEMMs with fused
+Without the direct convolutions (odd batches, ``GEOMX_DIRECT_CONV=0``) the cluster kernel starts from a2 and computes dense0 itself
+(mlp_chain_kernel).  Larger batches (and ``GEOMX_DIRECT_CONV=0`` / ``GEOMX_FUSED_MLP=0``) use the generic kernels: direct conv0 + im2col, wgmma GEMMs with fused
 bias / ReLU / max-pool / mask / column-sum epilogues (3xTF32 = fp32-accurate by default), weight-gradient GEMMs on a parallel graph branch.
 With one rank and one party both PS tiers collapse into the arena optimizer inside the exchange kernels.
 
@@ -97,7 +100,8 @@ class HipsCNNTrainStep:
         the forward convolutions of batch k+1, and returns the loss of batch k (``nan`` on the first call; ``flush()`` trains the last batch).
         The arithmetic and its order are unchanged — batch k+1's convolutions still read the conv weights updated by batch k, its head the
         dense weights updated by batch k — only the place where the step is cut into launches moves, so that the two-hop exchange of the
-        660 KB dense keys has ~25 us of independent work to hide behind instead of ~9."""
+        660 KB dense keys has ~25 us of independent work to hide behind instead of ~9.  (Where the forward kernel also computes dense0, even
+        batches <= 32, it reads W0 and so waits for the dense keys' exchange.)"""
         native.require()
         from .. import optimizer as opt
         self.B = B = int(batch_size)
@@ -233,7 +237,8 @@ class HipsCNNTrainStep:
     # ------------------------------------------------------------------------------------------------------------
     def _steps(self):
         """The training step as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch for weight
-        gradients), 'comm' (a key group's exchange on the high-priority stream) or 'join' (main, after the side branch)."""
+        gradients), 'comm' (a key group's exchange on the high-priority stream), 'join' (main, after the side branch) or 'join_comm' (main,
+        after the side branch and the comm stream)."""
         n = native
         B, P, G, f = self.B, self.P, self.G, self.fabric
         a2f = self.a2.view(B, 512)
@@ -245,6 +250,7 @@ class HipsCNNTrainStep:
         elif self.single:
             kv = lambda: f.channel_step(self.single, zero_grad=self.fused_zero_grad)
         kv_dense = [("hips push+opt+pull (dense keys, overlapped)", "comm", lambda: f.channel_step("dense", zero_grad=self.fused_zero_grad))] if self.overlap else []
+        carry = (self.label, self.label_cur) if self.lookahead else None
         self._tail = []
         if self.update == "local":
             sp = self._local_spec
@@ -277,11 +283,27 @@ class HipsCNNTrainStep:
             ("dW0 gemm", "side", lambda: n.gemm(self.dz3, a2f, G[4], a_mn=True, b_mn=True)),
             ("da2 gemm", "main", lambda: n.gemm(self.dz3, P[4], self.da2, b_mn=True)),
         ]
+        # even B <= 32 (paths with both the direct convolutions and the cluster kernel): dense0 is row-separable, so the forward kernel
+        # computes a3 on its 128 SMs and the cluster kernel starts from a3
+        self._fwd_dense0 = fwd_dense0 = self.direct_conv and self.fused_mlp
+        if fwd_dense0:
+            def fwd():
+                if not n.cnn_fwd_dense0(self.x, P[0], P[1], P[2], P[3], P[4], P[5], self.a1, self.idx1, self.a2, self.idx2, self.a3, carry=carry,
+                                        x_keep=self.x_cur if self.lookahead else None):
+                    raise RuntimeError("cnn_fwd_dense0 does not cover batch %d" % B)
+        else:
+            fwd = lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry,
+                                    x_keep=self.x_cur if self.lookahead else None)
         if self.fused_mlp:
             # dense0 -> dense1 -> classifier -> softmax-CE forward and backward: one cluster launch for the data path (what the convolution
             # backward pass waits for) and one weight-gradient launch on a parallel branch, instead of the seven above
-            head = [("mlp chain fwd+bwd (cluster)", "main", lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss,
-                                                                                   self.logits, self.da2, self.a3, self.a4, self.dz4, self.dz3, self.dl))]
+            if fwd_dense0:
+                chain = lambda: n.dense_tail(self.a3, P[4], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2, self.a4,
+                                             self.dz4, self.dz3, self.dl)
+            else:
+                chain = lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2,
+                                                 self.a3, self.a4, self.dz4, self.dz3, self.dl)
+            head = [("mlp chain fwd+bwd (cluster)", "main", chain)]
             wgrad = lambda: n.dense_wgrad(a2f, self.a3, self.a4, self.dz4, self.dz3, self.dl, G[4], G[5], G[6], G[7], G[8], G[9])
             if kv_dense and not self.lookahead:
                 # the dense channel reads these gradients: issued in the same comm-stream step, only a programmatic edge separates the two
@@ -291,9 +313,8 @@ class HipsCNNTrainStep:
                 # side stream, joined before the exchange (a dense channel's comm step waits for it too).  A look-ahead launch ends with
                 # the next batch's forward convolutions, which overwrite the x this kernel reads: _body joins the side branch before them
                 head.append(("dense weight gradients", "side", wgrad))
-        # number of leading steps that only need the batch and the conv weights (the part a look-ahead launch runs for the NEXT batch)
+        # number of leading steps that only need the batch and the weights (the part a look-ahead launch runs for the NEXT batch)
         self._n_fwd = 1 if self.direct_conv else 2
-        carry = (self.label, self.label_cur) if self.lookahead else None
         if self.direct_conv:
             da2v = self.da2
             if os.environ.get("GEOMX_CNN_BWD_ONE_LAUNCH", "1") == "1" and B % 2 == 0 and B <= 64:
@@ -304,20 +325,20 @@ class HipsCNNTrainStep:
                     # ... and the conv keys' exchange in the tail of the same launch (the CTAs that finish last serve one tile each)
                     blk, tiles, n_act = fused
                     return [
-                        ("conv0+conv1 fwd (direct, relu+pool fused)", "main", lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry, x_keep=self.x_cur if self.lookahead else None)),
+                        ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
                     ] + head + kv_dense + [
                         ("conv bwd (one grid) + conv-key exchange in its tail", "main",
                          lambda: n.cnn_bwd_exchange(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1], G[2], G[3], blk, tiles, n_act)),
                     ] + self._tail
                 return [
-                    ("conv0+conv1 fwd (direct, relu+pool fused)", "main", lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry, x_keep=self.x_cur if self.lookahead else None)),
+                    ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
                 ] + head + kv_dense + [
                     ("conv bwd: conv1 wgrad + dgrad + conv0 wgrad (direct, one grid)", "main",
                      lambda: n.cnn_bwd_all(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1], G[2], G[3])),
                     ("hips push+opt+pull", "join", kv),
                 ] + self._tail
             return [
-                ("conv0+conv1 fwd (direct, relu+pool fused)", "main", lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry, x_keep=self.x_cur if self.lookahead else None)),
+                ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
             ] + head + kv_dense + [
                 ("conv1 wgrad (direct, sparse)", "side", lambda: n.cnn_wgrad1(self.a1, self.a2, self.idx2, da2v, G[2], G[3])),
                 ("conv1 dgrad + conv0 wgrad (direct)", "main", lambda: n.cnn_bwd(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1])),
@@ -349,8 +370,10 @@ class HipsCNNTrainStep:
         forked = comm_forked = False
         steps = self._steps()
         nf = self._n_fwd
-        # rotated: the next batch's forward convolutions overwrite a2, which the side branch (dense weight gradients) may still be reading
-        rotated = steps[nf:] + [(name, "join" if where == "main" else where, fn) for name, where, fn in steps[:nf]]
+        # rotated: the next batch's forward convolutions overwrite a2 (and a3), which the side branch (dense weight gradients) may still be
+        # reading; a forward kernel that also computes dense0 reads W0 / b0, which the dense keys' exchange (comm) updates
+        join = "join_comm" if self._fwd_dense0 else "join"
+        rotated = steps[nf:] + [(name, join if where == "main" else where, fn) for name, where, fn in steps[:nf]]
         steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": rotated}[part]
         for i, (name, where, fn) in enumerate(steps):
             if stop_after is not None and i >= stop_after:
@@ -368,8 +391,10 @@ class HipsCNNTrainStep:
                     fn()
                 comm_forked = True
             else:
-                if where == "join" and forked:
+                if where in ("join", "join_comm") and forked:
                     main.wait_stream(side); forked = False
+                if where == "join_comm" and comm_forked:
+                    main.wait_stream(comm); comm_forked = False
                 fn()
         if forked:
             main.wait_stream(side)

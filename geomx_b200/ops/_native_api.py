@@ -117,6 +117,21 @@ def mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, d
     return True
 
 
+def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl):
+    """The data path of the dense chain from a3 [B,D1] on (what :func:`cnn_fwd_dense0` computed), in ONE cluster launch: per-sample loss,
+    logits and dx [B,D0]; it also stores a4, dz4, dz3 and the dlogits dl [B,16] for :func:`dense_wgrad` (a3 is already in memory).  ``w0``
+    [D1,D0] is read for dx only.  Returns False for shapes other than 512 -> 256 -> 128 -> C<=16, batch <= 32."""
+    B, D1 = a3.shape
+    D0, D2, C = w0.shape[1], w1.shape[0], w2.shape[0]
+    assert w0.shape[0] == D1 and dx.shape == (B, D0) and dl.shape == (B, 16)
+    rc = _lib().gx_dense_tail(_p(a3), _p(w0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dx), _p(a4), _p(dz4), _p(dz3),
+                              _p(dl), B, D0, D1, D2, C, _s())
+    if rc == -1:
+        return False
+    _ck(rc, "dense_tail")
+    return True
+
+
 def dense_wgrad(x, a3, a4, dz4, dz3, dl, dw0, db0, dw1, db1, dw2, db2):
     """The dense chain's weight and bias gradients (overwritten) from what :func:`mlp_chain_data` stored: dW0 = dz3ᵀ·x, dW1 = dz4ᵀ·a3,
     dW2 = dlᵀ·a4 and their column sums, one launch."""
@@ -136,6 +151,21 @@ def cnn_fwd(x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry=None, x_keep=None):
     src, dst = carry if carry is not None else (None, None)
     _ck(_lib().gx_cnn_fwd(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(a1), _p(idx1), _p(a2), _p(idx2), _p(src), _p(dst),
                           0 if src is None else src.numel(), _p(x_keep), x.shape[0], _s()), "cnn_fwd")
+
+
+def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None, x_keep=None):
+    """:func:`cnn_fwd` followed by the first dense layer in the same launch: also a3 [B,256] = relu(a2.view(B,512) · wdᵀ + bd), with
+    wd [256,512].  ``carry`` / ``x_keep`` as in :func:`cnn_fwd`.  Runs clusters of two images: returns False without launching for odd B or
+    B > 32."""
+    B = x.shape[0]
+    assert wd.shape == (256, 512) and a3.shape == (B, 256) and a3.is_contiguous()
+    src, dst = carry if carry is not None else (None, None)
+    rc = _lib().gx_cnn_fwd_dense0(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(wd), _p(bd), _p(a1), _p(idx1), _p(a2), _p(idx2), _p(a3), _p(src),
+                                  _p(dst), 0 if src is None else src.numel(), _p(x_keep), B, _s())
+    if rc == -1:
+        return False
+    _ck(rc, "cnn_fwd_dense0")
+    return True
 
 
 def cnn_bwd(x, w1, a1, idx1, a2, idx2, da2, dw0, db0):

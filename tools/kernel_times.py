@@ -47,6 +47,7 @@ if eng.fused_mlp:
     for rep in range(3):
         eng._body(); torch.cuda.synchronize()
         st = dbg.cpu().tolist()
+        # (the cluster kernel that starts from a3, dense_tail_kernel, leaves slots 4 and 10..13 at 0)
         print("mlp chain phases (us since kernel start): 0 start|1 prologue issued|2 pdl wait done|3 inputs landed+sync|4 a3 landed|5 a4 landed|"
               "6 dz4 computed|7 dz3 pushed|8 dz3 landed|9 end (da2 stored):",
               ["%.2f" % ((v - st[0]) / 1e3) for v in st[:10]], "| P1: 10 products done|11 partials synced|12 W0 prefetch issued|13 a3 pushed:",
@@ -60,7 +61,7 @@ if eng.direct_conv:
         eng._body(); torch.cuda.synchronize()
         st = dbg.cpu().tolist()
         r = lambda a, b: ["%.2f" % ((v - st[a]) / 1e3) for v in st[a:b]]
-        print("cnn_fwd  (us): 0 start|1 operands staged|2 conv0 done|3 conv1 partials|4 end:", r(0, 5))
+        print("cnn_fwd  (us): 0 start|1 operands staged|2 conv0 done|3 conv1 partials|4 end|5 a2 landed|6 a3 stored (5, 6: with dense0):", r(0, 7))
         print("cnn_bwd  (us): 8 start|9 staged|10 dz2 scattered|11 dgrad partials|12 da1 routed|13 end:", r(8, 14))
         print("cnn_wgrad1 (us): 16 start|17 staged|18 end:", r(16, 19))
     lib.gx_cnn_set_debug(ctypes.c_void_p(0))

@@ -19,16 +19,20 @@ import geomx_b200 as mx  # noqa: E402
 from geomx_b200.ops import native  # noqa: E402
 from geomx_b200.parallel import Topology  # noqa: E402
 
-# in-kernel %globaltimer stamps of the direct-convolution kernels (gx_cnn_set_debug slots, written by the first CTA of each body)
+# in-kernel %globaltimer stamps of the direct-convolution kernels (gx_cnn_set_debug slots, written by the first CTA of each body).  The
+# forward kernel that also computes dense0 (even batches <= 32) stamps 5 a2 landed | 6 a3 stored before its end (4).
 CNN_PHASES = {"cnn_fwd": (0, 1, 2, 3, 4), "cnn_bwd": (8, 9, 10, 11, 12, 13), "cnn_wgrad1": (16, 17, 18)}
 CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
                     "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
                     "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
+FWD_DENSE0_PHASES, FWD_DENSE0_LABELS = (0, 1, 2, 3, 5, 6), ("staging", "conv0", "conv1", "a2 landed", "dense0 -> a3 stored")
 # the same for the dense-chain cluster kernel (gx_mlp_chain_set_debug slots of cluster CTA 0): 0 start | 3 inputs landed | 4 a3 landed |
 # 5 a4 landed | 6 dz4 computed | 7 dz3 pushed | 8 dz3 landed | 9 end (da2 stored); and of the dense weight-gradient kernel: 16 start of its
-# CTA 0 | 17 its grid dependency resolved | 18 end of its last CTA
+# CTA 0 | 17 its grid dependency resolved | 18 end of its last CTA.  The kernel that starts from a3 (dense_tail_kernel) has no slot 4.
 MLP_PHASES = (0, 3, 4, 5, 6, 7, 8, 9)
 MLP_PHASE_LABELS = ("staging+pdl-wait", "dense0 -> a3", "dense1 -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
+TAIL_PHASES = (0, 3, 5, 6, 7, 8, 9)
+TAIL_PHASE_LABELS = ("staging+pdl-wait", "a3 staged -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
 
 
 def main():
@@ -53,6 +57,11 @@ def main():
         eng.step(X, y)
     fab = eng.fabric
     chans = list(fab.channels) or ["fsa"]
+    tail = getattr(eng, "_fwd_dense0", False)
+    cnn_phases, cnn_labels = dict(CNN_PHASES), dict(CNN_PHASE_LABELS)
+    if tail:
+        cnn_phases["cnn_fwd"], cnn_labels["cnn_fwd"] = FWD_DENSE0_PHASES, FWD_DENSE0_LABELS
+    mlp_phases, mlp_labels = (TAIL_PHASES, TAIL_PHASE_LABELS) if tail else (MLP_PHASES, MLP_PHASE_LABELS)
     for c in chans:
         fab.state[c][3] = 1
     flush = torch.empty(64 * 1024 * 1024, device=dev)
@@ -79,8 +88,8 @@ def main():
             per = [(c[64 + 3 * i], c[65 + 3 * i], c[66 + 3 * i]) for i in range(256)]
             row["_cta"] = per
         row["_ms"] = ev[0].elapsed_time(ev[1])
-        row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in CNN_PHASES.items()}
-        row["_mlp_ph"] = [(m[s1] - m[s0]) / 1e3 for s0, s1 in zip(MLP_PHASES, MLP_PHASES[1:])]
+        row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in cnn_phases.items()}
+        row["_mlp_ph"] = [(m[s1] - m[s0]) / 1e3 for s0, s1 in zip(mlp_phases, mlp_phases[1:])]
         if "chan:dense" in row and "chan:conv" in row:
             # the dense branch (weight gradients + dense channel) must end before the conv-key exchange does, or it is exposed
             row["_dense_vs_conv"] = (row["chan:dense"][1] - row["chan:conv"][1]) / 1e3
@@ -114,11 +123,11 @@ def main():
                 k = sum(1 for i in v if i < 128)
                 pair[["bwd+bwd", "bwd+wgrad", "wgrad+wgrad"][k]] += 1
         lines.append("  SM sharing: %s" % pair)
-    for name, labels in CNN_PHASE_LABELS.items():
+    for name, labels in cnn_labels.items():
         lines.append("  %s phases of CTA 0 (us): %s" % (name, "  ".join("%s %.2f" % (lab, statistics.median(r["_cnn_ph"][name][i] for r in rows))
                                                                       for i, lab in enumerate(labels))))
-    lines.append("  mlp_chain phases of CTA 0 (us): %s" % "  ".join("%s %.2f" % (lab, statistics.median(r["_mlp_ph"][i] for r in rows))
-                                                                    for i, lab in enumerate(MLP_PHASE_LABELS)))
+    lines.append("  %s phases of CTA 0 (us): %s" % ("dense_tail" if tail else "mlp_chain", "  ".join(
+        "%s %.2f" % (lab, statistics.median(r["_mlp_ph"][i] for r in rows)) for i, lab in enumerate(mlp_labels))))
     if "_dense_vs_conv" in rows[0]:
         d = statistics.median(r["_dense_vs_conv"] for r in rows)
         lines.append("  dense branch (weight gradients + dense channel) ends %.2f us %s the end of the conv-key exchange" % (abs(d), "after" if d > 0 else "before"))
