@@ -12,6 +12,10 @@
 //                       become resident and stage while that kernel still runs.
 //                       (cnn_bwd_kernel / cnn_wgrad1_kernel: the same bodies as separate launches; cnn_bwd_exchange_kernel: the same bodies
 //                       in one grid (data-gradient CTAs first) whose last CTAs also perform the conv keys' exchange — measured, no gain, opt-in.)
+// and, for inference, ONE launch for any number of images:
+//   cnn_eval_kernel     x -> logits, softmax-CE loss, arg-max and correct flag per image: the convolutions and dense0 of cnn_fwd_dense0_kernel
+//                       (clusters of two images, without the stores only the backward pass needs), then dense1 and the classifier in the
+//                       same cluster (HipsCNNTrainStep.evaluate / predict)
 //
 // Why not the tensor-core GEMM here: with a per-worker batch of 32 the conv1 products are M = 2048 x N = 32 x K = 400 — 16 tensor-core
 // tiles.  Forward + dgrad + wgrad + im2col/col2im traffic through the GEMM path is several launches of latency-bound work on 16 SMs, while
@@ -100,12 +104,14 @@ struct CnnFwdSmem {
 // (distributed shared memory), then conv1 for output channels [8g, 8g+8) over all 16.  Returns, in threads tid < 128, the pooled conv1
 // value that thread stored to a2 and its offset within the image's 512 (channel * 16 + window).  The kernel arms whatever its cluster
 // needs before this body's start-up cluster barrier.
-template <int IMGS>
+// TRAIN = false (inference): none of the stores the backward pass needs (a1, idx1, a2, idx2, carry, x_keep), and the image is read from
+// x[min(b, n_img - 1)], so that the missing second image of an odd batch's last cluster reads nothing past the batch.
+template <int IMGS, bool TRAIN = true>
 __device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __restrict__ x, const float* __restrict__ w0,
                                                const float* __restrict__ b0, const float* __restrict__ w1, const float* __restrict__ b1,
                                                float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
                                                unsigned char* __restrict__ idx2, const float* __restrict__ carry_src, float* __restrict__ carry_dst,
-                                               int carry_n, float* __restrict__ x_keep, unsigned long long* dbg, int& a2_off) {
+                                               int carry_n, float* __restrict__ x_keep, unsigned long long* dbg, int& a2_off, int n_img = 0) {
   float* sx = s.sx; float* sw0 = s.sw0; float* sb0 = s.sb0; float* sa1 = s.sa1; float* sw1 = s.sw1; float* sb1 = s.sb1; float* spart = s.spart;
   cg::cluster_group cluster = cg::this_cluster();
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
@@ -117,8 +123,9 @@ __device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __res
   const int b = blockIdx.x, g = blockIdx.y, tid = threadIdx.x, bl = b % IMGS;     // g == the image's rank among its four CTAs
   // look-ahead steps: this launch is the tail of the previous batch's step; it hands the labels that arrived with its image batch over to
   // the buffer the classifier head of the NEXT launch reads (a 128-byte side job instead of a copy node in the step graph)
-  if (carry_n > 0 && b == 0 && g == 0) for (int i = tid; i < carry_n; i += 256) carry_dst[i] = carry_src[i];
-  for (int i = tid; i < CD_H * CD_H / 4; i += 256) cpa16(sx + 4 * i, x + (long long)b * CD_H * CD_H + 4 * i);
+  if (TRAIN && carry_n > 0 && b == 0 && g == 0) for (int i = tid; i < carry_n; i += 256) carry_dst[i] = carry_src[i];
+  const int bx = TRAIN ? b : min(b, n_img - 1);
+  for (int i = tid; i < CD_H * CD_H / 4; i += 256) cpa16(sx + 4 * i, x + (long long)bx * CD_H * CD_H + 4 * i);
   if (tid < 4 * 25) { const int cl = tid / 25, t = tid - cl * 25; cpa4(sw0 + cl * CD_W1PAD + t, w0 + 4 * g * 25 + tid); }
   if (tid < 4 * 3) sw0[(tid / 3) * CD_W1PAD + 25 + tid % 3] = 0.f;                                   // pad taps 25..27
   if (tid < 4) sb0[tid] = b0[4 * g + tid];
@@ -133,7 +140,7 @@ __device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __res
   cluster.barrier_wait();
   stamp(1);
   // look-ahead steps: the backward pass of this batch runs in the NEXT launch, after the following batch has overwritten x — keep a copy
-  if (x_keep != nullptr && g == 0) for (int i = tid; i < CD_H * CD_H / 4; i += 256)
+  if (TRAIN && x_keep != nullptr && g == 0) for (int i = tid; i < CD_H * CD_H / 4; i += 256)
     reinterpret_cast<float4*>(x_keep + (long long)b * CD_H * CD_H)[i] = reinterpret_cast<const float4*>(sx)[i];
   // ---- conv0 + bias + ReLU + pool of this CTA's 4 channels: thread -> channel 4g + tid/64, windows (tid%64) + 64 j
   {
@@ -152,8 +159,10 @@ __device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __res
       const float v = pool4(acc, bias, bi);
 #pragma unroll
       for (int r = 0; r < 4; ++r) cluster.map_shared_rank(sa1, r * IMGS + bl)[ch * CD_P1 * CD_P1 + win] = v;
-      const long long o = ((long long)b * CD_C1 + ch) * (CD_P1 * CD_P1) + win;
-      a1[o] = v; idx1[o] = (unsigned char)bi;
+      if (TRAIN) {
+        const long long o = ((long long)b * CD_C1 + ch) * (CD_P1 * CD_P1) + win;
+        a1[o] = v; idx1[o] = (unsigned char)bi;
+      }
     }
   }
   cluster.sync();      // all 16 conv0 channels of image b are in every CTA's sa1
@@ -191,8 +200,10 @@ __device__ __forceinline__ float cnn_fwd_convs(CnnFwdSmem& s, const float* __res
     int bi;
     v = pool4(acc, sb1[ol], bi);
     a2_off = (8 * g + ol) * (CD_P2 * CD_P2) + win;
-    const long long o = (long long)b * CD_C2 * (CD_P2 * CD_P2) + a2_off;
-    a2[o] = v; idx2[o] = (unsigned char)bi;
+    if (TRAIN) {
+      const long long o = (long long)b * CD_C2 * (CD_P2 * CD_P2) + a2_off;
+      a2[o] = v; idx2[o] = (unsigned char)bi;
+    }
   }
   return v;
 }
@@ -227,34 +238,30 @@ struct CnnFwdDense0Smem {
 static_assert(sizeof(CnnFwdDense0Smem) == CNN_FWD_DENSE0_SMEM_BYTES, "CNN_FWD_DENSE0_SMEM_BYTES (common.cuh) must match");
 constexpr int CD_D1 = 256, CD_D0 = CD_C2 * CD_P2 * CD_P2;    // dense0: 512 -> 256
 
-__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
-    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
-                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
-                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
-                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
-                          unsigned long long* dbg) {
-  __shared__ CnnFwdDense0Smem s;
+// thread 0, before cnn_fwd_convs: arms the a2 buffer and has the first cluster prefetch W0 into L2
+__device__ __forceinline__ void fwd_dense0_arm(CnnFwdDense0Smem& s, const float* __restrict__ wd) {
+  // the a2 buffer expects all 1024 floats; the peers push only after the body's start-up cluster barrier, so it is armed in time
+  mbar_init(&s.bar_a2, 1);
+  mbar_arrive_expect_tx(&s.bar_a2, 2 * CD_D0 * 4);
+  fence_barrier_init();
+  // W0 into L2 now: it is read at the very end of the kernel, and the step may start with L2 cold.  The first cluster prefetches it (each
+  // CTA its 64 KB, rows 32 r .. 32 r + 31) and every cluster reads it from L2.  (Every cluster prefetching its own copy was measured
+  // 0.4 us slower per step: 8 MiB of prefetch traffic at B = 32 slowed the staging of the images.)
+  if (blockIdx.x < 2) {
+    const float* slice = wd + (long long)32 * cg::this_cluster().block_rank() * CD_D0;
+    for (int k = 0; k < 4; ++k)
+      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(slice + k * 8 * CD_D0), "r"(8 * CD_D0 * 4) : "memory");
+  }
+}
+
+// after cnn_fwd_convs<2> (v, a2_off: what it returned): the a2 hand-off to all 8 CTAs and dense0 of the cluster's two images.  The threads
+// with j = tid % 8 < 2 call store(j, a3[bpair + j][32 cr + tid / 8]) (cr = cluster rank).
+template <class Store>
+__device__ __forceinline__ void fwd_dense0(CnnFwdDense0Smem& s, float v, int a2_off, int cr, const float* __restrict__ wd,
+                                          const float* __restrict__ bd, unsigned long long* dbg, Store store) {
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
-  stamp(0);
-  if (threadIdx.x == 0) {
-    // the a2 buffer expects all 1024 floats; the peers push only after the body's start-up cluster barrier, so it is armed in time
-    mbar_init(&s.bar_a2, 1);
-    mbar_arrive_expect_tx(&s.bar_a2, 2 * CD_D0 * 4);
-    fence_barrier_init();
-    // W0 into L2 now: it is read at the very end of the kernel, and the step may start with L2 cold.  The first cluster prefetches it (each
-    // CTA its 64 KB, rows 32 r .. 32 r + 31) and every cluster reads it from L2.  (Every cluster prefetching its own copy was measured
-    // 0.4 us slower per step: 8 MiB of prefetch traffic at B = 32 slowed the staging of the images.)
-    if (blockIdx.x < 2) {
-      const float* slice = wd + (long long)32 * cg::this_cluster().block_rank() * CD_D0;
-      for (int k = 0; k < 4; ++k)
-        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(slice + k * 8 * CD_D0), "r"(8 * CD_D0 * 4) : "memory");
-    }
-  }
-  int a2_off;
-  const float v = cnn_fwd_convs<2>(s.conv, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
-  // (computed after the convolutions, which need every register they can get)
-  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), bl = blockIdx.x & 1, bpair = blockIdx.x - bl;
+  const int tid = threadIdx.x, bl = blockIdx.x & 1;
   const float* wrow = wd + (long long)(32 * cr + (tid >> 3)) * CD_D0;   // the W0 row of this thread's output column
   // ---- a2 hand-off: lane 2 win + which holds window win of channel 8g + 2 op + which (op = warp); lanes 8k + which + {0, 2, 4, 6} hold
   // windows 4k .. 4k + 3 of one channel, gathered into one float4 push
@@ -291,9 +298,141 @@ __global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 r
     acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
     acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
   }
-  if (j < 2) a3[(long long)(bpair + j) * CD_D1 + 32 * cr + (tid >> 3)] = fmaxf((j == 0 ? acc0 : acc1) + bias, 0.f);
+  if (j < 2) store(j, fmaxf((j == 0 ? acc0 : acc1) + bias, 0.f));
+}
+
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
+    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
+                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
+                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
+                          unsigned long long* dbg) {
+  __shared__ CnnFwdDense0Smem s;
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  stamp(0);
+  if (threadIdx.x == 0) fwd_dense0_arm(s, wd);
+  int a2_off;
+  const float v = cnn_fwd_convs<2>(s.conv, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
+  // (computed after the convolutions, which need every register they can get)
+  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), bl = blockIdx.x & 1, bpair = blockIdx.x - bl;
+  fwd_dense0(s, v, a2_off, cr, wd, bd, dbg, [&](int j, float y) { a3[(long long)(bpair + j) * CD_D1 + 32 * cr + (tid >> 3)] = y; });
   stamp(6);
   stamp(4);      // (slot 4 stays the end of the forward kernel)
+}
+
+// ------------------------------------------------------------------------------------------------------------------ inference
+// The whole forward pass of N images (any N >= 1) and its per-sample scores, in one launch: grid (N rounded up to even, 4), clusters of
+// (2, 4, 1) as in cnn_fwd_dense0_kernel, whose convolutions (without the stores only training needs) and dense0 it runs.  Then:
+//   dense1      every CTA pushes its 32 a3 columns of both images into all 8 CTAs (st.async, second transaction mbarrier); cluster rank r
+//               computes a4[.][16 r .. 16 r + 16): 16 threads per column, each over every 16th float4 of the column's W1 row, summed in a
+//               fixed shuffle order (W1, 128 KB, is read from L2 by every cluster)
+//   classifier  every CTA pushes its 16 a4 columns of both images into all 8 CTAs (third mbarrier); rank i < 2 (the g = 0 CTA of image
+//               bpair + i) computes that image's 10 logits (16 threads per logit, fixed shuffle order), softmax-CE with fp32 expf / logf
+//               and the arg-max (first maximum wins, like torch.argmax)
+// The missing second image of an odd N's last cluster is computed from a copy of image N - 1 and takes part in every push; nothing of it is
+// written.  No atomics: two launches on the same inputs give the same bits.
+constexpr int CD_D2 = 128, CD_NC = 10;       // dense1: 256 -> 128, classifier: 128 -> 10
+struct CnnEvalSmem {
+  CnnFwdDense0Smem d0;
+  __align__(16) float a3[2 * CD_D1];        // both images' a3, as pushed by the 8 CTAs
+  __align__(16) float a4[2 * CD_D2];        // both images' a4, as pushed by the 8 CTAs
+  __align__(16) float a3own[2 * 32];        // this CTA's a3 columns of both images, gathered into float4 pushes
+  __align__(16) float a4own[2 * 16];        // ... and its a4 columns
+  float logit[16];
+  uint64_t bar_a3, bar_a4;
+};
+
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256)
+    cnn_eval_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                    const float* __restrict__ b1, const float* __restrict__ wd0, const float* __restrict__ bd0, const float* __restrict__ wd1,
+                    const float* __restrict__ bd1, const float* __restrict__ wd2, const float* __restrict__ bd2, const float* __restrict__ label,
+                    float* __restrict__ logits, float* __restrict__ loss, int* __restrict__ pred, int* __restrict__ correct, int N) {
+  __shared__ CnnEvalSmem s;
+  if (threadIdx.x == 0) {
+    mbar_init(&s.bar_a3, 1);
+    mbar_arrive_expect_tx(&s.bar_a3, 2 * CD_D1 * 4);
+    mbar_init(&s.bar_a4, 1);
+    mbar_arrive_expect_tx(&s.bar_a4, 2 * CD_D2 * 4);
+    fwd_dense0_arm(s.d0, wd0);              // (its barrier-init fence covers these two as well)
+  }
+  int a2_off;
+  const float v = cnn_fwd_convs<2, false>(s.d0.conv, x, w0, b0, w1, b1, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
+                                          a2_off, N);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, cr = (int)cg::this_cluster().block_rank();
+  fwd_dense0(s.d0, v, a2_off, cr, wd0, bd0, nullptr, [&](int j, float y) { s.a3own[j * 32 + (tid >> 3)] = y; });
+  // ---- a3 hand-off: warp w wrote columns 32 r + 4 w .. 4 w + 3 of both images; its lanes 0 and 1 push those of image 0 and 1
+  __syncwarp();
+  if (lane < 2) push_all<8>(s.a3, lane * CD_D1 + 32 * cr + 4 * warp, &s.bar_a3, cr, reinterpret_cast<const float4*>(s.a3own)[lane * 8 + warp]);
+  // ---- dense1: thread -> column n = 16 r + tid / 16, K-segment j = tid % 16: float4 chunks j, j + 16, j + 32, j + 48 of the row
+  const int j = tid & 15, n = 16 * cr + (tid >> 4);
+  const float* wrow = wd1 + (long long)n * CD_D1;
+  float4 w[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) w[q] = __ldg(reinterpret_cast<const float4*>(wrow) + 16 * q + j);   // in flight while a3 lands
+  const float bias1 = __ldg(bd1 + n);
+  wait_landed(&s.bar_a3);
+  float acc0 = 0.f, acc1 = 0.f;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4 x0 = reinterpret_cast<const float4*>(s.a3)[16 * q + j];
+    const float4 x1 = reinterpret_cast<const float4*>(s.a3 + CD_D1)[16 * q + j];
+    acc0 = fmaf(w[q].x, x0.x, acc0); acc0 = fmaf(w[q].y, x0.y, acc0); acc0 = fmaf(w[q].z, x0.z, acc0); acc0 = fmaf(w[q].w, x0.w, acc0);
+    acc1 = fmaf(w[q].x, x1.x, acc1); acc1 = fmaf(w[q].y, x1.y, acc1); acc1 = fmaf(w[q].z, x1.z, acc1); acc1 = fmaf(w[q].w, x1.w, acc1);
+  }
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) {
+    acc0 += __shfl_xor_sync(0xffffffffu, acc0, o);
+    acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
+  }
+  if (j < 2) s.a4own[j * 16 + (tid >> 4)] = fmaxf((j == 0 ? acc0 : acc1) + bias1, 0.f);
+  // classifier operands in flight while a4 is gathered: thread t < 160 -> logit c = t / 16, float4 chunks j and j + 16 of its W2 row
+  const int c = tid >> 4;
+  float4 w2[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+  float bias2 = 0.f;
+  if (cr < 2 && c < CD_NC) {
+    w2[0] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + j);
+    w2[1] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + 16 + j);
+    bias2 = __ldg(bd2 + c);
+  }
+  __syncthreads();
+  // ---- a4 hand-off: 8 float4 (image tid / 4, columns 16 r + 4 (tid % 4) ..) into all 8 CTAs
+  if (tid < 8) push_all<8>(s.a4, (tid >> 2) * CD_D2 + 16 * cr + 4 * (tid & 3), &s.bar_a4, cr, reinterpret_cast<const float4*>(s.a4own)[tid]);
+  wait_landed(&s.bar_a4);       // every CTA: nothing may still be pushed into its shared memory when it exits
+  if (cr >= 2) return;
+  const int b = (blockIdx.x & ~1) + cr;      // ranks 0 and 1 are the g = 0 CTAs of images bpair and bpair + 1
+  if (tid < 16 * CD_NC) {
+    const float4 x0 = reinterpret_cast<const float4*>(s.a4 + cr * CD_D2)[j];
+    const float4 x1 = reinterpret_cast<const float4*>(s.a4 + cr * CD_D2)[16 + j];
+    float acc = 0.f;
+    acc = fmaf(w2[0].x, x0.x, acc); acc = fmaf(w2[0].y, x0.y, acc); acc = fmaf(w2[0].z, x0.z, acc); acc = fmaf(w2[0].w, x0.w, acc);
+    acc = fmaf(w2[1].x, x1.x, acc); acc = fmaf(w2[1].y, x1.y, acc); acc = fmaf(w2[1].z, x1.z, acc); acc = fmaf(w2[1].w, x1.w, acc);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (j == 0) {
+      s.logit[c] = acc + bias2;
+      if (logits != nullptr && b < N) logits[(long long)b * CD_NC + c] = acc + bias2;
+    }
+  }
+  __syncthreads();
+  if (tid == 0 && b < N) {
+    float mx = s.logit[0];
+    int am = 0;
+#pragma unroll
+    for (int k = 1; k < CD_NC; ++k) if (s.logit[k] > mx) { mx = s.logit[k]; am = k; }
+    pred[b] = am;
+    if (label != nullptr) {
+      float se = 0.f;
+#pragma unroll
+      for (int k = 0; k < CD_NC; ++k) se += expf(s.logit[k] - mx);
+      // a label that is not an integer in [0, 10) (NaN included) scores NaN and is never counted correct; it indexes nothing
+      const float yl = label[b];
+      const bool ok = yl >= 0.f && yl < (float)CD_NC && yl == truncf(yl);
+      const int yi = ok ? (int)yl : 0;
+      loss[b] = ok ? -(s.logit[yi] - mx - logf(se)) : __int_as_float(0x7fc00000);
+      correct[b] = ok && yi == am ? 1 : 0;
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------ backward (data + conv0)
@@ -651,6 +790,17 @@ GX_API int gx_cnn_fwd_dense0(const float* x, const float* w0, const float* b0, c
   if (B < 2 || (B & 1) || B > 32) return -1;
   launch_pdl(cnn_fwd_dense0_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n,
              x_keep, g_cnn_dbg);
+  return GX_CHECK_LAUNCH();
+}
+// inference of the whole demo CNN (cnn_eval_kernel): x [N,1,28,28], the ten parameters in CNN_PARAM_SHAPES order; writes logits [N,10] (unless
+// null), pred [N] (int32 arg-max) and, when `label` [N] (float class ids) is given, loss [N] (softmax-CE) and correct [N] (int32 0 / 1).
+// Returns -1 without launching for N < 1.
+GX_API int gx_cnn_eval(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* wd0, const float* bd0,
+                       const float* wd1, const float* bd1, const float* wd2, const float* bd2, const float* label, float* logits, float* loss,
+                       int* pred, int* correct, int N, cudaStream_t s) {
+  if (N < 1) return -1;
+  launch_pdl(cnn_eval_kernel, dim3(N + (N & 1), 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd0, bd0, wd1, bd1, wd2, bd2, label, logits, loss, pred,
+             correct, N);
   return GX_CHECK_LAUNCH();
 }
 // accumulates into dw0 [16,25] / db0 [16] (atomics: zero them first)

@@ -25,6 +25,11 @@ With one rank and one party both PS tiers collapse into the arena optimizer insi
 
 The reference runs the same step as ~200 engine ops (per-image im2col+SGEMM) + 20 ZMQ round trips (SURVEY §3.3-3.4).
 The public API a user calls is ``step(X_host, y_host) -> loss`` (H2D of the batch from pinned memory, graph replay, D2H of the loss).
+
+The engine also scores its live weights: ``evaluate(X, y) -> (mean_loss, accuracy)`` (``evaluate_async`` returns a handle) and
+``predict(X) -> logits`` run the whole forward pass of any number of images, the per-sample softmax-CE and the arg-max as ONE launch
+(cnn_eval_kernel, csrc/kernels/cnn_direct.cu: the forward kernel's clusters of two images, extended by dense1 and the classifier), on
+buffers of their own, ordered on the current stream after the steps enqueued before it.
 """
 from __future__ import annotations
 
@@ -72,6 +77,22 @@ class LossHandle:
         return float(self._host.sum()) / self._host.numel()
 
     asscalar = item
+
+
+class EvalHandle:
+    """Result of ``HipsCNNTrainStep.evaluate_async``: the fp64 loss sum and the count of correct samples in pinned host memory + the event
+    that guards them.  ``wait()`` / ``item()`` synchronise on that event and return ``(mean_loss, accuracy)``."""
+
+    __slots__ = ("_host", "_event", "_n")
+
+    def __init__(self, host, event, n):
+        self._host, self._event, self._n = host, event, n
+
+    def wait(self):
+        self._event.synchronize()
+        return float(self._host[0]) / self._n, float(self._host[1]) / self._n
+
+    item = wait
 
 
 class HipsCNNTrainStep:
@@ -202,6 +223,7 @@ class HipsCNNTrainStep:
         self.use_graph = use_graph
         self.steps_done = 0
         self.kernels_per_step = 0
+        self._ev = None             # evaluate / predict buffers (never shared with the step), grown to the largest N seen
 
     # ------------------------------------------------------------------------------------------------------------
     def _init_params(self, net):
@@ -587,6 +609,65 @@ class HipsCNNTrainStep:
     def step(self, X, y):
         """Public API: one training step; returns the mean loss as a Python float (forces the D2H read of the per-sample loss)."""
         return self.step_async(X, y).item()
+
+    # evaluation -----------------------------------------------------------------------------------------------------
+    def _eval_launch(self, X, y, want_logits=False):
+        """Stage ``X`` (and ``y``) and issue the one-launch forward pass of the live weights (``native.cnn_eval``) on the current stream.
+        Returns N, the logits (a new tensor, or None), the per-sample loss and the correct flags (None without ``y``)."""
+        X = X._t if isinstance(X, NDArray) else X
+        y = y._t if isinstance(y, NDArray) else y
+        N = int(X.shape[0]) if X.dim() > 0 else 0
+        if N < 1 or X.numel() != N * 784:
+            raise ValueError("X must be (N, 1, 28, 28) or (N, 784) with N >= 1, got %s" % (tuple(X.shape),))
+        if y is not None and y.numel() != N:
+            raise ValueError("y must hold one label per image: %d labels for %d images" % (y.numel(), N))
+        ev = self._ev
+        if ev is None or ev["cap"] < N:
+            e = lambda n, dt=torch.float32: torch.empty(n, dtype=dt, device=self.device)
+            ev = self._ev = {"cap": N, "x": e(N * 784), "label": e(N), "loss": e(N), "pred": e(N, torch.int32), "correct": e(N, torch.int32)}
+
+        def staged(t, buf):          # CUDA fp32 contiguous: used in place; anything else is copied (async from pinned memory) and converted
+            if t.is_cuda and t.device == self.device and t.dtype == torch.float32 and t.is_contiguous():
+                return t
+            return buf.copy_(t.reshape(buf.shape), non_blocking=True)
+
+        x = staged(X, ev["x"][:N * 784].view(N, 1, 28, 28))
+        label = None if y is None else staged(y, ev["label"][:N])
+        loss, correct = (None, None) if y is None else (ev["loss"][:N], ev["correct"][:N])
+        logits = torch.empty(N, 10, dtype=torch.float32, device=self.device) if want_logits else None
+        native.cnn_eval(x, *self.P, label, logits, loss, ev["pred"][:N], correct)
+        return N, logits, loss, correct
+
+    def evaluate_async(self, X, y):
+        """Public API: score the **live** weights (``self.P``: the fabric's parameter arena with ``update='server'``, the worker's own
+        ``Wl`` with ``update='local'`` / HFA) on ``X`` (N,1,28,28) or (N,784) and labels ``y`` (N,), float or int, for any N >= 1, and return
+        an :class:`EvalHandle` without waiting for the GPU.  ``X`` / ``y`` may be host tensors (pinned: async H2D), CUDA tensors (used in
+        place when contiguous fp32) or NDArrays.
+
+        The whole forward pass, per-sample softmax-CE loss and arg-max run as ONE kernel launch (``cnn_eval_kernel``) on the current stream,
+        so it sees the weights after every step enqueued before it: with ``lookahead=True`` the weights after the last completed update (the
+        next batch's convolutions, already run, do not change them); the overlapped exchange channels are joined into that stream within the
+        step.  Evaluation has buffers of its own and writes nothing the training step reads.  A label that is not an integer in [0, 10)
+        scores a NaN loss and counts as wrong.  The totals are summed from the per-sample results in a fixed order: the loss in fp64, the
+        correct samples as an exact integer count.  Rank-local: each rank scores what it is given."""
+        if y is None:
+            raise ValueError("evaluate needs labels; predict(X) gives the logits alone")
+        N, _, loss, correct = self._eval_launch(X, y)
+        tot = torch.stack((loss.double().sum(), correct.sum().double()))
+        host = torch.empty(2, dtype=torch.float64).pin_memory()
+        host.copy_(tot, non_blocking=True)
+        event = torch.cuda.Event()
+        event.record()
+        return EvalHandle(host, event, N)
+
+    def evaluate(self, X, y):
+        """Public API: ``evaluate_async(X, y).item()`` — ``(mean_loss, accuracy)`` of the live weights as Python floats."""
+        return self.evaluate_async(X, y).item()
+
+    def predict(self, X):
+        """Public API: logits [N, 10] (a new CUDA tensor) of the live weights for ``X`` (N,1,28,28) or (N,784); one launch on the current
+        stream, ordered after the steps enqueued before it, as in :meth:`evaluate_async`."""
+        return self._eval_launch(X, None, want_logits=True)[1]
 
     # reference semantics helpers ------------------------------------------------------------------------------------
     def params_numpy(self):

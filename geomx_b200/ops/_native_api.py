@@ -168,6 +168,32 @@ def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None
     return True
 
 
+def cnn_eval(x, w0, b0, w1, b1, wd0, bd0, wd1, bd1, wd2, bd2, label, logits, loss, pred, correct):
+    """Inference of the whole demo CNN for N >= 1 images in one launch (cnn_eval_kernel, csrc/kernels/cnn_direct.cu), fp32 FMA: x [N,1,28,28]
+    or [N,784], the ten parameters in ``CNN_PARAM_SHAPES`` order.  Writes logits [N,10] fp32 (skipped when None) and pred [N] int32 (arg-max);
+    with ``label`` [N] fp32 (class ids) also loss [N] fp32 (softmax-CE; NaN for a label that is not an integer in [0, 10)) and correct [N]
+    int32 (1 where pred == label).  ``label=None`` (predict only) leaves ``loss`` / ``correct`` unwritten; they may be None then."""
+    N = x.shape[0]
+    if N < 1:
+        raise ValueError("cnn_eval needs at least one image")
+    shapes = [(16, 1, 5, 5), (16,), (32, 16, 5, 5), (32,), (256, 512), (256,), (128, 256), (128,), (10, 128), (10,)]
+    for t, s in zip((w0, b0, w1, b1, wd0, bd0, wd1, bd1, wd2, bd2), shapes):
+        assert t.numel() == math.prod(s), ("parameter shape", tuple(t.shape), s)
+        _f32c(t)
+    assert x.numel() == N * 784, ("images must be [N,1,28,28] or [N,784]", tuple(x.shape))
+    _f32c(x)
+    outs = [(pred, torch.int32, (N,))]
+    if logits is not None:
+        outs.append((logits, torch.float32, (N, 10)))
+    if label is not None:
+        outs += [(label, torch.float32, (N,)), (loss, torch.float32, (N,)), (correct, torch.int32, (N,))]
+    for t, dt, s in outs:
+        assert t is not None and t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == math.prod(s), \
+            ("expected contiguous CUDA %s of %d elements" % (dt, math.prod(s)), None if t is None else (t.dtype, tuple(t.shape)))
+    _ck(_lib().gx_cnn_eval(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(wd0), _p(bd0), _p(wd1), _p(bd1), _p(wd2), _p(bd2), _p(label), _p(logits),
+                           _p(loss), _p(pred), _p(correct), N, _s()), "cnn_eval")
+
+
 def cnn_bwd(x, w1, a1, idx1, a2, idx2, da2, dw0, db0):
     """conv1 data gradient + pool/ReLU backward of both layers + conv0 weight / bias gradient (accumulated with atomics into dw0 / db0)."""
     _ck(_lib().gx_cnn_bwd(_p(x), _p(w1), _p(a1), _p(idx1), _p(a2), _p(idx2), _p(da2), _p(dw0), _p(db0), x.shape[0], _s()), "cnn_bwd")

@@ -16,6 +16,7 @@ SIGS = {
     "gx_cnn_wgrad1": [P] * 6 + [I, P],
     "gx_cnn_bwd_all": [P] * 11 + [I, P],
     "gx_cnn_bwd_exchange": [P] * 11 + [I, P, P, I, P],
+    "gx_cnn_eval": [P] * 16 + [I, P],
     "gx_depthwise_fwd": [P, P, P, P] + [I] * 11 + [P],
     "gx_depthwise_dgrad": [P, P, P] + [I] * 10 + [P],
     "gx_depthwise_wgrad": [P, P, P, P] + [I] * 10 + [P],
