@@ -247,6 +247,8 @@ class HipsCNNTrainStep:
         f.load_master_from_param()
         if self.update == "local":
             self.Wl.copy_(f.param.tensor)
+            if self._local_spec["name"] == "dcasgd":
+                self.s1l.copy_(self.Wl)      # DCASGD's previous weight starts as the initial weight (reference create_state)
         if net is not None:  # re-home the Gluon parameters onto the live arena (zero-copy pull)
             for i, p in enumerate(net.collect_params().values()):
                 d = p.data()
@@ -277,9 +279,12 @@ class HipsCNNTrainStep:
         if self.update == "local":
             sp = self._local_spec
             clip = sp.get("clip_gradient", -1.0)
+            # HFA applies the optimizer to the worker's own gradient arena, a sum over the batch: the reference's cnn_hfa.py steps the
+            # trainer with `trainer.step(num_samples)`, i.e. rescale_grad / B.  The pulled aggregate of the other local mode is already averaged.
+            rescale = sp["rescale_grad"] / B if self.hfa else sp["rescale_grad"]
 
             def local_opt(grad_tensor, zero=None):
-                n.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], sp["rescale_grad"],
+                n.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], rescale,
                             -1.0 if clip is None else clip, sp.get("momentum", 0.0), sp.get("beta1", 0.9), sp.get("beta2", 0.999), sp.get("epsilon", 1e-8),
                             sp.get("lamda", 0.04), self.opt_state, zero)
             if self.hfa:

@@ -395,6 +395,13 @@ class HipsFabric:
     def load_master_from_param(self):
         """Global owners adopt the (already broadcast) parameter arena as master weights — the `init` handshake."""
         self.w.copy_(self.param.tensor)
+        self.init_dcasgd_previous_weight()
+
+    def init_dcasgd_previous_weight(self):
+        """DCASGD's previous weight (state slot ``s1``) starts as the current master weight, as the reference's ``create_state`` makes it
+        (``(mom, weight.copy())``); a zero start would add ``lamda * g^2 * w`` to the first update."""
+        if self.opt_spec is not None and self.opt_spec.get("name") == "dcasgd":
+            self.s1.copy_(self.w)
 
     # -- parameter block ------------------------------------------------------------------------------------------------
     def _hyper(self):

@@ -108,6 +108,7 @@ class KVStoreFabric(KVStoreBase):
             self._opt_spec, self._host_optimizer = None, optimizer
         if self._fabric is not None:
             self._fabric.set_optimizer(self._opt_spec)
+            self._fabric.init_dcasgd_previous_weight()      # the reference's servers create the new optimizer's state from the current weight
             if self._host_optimizer is not None:
                 from .. import optimizer as opt
                 self._host_updater = opt.get_updater(self._host_optimizer)
