@@ -5,13 +5,15 @@
 //                       image: each CTA computes a quarter of conv0 and shares it through distributed shared memory, so conv0 runs once
 //                       (cnn_fwd_dense0_kernel, even batches <= 32: the same, in clusters of two images, followed by the first dense
 //                       layer a2 -> a3, so that the dense-chain cluster kernel starts from a3)
-//   cnn_bwd_all_kernel  one heterogeneous grid: CTAs [128, 128+4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1 data gradient gathered
-//                       from the non-zeros of dz2 + pool/ReLU backward of both layers + conv0 weight gradient), CTAs [0, 128)  da2, a1 -> dW1, db1
-//                       (conv1 weight gradient); both exploit the sparsity of dz2 (one non-zero per pooling window).  Both bodies resolve
+//   cnn_bwd_all_kernel  one heterogeneous grid in clusters of two: CTAs [256, 256+4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1
+//                       data gradient gathered from the non-zeros of dz2 + pool/ReLU backward of both layers + conv0 weight gradient), CTAs
+//                       [0, 256)  da2, a1 -> dW1, db1 (conv1 weight gradient, each cluster's two CTAs splitting the batch and combining their
+//                       sums in shared memory); both exploit the sparsity of dz2 (one non-zero per pooling window).  Both bodies resolve
 //                       the programmatic grid dependency only AFTER the staging that does not depend on the preceding kernel, so the CTAs
-//                       become resident and stage while that kernel still runs.
+//                       become resident and stage while that kernel still runs — at B <= 32 the whole grid, in one wave.
 //                       (cnn_bwd_kernel / cnn_wgrad1_kernel: the same bodies as separate launches; cnn_bwd_exchange_kernel: the same bodies
-//                       in one grid (data-gradient CTAs first) whose last CTAs also perform the conv keys' exchange — measured, no gain, opt-in.)
+//                       in one grid without clusters (data-gradient CTAs first, one weight-gradient CTA per output slice) whose last CTAs also
+//                       perform the conv keys' exchange — measured, no gain, opt-in.)
 // and, for inference, ONE launch for any number of images:
 //   cnn_eval_kernel     x -> logits, softmax-CE loss, arg-max and correct flag per image: the convolutions and dense0 of cnn_fwd_dense0_kernel
 //                       (clusters of two images, without the stores only the backward pass needs), then dense1 and the classifier in the
@@ -455,6 +457,7 @@ struct CnnBwdSmem {
   static constexpr int TOTAL = NZCNT + 16;
   static constexpr int BYTES = TOTAL * 4;
 };
+constexpr int CNN_BWD_CTA_STAMPS = 320;   // CTAs of cnn_bwd_all_kernel that record (start, end, SM) in the debug buffer (see there)
 
 __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int cg, const float* __restrict__ x, const float* __restrict__ w1,
                                              const float* __restrict__ a1, const unsigned char* __restrict__ idx1, const float* __restrict__ a2,
@@ -574,63 +577,118 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
 }
 
 // ------------------------------------------------------------------------------------------------------------------ conv1 weight gradient
-// grid (32 oc, 4 cg), 256 threads.  CTA owns dW1[oc][4cg..4cg+3][5][5] (100 outputs, written once: no atomics) and sums over all images:
+// CTA (oc, cg, h), 256 threads, owns dW1[oc][4cg..4cg+3][5][5] (100 outputs, written once: no atomics) over images [h NI, (h+1) NI):
 //   dW1[oc][c][kh][kw] = sum_{b, window} g[b][oc][window] * a1[b][c][oh+kh][ow+kw]     (g != 0 only at the window's arg-max where a2 > 0)
-__device__ __forceinline__ void cnn_wgrad1_body(float* sm, const int oc, const int cg, const float* __restrict__ a1, const float* __restrict__ a2,
-                                                const unsigned char* __restrict__ idx2, const float* __restrict__ da2, float* __restrict__ dw1,
-                                                float* __restrict__ db1, int B, unsigned long long* dbg) {
-  float* sa = sm;                               // [B][4][144] the four input-channel planes of every image
-  float* sg = sa + (size_t)B * 576;             // [B*16] routed gradients of this output channel
-  int* sp = reinterpret_cast<int*>(sg + B * 16);  // [B*16] arg-max position as offset into a 12x12 plane
-  float* sacc = reinterpret_cast<float*>(sp + B * 16);   // [2][128]
-  const bool dbg_on = dbg != nullptr && oc == 0 && cg == 0 && threadIdx.x == 0;
+// PAIR: NI = B / 2 and the two CTAs h = 0, 1 of a cluster of two split the batch (half the staging, half the sums per CTA); h = 1 pushes its
+// 100 partial sums (and db1's) into h = 0 (st.async, transaction mbarrier), which adds them in the order h0 + h1 and stores.  Otherwise
+// NI = B, h = 0.  Where g can be non-zero (a2 > 0) is known from the forward pass: the staging lists those (image, window) entries in
+// ascending order, with the arg-max pixel's offset into the staged planes, so that after the grid dependency only their da2 values are
+// loaded and only they are summed.
+__host__ __device__ constexpr int wgrad1_list(int ni) { return ni * 16 + 8; }       // entry list, padded for the 2 x 4-way split below
+// dynamic shared memory of the body for NI images: planes, list values + positions, warp counts, partials, received partials, mbarrier
+__host__ __device__ constexpr int wgrad1_smem_bytes(int ni) { return (ni * 576 + 2 * wgrad1_list(ni) + 16 + 256 + 128 + 4) * 4; }
+
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive;" ::: "memory"); }   // (release)
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait;" ::: "memory"); }       // (acquire)
+
+template <bool PAIR>
+__device__ __forceinline__ void cnn_wgrad1_body(float* sm, const int oc, const int cg, const int h, const float* __restrict__ a1,
+                                                const float* __restrict__ a2, const unsigned char* __restrict__ idx2, const float* __restrict__ da2,
+                                                float* __restrict__ dw1, float* __restrict__ db1, int B, unsigned long long* dbg) {
+  const int ni = PAIR ? B / 2 : B, b0 = h * ni, L = wgrad1_list(ni);
+  float* sa = sm;                                      // [ni][4][144] the four input-channel planes of every image
+  float* sg = sa + ni * 576;                           // [L] listed entries: da2 offset (int bits) until the grid dependency, then g
+  int* sp = reinterpret_cast<int*>(sg + L);            // [L] arg-max pixel as offset into sa (image * 576 + offset in a 12x12 plane)
+  int* scnt = sp + L;                                  // [8] per-warp entry counts of one listing round
+  float* sacc = reinterpret_cast<float*>(scnt + 16);   // [2][128]
+  float* srecv = sacc + 256;                           // PAIR, h = 0: the partner's 100 partial sums, db1's at [100]
+  uint64_t* bar = reinterpret_cast<uint64_t*>(srecv + 128);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool dbg_on = dbg != nullptr && oc == 0 && cg == 0 && h == 0 && tid == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
   stamp(16);
-  const int tid = threadIdx.x;
-  for (int i = tid; i < B * 144; i += 256) {          // 144 float4 per image: 4 contiguous planes
-    const int bb = i / 144, r = i % 144;
-    cpa16(sa + 4 * i, a1 + ((long long)bb * CD_C1 + 4 * cg) * 144 + 4 * r);
+  if (PAIR) {
+    if (h == 0 && tid == 0) {
+      mbar_init(bar, 1);
+      mbar_arrive_expect_tx(bar, (cg == 0 ? 26 : 25) * 16);    // 25 float4 of dW1 partials (+ one carrying db1's)
+      fence_barrier_init();
+    }
+    cluster_arrive();        // h = 1 pushes only after its wait for this arrive: the barrier above is armed by then
   }
-  for (int e = tid; e < B * 16; e += 256) {
-    const int bb = e >> 4, win = e & 15;
-    const int id = idx2[((long long)bb * CD_C2 + oc) * 16 + win];
-    sp[e] = (2 * (win >> 2) + (id >> 1)) * CD_P1 + 2 * (win & 3) + (id & 1);
+  for (int i = tid; i < ni * 144; i += 256) {          // 144 float4 per image: 4 contiguous planes
+    const int bb = i / 144, r = i - bb * 144;
+    cpa16(sa + 4 * i, a1 + ((long long)(b0 + bb) * CD_C1 + 4 * cg) * 144 + 4 * r);
   }
+  // the list: rounds of 256 entries, each thread one entry, ranked by warp ballots and the counts of the warps before it
+  int n = 0;
+  for (int base = 0; base < ni * 16; base += 256) {
+    const int e = base + tid, bb = e >> 4, win = e & 15;
+    const int src = ((b0 + bb) * CD_C2 + oc) * 16 + win;
+    const bool nz = e < ni * 16 && a2[src] > 0.f;
+    const unsigned m = __ballot_sync(0xffffffffu, nz);
+    if (lane == 0) scnt[warp] = __popc(m);
+    __syncthreads();
+    int k = n, tot = n;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) { const int c = scnt[w]; k += w < warp ? c : 0; tot += c; }
+    if (nz) {
+      const int id = idx2[src];
+      k += __popc(m & ((1u << lane) - 1u));
+      sg[k] = __int_as_float(src);
+      sp[k] = bb * 576 + (2 * (win >> 2) + (id >> 1)) * CD_P1 + 2 * (win & 3) + (id & 1);
+    }
+    n = tot;
+    __syncthreads();         // (scnt is rewritten by the next round)
+  }
+  if (tid < 8) { sg[n + tid] = 0.f; sp[n + tid] = 0; }   // pad to a multiple of 8 with entries that add 0
   pdl_wait();            // (see cnn_bwd_body: only da2 depends on the preceding kernel)
   pdl_launch();
-  for (int e = tid; e < B * 16; e += 256) {
-    const long long o = ((long long)(e >> 4) * CD_C2 + oc) * 16 + (e & 15);
-    sg[e] = a2[o] > 0.f ? da2[o] : 0.f;
-  }
+  for (int k = tid; k < n; k += 256) sg[k] = da2[__float_as_int(sg[k])];
   cpa_wait_all();
   __syncthreads();
   stamp(17);
-  const int half = tid >> 7, t = tid & 127;
+  // thread -> (input channel cl, tap) = t < 100, half q of the list; four independent accumulators per thread
+  const int q = tid >> 7, t = tid & 127, hn = ((n + 7) & ~7) >> 1;
   float acc = 0.f;
   if (t < 100) {
     const int cl = t / 25, tap = t % 25, koff = (tap / 5) * CD_P1 + tap % 5;
-    const int e0 = half * (B * 8), e1 = e0 + B * 8;      // images [half*B/2, (half+1)*B/2)
-    // four independent accumulators (the chain of B*8 dependent FMAs was the critical path of this phase)
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
     const float* sak = sa + cl * 144 + koff;
 #pragma unroll 2
-    for (int e = e0; e < e1; e += 4) {       // B*8 is a multiple of 16; e .. e+3 belong to the same image
-      const float* img = sak + (e >> 4) * 576;
-      c0 = fmaf(sg[e], img[sp[e]], c0);
-      c1 = fmaf(sg[e + 1], img[sp[e + 1]], c1);
-      c2 = fmaf(sg[e + 2], img[sp[e + 2]], c2);
-      c3 = fmaf(sg[e + 3], img[sp[e + 3]], c3);
+    for (int k = q * hn; k < (q + 1) * hn; k += 4) {    // hn is a multiple of 4: float4 / int4 reads of the list
+      const float4 g = *reinterpret_cast<const float4*>(sg + k);
+      const int4 p = *reinterpret_cast<const int4*>(sp + k);
+      c0 = fmaf(g.x, sak[p.x], c0);
+      c1 = fmaf(g.y, sak[p.y], c1);
+      c2 = fmaf(g.z, sak[p.z], c2);
+      c3 = fmaf(g.w, sak[p.w], c3);
     }
     acc = (c0 + c1) + (c2 + c3);
   }
-  sacc[half * 128 + t] = acc;
+  sacc[q * 128 + t] = acc;
   __syncthreads();
-  if (tid < 100) dw1[((long long)oc * CD_C1 + 4 * cg + tid / 25) * 25 + tid % 25] = sacc[tid] + sacc[128 + tid];
-  if (cg == 0 && tid < 32) {                 // db1[oc] = sum of all routed gradients of this channel
-    float s = 0.f;
-    for (int e = tid; e < B * 16; e += 32) s += sg[e];
+  float s = 0.f;                                       // warp 7, cg == 0: db1's part = sum of the listed routed gradients
+  if (cg == 0 && warp == 7) {
+    for (int k = lane; k < n; k += 32) s += sg[k];
     s = warp_sum(s);
-    if (tid == 0) db1[oc] = s;
+  }
+  float* dst = dw1 + ((long long)oc * CD_C1 + 4 * cg) * 25;
+  if (!PAIR) {
+    if (tid < 100) dst[tid] = sacc[tid] + sacc[128 + tid];
+    if (cg == 0 && tid == 224) db1[oc] = s;
+  } else if (h == 1) {
+    cluster_wait();
+    if (tid < 25) {
+      const float4 v = make_float4(sacc[4 * tid] + sacc[128 + 4 * tid], sacc[4 * tid + 1] + sacc[129 + 4 * tid],
+                                   sacc[4 * tid + 2] + sacc[130 + 4 * tid], sacc[4 * tid + 3] + sacc[131 + 4 * tid]);
+      push_all<2, 1>(srecv, 4 * tid, bar, 1, v);
+    }
+    if (cg == 0 && tid == 224) push_all<2, 1>(srecv, 100, bar, 1, make_float4(s, 0.f, 0.f, 0.f));
+  } else {
+    cluster_wait();
+    wait_landed(bar);
+    if (tid < 100) dst[tid] = (sacc[tid] + sacc[128 + tid]) + srecv[tid];
+    if (cg == 0 && tid == 224) db1[oc] = s + srecv[100];
   }
   stamp(18);
 }
@@ -640,41 +698,49 @@ __global__ void __launch_bounds__(288) cnn_bwd_kernel(const float* x, const floa
   extern __shared__ __align__(16) float sm[];
   cnn_bwd_body(sm, blockIdx.x, blockIdx.y, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dbg);
 }
-__global__ void __launch_bounds__(256) cnn_wgrad1_kernel(const float* a1, const float* a2, const unsigned char* idx2, const float* da2, float* dw1,
-                                                          float* db1, int B, unsigned long long* dbg) {
+// grid (32 oc, 4 cg, 2 h), 256 threads, clusters of (1, 1, 2): the two CTAs that split the batch for one (oc, cg)
+__global__ void __cluster_dims__(1, 1, 2) __launch_bounds__(256) cnn_wgrad1_kernel(const float* a1, const float* a2, const unsigned char* idx2,
+                                                                                    const float* da2, float* dw1, float* db1, int B,
+                                                                                    unsigned long long* dbg) {
   extern __shared__ __align__(16) float sm[];
-  cnn_wgrad1_body(sm, blockIdx.x, blockIdx.y, a1, a2, idx2, da2, dw1, db1, B, dbg);
+  cnn_wgrad1_body<true>(sm, blockIdx.x, blockIdx.y, blockIdx.z, a1, a2, idx2, da2, dw1, db1, B, dbg);
 }
-// The whole convolution backward pass as ONE launch: CTAs [0, 128) run the conv1 weight-gradient body, CTAs [128, 128 + 4B) the data-gradient /
-// conv0 body (two independent jobs that read the same inputs; a single heterogeneous grid saves a stream fork / join in the step graph).
-// The weight-gradient CTAs come first: CTAs are dispatched in index order and, while the dense-chain cluster runs, only part of the grid
-// becomes resident; the weight-gradient body is the longer one after its grid dependency resolves, so it is the one that should be resident
-// and staged by then.
-__global__ void __launch_bounds__(288) cnn_bwd_all_kernel(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2,
-                                                           const unsigned char* idx2, const float* da2, float* dw0, float* db0, float* dw1, float* db1,
-                                                           int B, unsigned long long* dbg) {
+// The whole convolution backward pass as ONE launch, in clusters of two CTAs: CTAs [0, 256) run the conv1 weight-gradient body (CTA
+// 8 oc + 2 cg + h: pairs of CTAs that split the batch), CTAs [256, 256 + 4B) the data-gradient / conv0 body (CTA 256 + 4 b + cg; a cluster
+// never mixes the two bodies, and the data-gradient CTAs do not use theirs).  Two independent jobs that read the same inputs; a single
+// heterogeneous grid saves a stream fork / join in the step graph.  The grid's dynamic shared memory is the larger body's: at B <= 32 the
+// data-gradient body's 41,344 bytes, so that the whole grid is resident at once (5 CTAs per SM, one beside each CTA of the dense-chain
+// cluster) while the dense chain still runs, and every CTA has finished its staging when da2 arrives.
+__global__ void __launch_bounds__(288) __cluster_dims__(2, 1, 1)
+    cnn_bwd_all_kernel(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2, const unsigned char* idx2,
+                       const float* da2, float* dw0, float* db0, float* dw1, float* db1, int B, unsigned long long* dbg) {
   extern __shared__ __align__(16) float sm[];
   const int i = blockIdx.x;      // (the grid dependency is resolved inside the bodies, after their independent staging)
-  // debug: every CTA records (start, end, SM id) at dbg[64 + 3 i ..] so that tools/step_timeline.py can show how the grid packs onto the SMs
+  // debug: the last CNN_BWD_CTA_STAMPS CTAs record (start, end, SM id) at dbg[64 + 3 k ..], k = i - (grid - CNN_BWD_CTA_STAMPS) (all CTAs of
+  // a smaller grid: k = i), so that tools/step_timeline.py can show how the grid packs onto the SMs; slots stay below 64 + 3 * 320 = 1024
   unsigned long long t0 = 0;
   if (dbg != nullptr && threadIdx.x == 0) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t0));
-  if (i >= 4 * CD_C2) {
-    const int j = i - 4 * CD_C2;
+  if (i >= 8 * CD_C2) {
+    const int j = i - 8 * CD_C2;
     cnn_bwd_body(sm, j >> 2, j & 3, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dbg);
   } else if (threadIdx.x < 256) {            // (no thread of this CTA takes the other branch, so its __syncthreads pair up among these 256)
-    cnn_wgrad1_body(sm, i >> 2, i & 3, a1, a2, idx2, da2, dw1, db1, B, dbg);
+    cnn_wgrad1_body<true>(sm, i >> 3, (i >> 1) & 3, i & 1, a1, a2, idx2, da2, dw1, db1, B, dbg);
+  } else {                                   // threads 256..287 take part in the pair's cluster barrier, which would otherwise wait for them
+    cluster_arrive();
+    cluster_wait();
   }
-  if (dbg != nullptr && threadIdx.x == 0) {
+  const int k = i - max((int)gridDim.x - CNN_BWD_CTA_STAMPS, 0);
+  if (dbg != nullptr && threadIdx.x == 0 && k >= 0) {
     unsigned long long t1; unsigned smid;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t1));
     asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-    dbg[64 + 3 * i] = t0; dbg[65 + 3 * i] = t1; dbg[66 + 3 * i] = smid;
+    dbg[64 + 3 * k] = t0; dbg[65 + 3 * k] = t1; dbg[66 + 3 * k] = smid;
   }
 }
 
 // The convolution backward pass AND the exchange of the four conv keys (push -> both server tiers -> optimizer -> pull, the replicated one-hop
-// mode of hips_fabric.cu's direct protocol) as ONE launch.  The bodies of cnn_bwd_all_kernel: CTAs [0, 4B) data gradient, [4B, 4B+128) conv1
-// weight gradient.  Every CTA takes a ticket when its
+// mode of hips_fabric.cu's direct protocol) as ONE launch.  The bodies of cnn_bwd_all_kernel, without clusters: CTAs [0, 4B) data gradient,
+// [4B, 4B+128) conv1 weight gradient, one CTA per (oc, cg) over the whole batch.  Every CTA takes a ticket when its
 // gradients are written; the CTAs that draw the last `n_active` tickets wait until the ticket counter shows that the whole grid has finished
 // and then each serve one 1024-float tile of the conv keys: gradient -> LL packets into every rank's slot, poll the packets of all ranks, sum
 // in the hierarchy's order (party sums, push_scale, sum over parties), optimizer on this rank's replica of the server state, fresh weights
@@ -693,7 +759,7 @@ __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, c
     cnn_bwd_body(sm, i >> 2, i & 3, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dbg);
   } else if (threadIdx.x < 256) {
     const int j = i - 4 * B;
-    cnn_wgrad1_body(sm, j >> 2, j & 3, a1, a2, idx2, da2, dw1, db1, B, dbg);
+    cnn_wgrad1_body<false>(sm, j >> 2, j & 3, 0, a1, a2, idx2, da2, dw1, db1, B, dbg);
   }
   if (threadIdx.x >= FAB_THREADS) return;                       // the exchange tail is written for 256 threads (one float4 of a tile each)
   // the channel's round / optimizer step (they can only advance after every CTA of this launch has drawn its ticket below)
@@ -816,34 +882,67 @@ GX_API int gx_cnn_bwd(const float* x, const float* w1, const float* a1, const un
   launch_pdl(cnn_bwd_kernel, dim3(B, 4), dim3(288), (size_t)CnnBwdSmem::BYTES, s, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, g_cnn_dbg);
   return GX_CHECK_LAUNCH();
 }
-// overwrites dw1 [32,16,5,5] and db1 [32].  B even, B <= 64 (shared-memory planes of all images).
+// overwrites dw1 [32,16,5,5] and db1 [32].  B even, B <= 64 (shared-memory planes of half the images per CTA).
 GX_API int gx_cnn_wgrad1(const float* a1, const float* a2, const unsigned char* idx2, const float* da2, float* dw1, float* db1, int B, cudaStream_t s) {
   if (B < 2 || (B & 1) || B > 64) return -1;
-  const size_t smem = ((size_t)B * 576 + (size_t)B * 16 * 2 + 256) * 4;
+  const size_t smem = (size_t)wgrad1_smem_bytes(B / 2);
   static size_t attr = 0;
   if (smem > attr) {
     cudaError_t e = cudaFuncSetAttribute(cnn_wgrad1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     attr = smem;
   }
-  launch_pdl(cnn_wgrad1_kernel, dim3(CD_C2, 4), dim3(256), smem, s, a1, a2, idx2, da2, dw1, db1, B, g_cnn_dbg);
+  launch_pdl(cnn_wgrad1_kernel, dim3(CD_C2, 4, 2), dim3(256), smem, s, a1, a2, idx2, da2, dw1, db1, B, g_cnn_dbg);
   return GX_CHECK_LAUNCH();
 }
 
-// conv backward in one launch (see cnn_bwd_all_kernel): accumulates dw0 / db0 (zero them first), overwrites dw1 / db1.  B even, <= 64.
-GX_API int gx_cnn_bwd_all(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2, const unsigned char* idx2,
-                          const float* da2, float* dw0, float* db0, float* dw1, float* db1, int B, cudaStream_t s) {
-  if (B < 2 || (B & 1) || B > 64) return -1;
-  const size_t smem_w = ((size_t)B * 576 + (size_t)B * 16 * 2 + 256) * 4;
-  const size_t smem = smem_w > (size_t)CnnBwdSmem::BYTES ? smem_w : (size_t)CnnBwdSmem::BYTES;
+// grid and dynamic shared memory of cnn_bwd_all_kernel at batch B (0 for batches it does not cover)
+static int bwd_all_grid(int B) { return 8 * CD_C2 + 4 * B; }
+static size_t bwd_all_smem(int B) {
+  const size_t w = (size_t)wgrad1_smem_bytes(B / 2);
+  return w > (size_t)CnnBwdSmem::BYTES ? w : (size_t)CnnBwdSmem::BYTES;
+}
+static int bwd_all_prepare(size_t smem) {
   static size_t attr = 0;
   if (smem > attr) {
     cudaError_t e = cudaFuncSetAttribute(cnn_bwd_all_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     attr = smem;
   }
-  launch_pdl(cnn_bwd_all_kernel, dim3(4 * B + 4 * CD_C2), dim3(288), smem, s, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1, B, g_cnn_dbg);
+  return 0;
+}
+
+// conv backward in one launch (see cnn_bwd_all_kernel): accumulates dw0 / db0 (zero them first), overwrites dw1 / db1.  B even, <= 64.
+GX_API int gx_cnn_bwd_all(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2, const unsigned char* idx2,
+                          const float* da2, float* dw0, float* db0, float* dw1, float* db1, int B, cudaStream_t s) {
+  if (B < 2 || (B & 1) || B > 64) return -1;
+  const size_t smem = bwd_all_smem(B);
+  if (int e = bwd_all_prepare(smem)) return e;
+  launch_pdl(cnn_bwd_all_kernel, dim3(bwd_all_grid(B)), dim3(288), smem, s, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1, B, g_cnn_dbg);
   return GX_CHECK_LAUNCH();
+}
+
+// how cnn_bwd_all_kernel runs at batch B, for tests and tools: out[0] CTAs of the grid, [1] its dynamic shared memory (bytes), [2] the
+// data-gradient body's, [3] the weight-gradient body's, [4] CTAs resident per SM on an idle device, [5] clusters of two resident at once
+// on the whole idle device (cudaOccupancyMaxActiveClusters), [6] registers per thread, [7] CTAs whose (start, end, SM) the debug buffer
+// records (the last ones of the grid).  Returns -1 for batches it does not cover.
+GX_API int gx_cnn_bwd_all_geometry(int B, int* out) {
+  if (B < 2 || (B & 1) || B > 64) return -1;
+  const size_t smem = bwd_all_smem(B);
+  if (int e = bwd_all_prepare(smem)) return e;
+  int per_sm = 0, clusters = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cnn_bwd_all_kernel, 288, smem);
+  if (e != cudaSuccess) return (int)e;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(bwd_all_grid(B)); cfg.blockDim = dim3(288); cfg.dynamicSmemBytes = smem;
+  e = cudaOccupancyMaxActiveClusters(&clusters, cnn_bwd_all_kernel, &cfg);
+  if (e != cudaSuccess) return (int)e;
+  cudaFuncAttributes fa;
+  e = cudaFuncGetAttributes(&fa, cnn_bwd_all_kernel);
+  if (e != cudaSuccess) return (int)e;
+  out[0] = bwd_all_grid(B); out[1] = (int)smem; out[2] = CnnBwdSmem::BYTES; out[3] = wgrad1_smem_bytes(B / 2);
+  out[4] = per_sm; out[5] = clusters; out[6] = fa.numRegs; out[7] = min(bwd_all_grid(B), CNN_BWD_CTA_STAMPS);
+  return 0;
 }
 
 // conv backward + exchange of the conv keys in one launch (see cnn_bwd_exchange_kernel).  `params`: FabricParams block of the channel
@@ -858,7 +957,7 @@ GX_API int gx_cnn_bwd_exchange(const float* x, const float* w1, const float* a1,
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (grid > 2 * sms) return -1;                                  // the ticket wait needs the whole grid resident (2 CTAs per SM)
-  const size_t smem_w = ((size_t)B * 576 + (size_t)B * 16 * 2 + 256) * 4;
+  const size_t smem_w = (size_t)wgrad1_smem_bytes(B);
   const size_t smem = smem_w > (size_t)CnnBwdSmem::BYTES ? smem_w : (size_t)CnnBwdSmem::BYTES;
   static size_t attr = 0;
   if (smem > attr) {

@@ -205,6 +205,20 @@ def cnn_bwd_all(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1):
         "cnn_bwd_all")
 
 
+def cnn_bwd_all_geometry(B):
+    """How ``cnn_bwd_all`` runs at batch ``B``: a dict of its grid (CTAs), dynamic shared memory, the two bodies' shared memory, CTAs resident
+    per SM and clusters of two resident on the whole idle device (occupancy queries), registers per thread, and how many of its last CTAs
+    record (start, end, SM) in the debug buffer.  None for batches it does not cover."""
+    import ctypes
+    out = (ctypes.c_int * 8)()
+    rc = _lib().gx_cnn_bwd_all_geometry(int(B), out)
+    if rc == -1:
+        return None
+    _ck(rc, "cnn_bwd_all_geometry")
+    keys = ("grid", "smem", "dgrad_smem", "wgrad_smem", "ctas_per_sm", "clusters", "regs", "stamped_ctas")
+    return dict(zip(keys, list(out)))
+
+
 def cnn_bwd_exchange(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1, params, tile_list, n_active):
     """``cnn_bwd_all`` whose last CTAs also perform the exchange of the conv keys (``params``: the channel's FabricParams block from
     ``HipsFabric.channel_fused_args``): convolution backward + push + server tiers + optimizer + pull in one launch."""

@@ -15,6 +15,7 @@ SIGS = {
     "gx_cnn_bwd": [P] * 9 + [I, P],
     "gx_cnn_wgrad1": [P] * 6 + [I, P],
     "gx_cnn_bwd_all": [P] * 11 + [I, P],
+    "gx_cnn_bwd_all_geometry": [I, P],
     "gx_cnn_bwd_exchange": [P] * 11 + [I, P, P, I, P],
     "gx_cnn_eval": [P] * 16 + [I, P],
     "gx_depthwise_fwd": [P, P, P, P] + [I] * 11 + [P],

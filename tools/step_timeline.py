@@ -64,6 +64,10 @@ def main():
     mlp_phases, mlp_labels = (TAIL_PHASES, TAIL_PHASE_LABELS) if tail else (MLP_PHASES, MLP_PHASE_LABELS)
     for c in chans:
         fab.state[c][3] = 1
+    # cnn_bwd_all: weight-gradient CTAs [0, 256) (pairs that split the batch), data-gradient CTAs [256, grid); its last `stamped_ctas` CTAs
+    # record (start, end, SM)
+    geo = native.cnn_bwd_all_geometry(32)
+    first = geo["grid"] - geo["stamped_ctas"]
     flush = torch.empty(64 * 1024 * 1024, device=dev)
     rows = []
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
@@ -85,8 +89,8 @@ def main():
             row["bwd tail"] = (c[20], c[24])
             row["_tail"] = [(v - c[20]) / 1e3 for v in c[20:25]]
         if not getattr(eng, "fused_exchange", False):
-            per = [(c[64 + 3 * i], c[65 + 3 * i], c[66 + 3 * i]) for i in range(256)]
-            row["_cta"] = per
+            # (start, end, SM) of the backward grid's CTAs [first, grid), keyed by CTA index
+            row["_cta"] = {first + k: (c[64 + 3 * k], c[65 + 3 * k], c[66 + 3 * k]) for k in range(geo["stamped_ctas"])}
         row["_ms"] = ev[0].elapsed_time(ev[1])
         row["_cnn_ph"] = {name: [(c[s1] - c[s0]) / 1e3 for s0, s1 in zip(slots, slots[1:])] for name, slots in cnn_phases.items()}
         row["_mlp_ph"] = [(m[s1] - m[s0]) / 1e3 for s0, s1 in zip(mlp_phases, mlp_phases[1:])]
@@ -104,25 +108,34 @@ def main():
         lines.append("  %-12s start %7.2f  end %7.2f  (dur %6.2f us)" % (k, statistics.median(rel0), statistics.median(rel1),
                                                                         statistics.median(b - a for a, b in zip(rel0, rel1))))
     if "_cta" in rows[0]:
-        # how the 256 CTAs of the convolution-backward grid pack onto the SMs (last sampled step)
+        # how the convolution-backward grid packs onto the SMs (last sampled step; the stamped CTAs only)
         r = rows[-1]
         base = min(v[0] for kk, v in r.items() if not kk.startswith("_") and v[0] > 0)
-        for name, lo, hi in (("wgrad CTAs (0..127)", 0, 128), ("bwd CTAs  (128..255)", 128, 256)):
-            st = sorted((a - base) / 1e3 for a, b, sm_ in r["_cta"][lo:hi]); en = sorted((b - base) / 1e3 for a, b, sm_ in r["_cta"][lo:hi])
-            du = sorted((b - a) / 1e3 for a, b, sm_ in r["_cta"][lo:hi])
+        for name, lo, hi in (("wgrad CTAs (%d..255)" % first, first, 256), ("bwd CTAs  (256..%d)" % (geo["grid"] - 1), 256, geo["grid"])):
+            cs = [r["_cta"][i] for i in range(max(lo, first), hi)]
+            st = sorted((a - base) / 1e3 for a, b, sm_ in cs); en = sorted((b - base) / 1e3 for a, b, sm_ in cs)
+            du = sorted((b - a) / 1e3 for a, b, sm_ in cs)
+            m = len(cs) // 2
             lines.append("  %-22s start min/med/max %.2f %.2f %.2f | end %.2f %.2f %.2f | duration %.2f %.2f %.2f" % (
-                name, st[0], st[64], st[-1], en[0], en[64], en[-1], du[0], du[64], du[-1]))
+                name, st[0], st[m], st[-1], en[0], en[m], en[-1], du[0], du[m], du[-1]))
         sms = {}
-        for i, (a, b, sm_) in enumerate(r["_cta"]):
+        for i, (a, b, sm_) in r["_cta"].items():
             sms.setdefault(sm_, []).append(i)
         shared = sorted(len(v) for v in sms.values())
         lines.append("  SMs used %d; CTAs per SM: %s" % (len(sms), {k: shared.count(k) for k in sorted(set(shared))}))
-        pair = {"bwd+bwd": 0, "bwd+wgrad": 0, "wgrad+wgrad": 0}
+        mix = {}
         for v in sms.values():
-            if len(v) == 2:
-                k = sum(1 for i in v if i < 128)
-                pair[["bwd+bwd", "bwd+wgrad", "wgrad+wgrad"][k]] += 1
-        lines.append("  SM sharing: %s" % pair)
+            k = "%d wgrad + %d bwd" % (sum(1 for i in v if i < 256), sum(1 for i in v if i >= 256))
+            mix[k] = mix.get(k, 0) + 1
+        lines.append("  SM sharing: %s" % dict(sorted(mix.items())))
+        # the part of the step after da2: CTAs that could only start once the dense-chain cluster had ended, and where the segment ends
+        late = [sum(1 for a, b, sm_ in q["_cta"].values() if a > q["mlp_chain"][1]) for q in rows]
+        to_bwd = [(max(max(b for a, b, sm_ in q["_cta"].values()), q["cnn_wgrad1"][1], q["cnn_bwd"][1]) - q["mlp_chain"][1]) / 1e3 for q in rows]
+        line = "  after da2 stored: CTAs starting later %s (median %d); to the end of cnn_bwd_all %.2f us" % (
+            max(late), statistics.median(late), statistics.median(to_bwd))
+        if "chan:conv" in rows[0]:
+            line += ", to the end of the conv-key exchange %.2f us" % statistics.median((q["chan:conv"][1] - q["mlp_chain"][1]) / 1e3 for q in rows)
+        lines.append(line)
     for name, labels in cnn_labels.items():
         lines.append("  %s phases of CTA 0 (us): %s" % (name, "  ".join("%s %.2f" % (lab, statistics.median(r["_cnn_ph"][name][i] for r in rows))
                                                                       for i, lab in enumerate(labels))))
