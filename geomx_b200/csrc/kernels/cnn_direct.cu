@@ -4,7 +4,8 @@
 //   cnn_fwd_kernel      x -> a1 (+argmax) -> a2 (+argmax)          both convolutions, bias, ReLU and both max-pools; one 4-CTA cluster per
 //                       image: each CTA computes a quarter of conv0 and shares it through distributed shared memory, so conv0 runs once
 //                       (cnn_fwd_dense0_kernel, even batches <= 32: the same, in clusters of two images, followed by the first dense
-//                       layer a2 -> a3, so that the dense-chain cluster kernel starts from a3)
+//                       layer a2 -> a3, so that the dense-chain cluster kernel starts from a3; in the classic training step also by the
+//                       rest of the row-separable chain, dense1, classifier, softmax-CE, dz4 and dz3, so that it only computes da2)
 //   cnn_bwd_all_kernel  one heterogeneous grid in clusters of two: CTAs [256, 256+4B)  da2 -> da1 (shared memory only) -> dW0, db0   (conv1
 //                       data gradient gathered from the non-zeros of dz2 + pool/ReLU backward of both layers + conv0 weight gradient), CTAs
 //                       [0, 256)  da2, a1 -> dW1, db1 (conv1 weight gradient, each cluster's two CTAs splitting the batch and combining their
@@ -237,8 +238,8 @@ struct CnnFwdDense0Smem {
   __align__(16) float a2[2 * CD_C2 * CD_P2 * CD_P2];   // both images' a2, as pushed by the 8 CTAs
   uint64_t bar_a2;
 };
-static_assert(sizeof(CnnFwdDense0Smem) == CNN_FWD_DENSE0_SMEM_BYTES, "CNN_FWD_DENSE0_SMEM_BYTES (common.cuh) must match");
 constexpr int CD_D1 = 256, CD_D0 = CD_C2 * CD_P2 * CD_P2;    // dense0: 512 -> 256
+constexpr int CD_D2 = 128, CD_NC = 10;                       // dense1: 256 -> 128, classifier: 128 -> 10
 
 // thread 0, before cnn_fwd_convs: arms the a2 buffer and has the first cluster prefetch W0 into L2
 __device__ __forceinline__ void fwd_dense0_arm(CnnFwdDense0Smem& s, const float* __restrict__ wd) {
@@ -303,66 +304,43 @@ __device__ __forceinline__ void fwd_dense0(CnnFwdDense0Smem& s, float v, int a2_
   if (j < 2) store(j, fmaxf((j == 0 ? acc0 : acc1) + bias, 0.f));
 }
 
-__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
-    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
-                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
-                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
-                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
-                          unsigned long long* dbg) {
-  __shared__ CnnFwdDense0Smem s;
-  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
-  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
-  stamp(0);
-  if (threadIdx.x == 0) fwd_dense0_arm(s, wd);
-  int a2_off;
-  const float v = cnn_fwd_convs<2>(s.conv, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
-  // (computed after the convolutions, which need every register they can get)
-  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), bl = blockIdx.x & 1, bpair = blockIdx.x - bl;
-  fwd_dense0(s, v, a2_off, cr, wd, bd, dbg, [&](int j, float y) { a3[(long long)(bpair + j) * CD_D1 + 32 * cr + (tid >> 3)] = y; });
-  stamp(6);
-  stamp(4);      // (slot 4 stays the end of the forward kernel)
-}
-
-// ------------------------------------------------------------------------------------------------------------------ inference
-// The whole forward pass of N images (any N >= 1) and its per-sample scores, in one launch: grid (N rounded up to even, 4), clusters of
-// (2, 4, 1) as in cnn_fwd_dense0_kernel, whose convolutions (without the stores only training needs) and dense0 it runs.  Then:
-//   dense1      every CTA pushes its 32 a3 columns of both images into all 8 CTAs (st.async, second transaction mbarrier); cluster rank r
-//               computes a4[.][16 r .. 16 r + 16): 16 threads per column, each over every 16th float4 of the column's W1 row, summed in a
-//               fixed shuffle order (W1, 128 KB, is read from L2 by every cluster)
-//   classifier  every CTA pushes its 16 a4 columns of both images into all 8 CTAs (third mbarrier); rank i < 2 (the g = 0 CTA of image
-//               bpair + i) computes that image's 10 logits (16 threads per logit, fixed shuffle order), softmax-CE with fp32 expf / logf
-//               and the arg-max (first maximum wins, like torch.argmax)
-// The missing second image of an odd N's last cluster is computed from a copy of image N - 1 and takes part in every push; nothing of it is
-// written.  No atomics: two launches on the same inputs give the same bits.
-constexpr int CD_D2 = 128, CD_NC = 10;       // dense1: 256 -> 128, classifier: 128 -> 10
-struct CnnEvalSmem {
+// ---- dense1 and the classifier in the same clusters: the part cnn_eval_kernel and the training head of cnn_fwd_dense0_kernel share.
+//   dense1       every CTA pushes its 32 a3 columns of both images into all 8 CTAs (st.async, second transaction mbarrier); cluster rank r
+//                computes a4[.][16 r .. 16 r + 16): 16 threads per column, each over every 16th float4 of the column's W1 row, summed in a
+//                fixed shuffle order (W1, 128 KB, is read from L2 by every cluster)
+//   a4 hand-off  every CTA pushes its 16 a4 columns of both images into all 8 CTAs (third mbarrier)
+//   logits       16 threads per logit (thread t < 160: class t / 16, float4 chunks j and j + 16 of its W2 row), fixed shuffle order
+struct CnnHeadSmem {
   CnnFwdDense0Smem d0;
   __align__(16) float a3[2 * CD_D1];        // both images' a3, as pushed by the 8 CTAs
   __align__(16) float a4[2 * CD_D2];        // both images' a4, as pushed by the 8 CTAs
   __align__(16) float a3own[2 * 32];        // this CTA's a3 columns of both images, gathered into float4 pushes
   __align__(16) float a4own[2 * 16];        // ... and its a4 columns
-  float logit[16];
+  float logit[2 * 16];                      // [image][class]
   uint64_t bar_a3, bar_a4;
 };
 
-__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256)
-    cnn_eval_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
-                    const float* __restrict__ b1, const float* __restrict__ wd0, const float* __restrict__ bd0, const float* __restrict__ wd1,
-                    const float* __restrict__ bd1, const float* __restrict__ wd2, const float* __restrict__ bd2, const float* __restrict__ label,
-                    float* __restrict__ logits, float* __restrict__ loss, int* __restrict__ pred, int* __restrict__ correct, int N) {
-  __shared__ CnnEvalSmem s;
-  if (threadIdx.x == 0) {
-    mbar_init(&s.bar_a3, 1);
-    mbar_arrive_expect_tx(&s.bar_a3, 2 * CD_D1 * 4);
-    mbar_init(&s.bar_a4, 1);
-    mbar_arrive_expect_tx(&s.bar_a4, 2 * CD_D2 * 4);
-    fwd_dense0_arm(s.d0, wd0);              // (its barrier-init fence covers these two as well)
+// thread 0, before fwd_dense0_arm (whose barrier-init fence covers these barriers too): arms the a3 and a4 buffers, and has the first cluster
+// prefetch W1 (each CTA its 16 KB, rows 16 r .. 16 r + 15) and W2 into L2, as fwd_dense0_arm does for W0
+__device__ __forceinline__ void fwd_head_arm(CnnHeadSmem& s, const float* __restrict__ wd1, const float* __restrict__ wd2) {
+  mbar_init(&s.bar_a3, 1);
+  mbar_arrive_expect_tx(&s.bar_a3, 2 * CD_D1 * 4);
+  mbar_init(&s.bar_a4, 1);
+  mbar_arrive_expect_tx(&s.bar_a4, 2 * CD_D2 * 4);
+  if (blockIdx.x < 2) {
+    const int r = (int)cg::this_cluster().block_rank();
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(wd1 + (long long)16 * r * CD_D1), "r"(16 * CD_D1 * 4) : "memory");
+    if (r == 0) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(wd2), "r"(CD_NC * CD_D2 * 4) : "memory");
   }
-  int a2_off;
-  const float v = cnn_fwd_convs<2, false>(s.d0.conv, x, w0, b0, w1, b1, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
-                                          a2_off, N);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, cr = (int)cg::this_cluster().block_rank();
-  fwd_dense0(s.d0, v, a2_off, cr, wd0, bd0, nullptr, [&](int j, float y) { s.a3own[j * 32 + (tid >> 3)] = y; });
+}
+
+// after fwd_dense0 has left this CTA's a3 columns of both images in s.a3own: the a3 hand-off and dense1.  Leaves this CTA's a4 columns in
+// s.a4own; the caller then runs fwd_a4_handoff (loads it issues in between are in flight while a4 is gathered).
+__device__ __forceinline__ void fwd_dense1(CnnHeadSmem& s, int cr, const float* __restrict__ wd1, const float* __restrict__ bd1,
+                                           unsigned long long* dbg) {
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // ---- a3 hand-off: warp w wrote columns 32 r + 4 w .. 4 w + 3 of both images; its lanes 0 and 1 push those of image 0 and 1
   __syncwarp();
   if (lane < 2) push_all<8>(s.a3, lane * CD_D1 + 32 * cr + 4 * warp, &s.bar_a3, cr, reinterpret_cast<const float4*>(s.a3own)[lane * 8 + warp]);
@@ -374,6 +352,7 @@ __global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256)
   for (int q = 0; q < 4; ++q) w[q] = __ldg(reinterpret_cast<const float4*>(wrow) + 16 * q + j);   // in flight while a3 lands
   const float bias1 = __ldg(bd1 + n);
   wait_landed(&s.bar_a3);
+  stamp(7);
   float acc0 = 0.f, acc1 = 0.f;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
@@ -388,29 +367,187 @@ __global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256)
     acc1 += __shfl_xor_sync(0xffffffffu, acc1, o);
   }
   if (j < 2) s.a4own[j * 16 + (tid >> 4)] = fmaxf((j == 0 ? acc0 : acc1) + bias1, 0.f);
-  // classifier operands in flight while a4 is gathered: thread t < 160 -> logit c = t / 16, float4 chunks j and j + 16 of its W2 row
-  const int c = tid >> 4;
+}
+// every CTA: returns once a4 of both images has landed in s.a4 (so that nothing is still pushed into its shared memory when it exits)
+__device__ __forceinline__ void fwd_a4_handoff(CnnHeadSmem& s, int cr) {
+  const int tid = threadIdx.x;
+  __syncthreads();
+  // 8 float4 (image tid / 4, columns 16 r + 4 (tid % 4) ..) into all 8 CTAs
+  if (tid < 8) push_all<8>(s.a4, (tid >> 2) * CD_D2 + 16 * cr + 4 * (tid & 3), &s.bar_a4, cr, reinterpret_cast<const float4*>(s.a4own)[tid]);
+  wait_landed(&s.bar_a4);
+}
+// the W2 row chunks of logit c: float4 j and j + 16 (j = tid % 16)
+__device__ __forceinline__ void fwd_w2_row(const float* __restrict__ wd2, int c, int j, float4 (&w2)[2]) {
+  w2[0] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + j);
+  w2[1] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + 16 + j);
+}
+// logit c of the a4 row `a4r`, without its bias: the 16 threads of the logit (j = tid % 16) sum in a fixed shuffle order and all return it
+__device__ __forceinline__ float fwd_logit(const float* a4r, const float4 (&w2)[2], int j) {
+  const float4 x0 = reinterpret_cast<const float4*>(a4r)[j];
+  const float4 x1 = reinterpret_cast<const float4*>(a4r)[16 + j];
+  float acc = 0.f;
+  acc = fmaf(w2[0].x, x0.x, acc); acc = fmaf(w2[0].y, x0.y, acc); acc = fmaf(w2[0].z, x0.z, acc); acc = fmaf(w2[0].w, x0.w, acc);
+  acc = fmaf(w2[1].x, x1.x, acc); acc = fmaf(w2[1].y, x1.y, acc); acc = fmaf(w2[1].z, x1.z, acc); acc = fmaf(w2[1].w, x1.w, acc);
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  return acc;
+}
+
+// ---- the training head of cnn_fwd_dense0_kernel.  Everything from a3 to dz3 is row-separable (only the weight gradients mix images), so the
+// forward clusters compute it for their two images and the dense-chain cluster kernel is left with da2 = dz3 W0 only.
+struct FwdHeadArgs {
+  const float* wd1; const float* bd1; const float* wd2; const float* bd2;   // [128][256], [128], [10][128], [10]
+  const float* label;                                                       // [B] class index as float
+  float* loss; float* logits;                                               // [B], [B][10] (logits may be null)
+  float* a4; float* dz4; float* dz3; float* dl;                              // [B][128], [B][128], [B][256], [B][16] (classes >= 10 zero)
+};
+struct CnnFwdHeadSmem {
+  CnnHeadSmem h;
+  __align__(16) float dz4[2 * CD_D2];       // both images' dz4, computed whole by every CTA
+  __align__(16) float part[8 * 2 * 32];     // dz3 partial sums [warp][image][column]
+  float dl[2 * 16];                         // both images' dlogits
+};
+static_assert(sizeof(CnnFwdHeadSmem) == CNN_FWD_DENSE0_SMEM_BYTES, "CNN_FWD_DENSE0_SMEM_BYTES (common.cuh) must match");
+
+// After fwd_dense0 (this CTA's a3 columns in s.h.a3own): dense1 and the a4 hand-off, then on every CTA the logits, softmax-CE (the dense
+// chain's, softmax_ce_quad) and the whole dz4 of the cluster's two images, and from dz4 this CTA's dz3 columns 32 r .. 32 r + 32: warp w
+// sums over W1 rows 16 w .. 16 w + 15 (lane = column, so a warp reads 128 contiguous bytes of a row from L2), the 8 partials are added in
+// warp order.  Stores this CTA's a4, dz4 and dz3 columns; ranks 0 and 1 store the loss, logits and dlogits of image bpair + rank.  Every
+// output has one writer and a fixed summation order: two launches give the same bits.
+__device__ __forceinline__ void fwd_train_head(CnnFwdHeadSmem& s, const FwdHeadArgs& hd, int cr, int bpair, unsigned long long* dbg) {
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, j = tid & 15, c = tid >> 4;
+  fwd_dense1(s.h, cr, hd.wd1, hd.bd1, dbg);
   float4 w2[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
   float bias2 = 0.f;
-  if (cr < 2 && c < CD_NC) {
-    w2[0] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + j);
-    w2[1] = __ldg(reinterpret_cast<const float4*>(wd2 + c * CD_D2) + 16 + j);
-    bias2 = __ldg(bd2 + c);
+  if (c < CD_NC) { fwd_w2_row(hd.wd2, c, j, w2); bias2 = __ldg(hd.bd2 + c); }
+  fwd_a4_handoff(s.h, cr);
+  stamp(14);
+  float w1c[16];                            // the dz3 operands W1[16 warp + k][32 r + lane], in flight during the classifier
+#pragma unroll
+  for (int k = 0; k < 16; ++k) w1c[k] = __ldg(hd.wd1 + (long long)(16 * warp + k) * CD_D1 + 32 * cr + lane);
+  if (c < CD_NC) {
+    const float l0 = fwd_logit(s.h.a4, w2, j) + bias2, l1 = fwd_logit(s.h.a4 + CD_D2, w2, j) + bias2;
+    if (j == 0) { s.h.logit[c] = l0; s.h.logit[16 + c] = l1; }
   }
   __syncthreads();
-  // ---- a4 hand-off: 8 float4 (image tid / 4, columns 16 r + 4 (tid % 4) ..) into all 8 CTAs
-  if (tid < 8) push_all<8>(s.a4, (tid >> 2) * CD_D2 + 16 * cr + 4 * (tid & 3), &s.bar_a4, cr, reinterpret_cast<const float4*>(s.a4own)[tid]);
-  wait_landed(&s.bar_a4);       // every CTA: nothing may still be pushed into its shared memory when it exits
+  if (warp == 0) {
+    // lanes 4 i + q (i < 2) hold classes 4 q .. 4 q + 3 of image i; lanes >= 8 repeat lanes 0 .. 7 (the shuffles take the whole warp)
+    const int i = (lane >> 2) & 1, c0 = 4 * (lane & 3), b = bpair + i;
+    float lg[4], dl[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) lg[k] = c0 + k < CD_NC ? s.h.logit[16 * i + c0 + k] : 0.f;
+    const float loss = softmax_ce_quad(lg, CD_NC, (int)__ldg(hd.label + b), dl);
+    if (lane < 8) {
+      *reinterpret_cast<float4*>(s.dl + 16 * i + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
+      if (cr == i) {
+        *reinterpret_cast<float4*>(hd.dl + (long long)b * 16 + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
+        if (c0 == 0) hd.loss[b] = loss;
+        if (hd.logits != nullptr)
+#pragma unroll
+          for (int k = 0; k < 4; ++k) if (c0 + k < CD_NC) hd.logits[(long long)b * CD_NC + c0 + k] = lg[k];
+      }
+    }
+  }
+  __syncthreads();
+  {
+    // dz4[i][m] = relu'(a4[i][m]) * sum_c dl[i][c] * W2[c][m]: thread -> image tid / 128, column m = tid % 128 (c ascending, as the chain)
+    const int i = tid >> 7, m = tid & (CD_D2 - 1);
+    float d = 0.f;
+#pragma unroll
+    for (int cc = 0; cc < CD_NC; ++cc) d = fmaf(s.dl[16 * i + cc], __ldg(hd.wd2 + cc * CD_D2 + m), d);
+    if (!(s.h.a4[i * CD_D2 + m] > 0.f)) d = 0.f;
+    s.dz4[i * CD_D2 + m] = d;
+    if ((m >> 4) == cr) hd.dz4[(long long)(bpair + i) * CD_D2 + m] = d;
+    if (tid < 8)
+      *reinterpret_cast<float4*>(hd.a4 + (long long)(bpair + (tid >> 2)) * CD_D2 + 16 * cr + 4 * (tid & 3)) = reinterpret_cast<const float4*>(s.h.a4own)[tid];
+  }
+  __syncthreads();
+  {
+    float acc0 = 0.f, acc1 = 0.f;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      acc0 = fmaf(s.dz4[16 * warp + k], w1c[k], acc0);
+      acc1 = fmaf(s.dz4[CD_D2 + 16 * warp + k], w1c[k], acc1);
+    }
+    s.part[(2 * warp) * 32 + lane] = acc0;
+    s.part[(2 * warp + 1) * 32 + lane] = acc1;
+  }
+  __syncthreads();
+  if (tid < 64) {
+    const int i = tid >> 5;
+    float d = s.part[i * 32 + lane];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) d += s.part[(2 * w + i) * 32 + lane];
+    if (!(s.h.a3own[i * 32 + lane] > 0.f)) d = 0.f;
+    hd.dz3[(long long)(bpair + i) * CD_D1 + 32 * cr + lane] = d;
+  }
+  stamp(15);
+}
+
+// grid (B, 4), B even, 256 threads, clusters of (2, 4, 1).  Without the head's outputs (hd.a4 == nullptr) it ends with a3 (stamps 5 a2 landed,
+// 6 a3 stored); with them it also runs fwd_train_head (stamps 7 a3 landed, 14 a4 landed, 15 dz3 stored).  Slot 4 is the end of the kernel.
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
+    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
+                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
+                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
+                          unsigned long long* dbg, const FwdHeadArgs hd) {
+  __shared__ CnnFwdHeadSmem s;
+  const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
+  auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
+  stamp(0);
+  const bool head = hd.a4 != nullptr;
+  if (threadIdx.x == 0) {
+    if (head) fwd_head_arm(s.h, hd.wd1, hd.wd2);
+    fwd_dense0_arm(s.h.d0, wd);
+  }
+  int a2_off;
+  const float v = cnn_fwd_convs<2>(s.h.d0.conv, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, dbg, a2_off);
+  // (computed after the convolutions, which need every register they can get)
+  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), bl = blockIdx.x & 1, bpair = blockIdx.x - bl;
+  fwd_dense0(s.h.d0, v, a2_off, cr, wd, bd, dbg, [&](int j, float y) {
+    a3[(long long)(bpair + j) * CD_D1 + 32 * cr + (tid >> 3)] = y;
+    s.h.a3own[j * 32 + (tid >> 3)] = y;
+  });
+  stamp(6);
+  if (head) fwd_train_head(s, hd, cr, bpair, dbg);
+  stamp(4);      // (slot 4 stays the end of the forward kernel)
+}
+
+// ------------------------------------------------------------------------------------------------------------------ inference
+// The whole forward pass of N images (any N >= 1) and its per-sample scores, in one launch: grid (N rounded up to even, 4), clusters of
+// (2, 4, 1) as in cnn_fwd_dense0_kernel, whose convolutions (without the stores only training needs), dense0 and dense1 it runs.  Then
+// rank i < 2 (the g = 0 CTA of image bpair + i) computes that image's 10 logits, softmax-CE with fp32 expf / logf and the arg-max (first
+// maximum wins, like torch.argmax).
+// The missing second image of an odd N's last cluster is computed from a copy of image N - 1 and takes part in every push; nothing of it is
+// written.  No atomics: two launches on the same inputs give the same bits.
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256)
+    cnn_eval_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                    const float* __restrict__ b1, const float* __restrict__ wd0, const float* __restrict__ bd0, const float* __restrict__ wd1,
+                    const float* __restrict__ bd1, const float* __restrict__ wd2, const float* __restrict__ bd2, const float* __restrict__ label,
+                    float* __restrict__ logits, float* __restrict__ loss, int* __restrict__ pred, int* __restrict__ correct, int N) {
+  __shared__ CnnHeadSmem s;
+  if (threadIdx.x == 0) {
+    fwd_head_arm(s, wd1, wd2);
+    fwd_dense0_arm(s.d0, wd0);
+  }
+  int a2_off;
+  const float v = cnn_fwd_convs<2, false>(s.d0.conv, x, w0, b0, w1, b1, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
+                                          a2_off, N);
+  const int tid = threadIdx.x, cr = (int)cg::this_cluster().block_rank(), j = tid & 15, c = tid >> 4;
+  fwd_dense0(s.d0, v, a2_off, cr, wd0, bd0, nullptr, [&](int jj, float y) { s.a3own[jj * 32 + (tid >> 3)] = y; });
+  fwd_dense1(s, cr, wd1, bd1, nullptr);
+  // classifier operands in flight while a4 is gathered
+  float4 w2[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+  float bias2 = 0.f;
+  if (cr < 2 && c < CD_NC) { fwd_w2_row(wd2, c, j, w2); bias2 = __ldg(bd2 + c); }
+  fwd_a4_handoff(s, cr);
   if (cr >= 2) return;
   const int b = (blockIdx.x & ~1) + cr;      // ranks 0 and 1 are the g = 0 CTAs of images bpair and bpair + 1
-  if (tid < 16 * CD_NC) {
-    const float4 x0 = reinterpret_cast<const float4*>(s.a4 + cr * CD_D2)[j];
-    const float4 x1 = reinterpret_cast<const float4*>(s.a4 + cr * CD_D2)[16 + j];
-    float acc = 0.f;
-    acc = fmaf(w2[0].x, x0.x, acc); acc = fmaf(w2[0].y, x0.y, acc); acc = fmaf(w2[0].z, x0.z, acc); acc = fmaf(w2[0].w, x0.w, acc);
-    acc = fmaf(w2[1].x, x1.x, acc); acc = fmaf(w2[1].y, x1.y, acc); acc = fmaf(w2[1].z, x1.z, acc); acc = fmaf(w2[1].w, x1.w, acc);
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (c < CD_NC) {
+    const float acc = fwd_logit(s.a4 + cr * CD_D2, w2, j);
     if (j == 0) {
       s.logit[c] = acc + bias2;
       if (logits != nullptr && b < N) logits[(long long)b * CD_NC + c] = acc + bias2;
@@ -848,14 +985,17 @@ GX_API int gx_cnn_fwd(const float* x, const float* w0, const float* b0, const fl
   launch_pdl(cnn_fwd_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry_src, carry_dst, carry_n, x_keep, g_cnn_dbg);
   return GX_CHECK_LAUNCH();
 }
-// the same, plus the first dense layer: a3 [B,256] = relu(a2 [B,512] · wd [256,512]^T + bd).  Only for even B <= 32 (clusters of two images);
-// returns -1 without launching otherwise.
+// the same, plus the first dense layer: a3 [B,256] = relu(a2 [B,512] · wd [256,512]^T + bd).  With a4 non-null also the training head
+// (fwd_train_head): wd1 [128,256], bd1, wd2 [10,128], bd2, label [B] in; loss [B], logits [B,10] (unless null), a4 [B,128], dz4 [B,128],
+// dz3 [B,256] and dl [B,16] out.  Only for even B <= 32 (clusters of two images); returns -1 without launching otherwise.
 GX_API int gx_cnn_fwd_dense0(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* wd, const float* bd,
                              float* a1, unsigned char* idx1, float* a2, unsigned char* idx2, float* a3, const float* carry_src, float* carry_dst,
-                             int carry_n, float* x_keep, int B, cudaStream_t s) {
+                             int carry_n, float* x_keep, const float* wd1, const float* bd1, const float* wd2, const float* bd2, const float* label,
+                             float* loss, float* logits, float* a4, float* dz4, float* dz3, float* dl, int B, cudaStream_t s) {
   if (B < 2 || (B & 1) || B > 32) return -1;
+  const FwdHeadArgs hd = {wd1, bd1, wd2, bd2, label, loss, logits, a4, dz4, dz3, dl};
   launch_pdl(cnn_fwd_dense0_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n,
-             x_keep, g_cnn_dbg);
+             x_keep, g_cnn_dbg, hd);
   return GX_CHECK_LAUNCH();
 }
 // inference of the whole demo CNN (cnn_eval_kernel): x [N,1,28,28], the ten parameters in CNN_PARAM_SHAPES order; writes logits [N,10] (unless

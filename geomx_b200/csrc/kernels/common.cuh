@@ -142,9 +142,33 @@ __device__ __forceinline__ void wait_landed(uint64_t* bar) {
       : "memory");
 }
 
+// softmax cross-entropy of one row whose logits four consecutive lanes hold (the lane with lane % 4 == q: classes 4 q .. 4 q + 3; classes
+// >= C are ignored), label l: dl = softmax - one-hot (0 for classes >= C); returns the row's loss, in all four lanes.  Every lane of the warp
+// takes part (shuffles).  The dense chain (mlp_chain.cu) and the training head of cnn_fwd_dense0_kernel (cnn_direct.cu) share it, so that both
+// round the same way.
+__device__ __forceinline__ float softmax_ce_quad(const float (&lg)[4], int C, int l, float (&dl)[4]) {
+  const int lane = threadIdx.x & 31, c0 = 4 * (lane & 3);
+  float mx = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) if (c0 + j < C) mx = fmaxf(mx, lg[j]);
+  mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+  mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+  float e[4], s = 0.f;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { e[j] = c0 + j < C ? __expf(lg[j] - mx) : 0.f; s += e[j]; }
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) dl[j] = c0 + j < C ? e[j] / s - (c0 + j == l ? 1.f : 0.f) : 0.f;
+  const int q = l & 3;
+  const float mine = q == 0 ? lg[0] : q == 1 ? lg[1] : q == 2 ? lg[2] : lg[3];
+  const float picked = __shfl_sync(0xffffffffu, mine, (lane & ~3) | ((l >> 2) & 3));
+  return -(picked - mx - __logf(s));
+}
+
 // Static shared memory of cnn_fwd_dense0_kernel (cnn_direct.cu asserts it).  Its successor in the step, dense_tail_kernel (mlp_chain.cu),
 // stages its weights while the forward kernel runs, on the SMs beside its CTAs: mlp_chain.cu checks that both fit into one SM.
-constexpr int CNN_FWD_DENSE0_SMEM_BYTES = 39488;
+constexpr int CNN_FWD_DENSE0_SMEM_BYTES = 46288;
 
 // ------------------------------------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {

@@ -25,7 +25,8 @@
 // times the chain with per-phase %globaltimer stamps.
 // dense0 is row-separable (a3[b] needs only the pooled conv output of image b), so where the direct forward kernel runs (even batches <= 32)
 // it computes a3 on its 128 SMs (cnn_fwd_dense0_kernel, cnn_direct.cu) and the cluster kernel is dense_tail_kernel: the same chain from a3
-// on, through the same body (dense_chain_body), with no x tile, no dense0 phase and no a3 hand-off.
+// on, through the same body (dense_chain_body), with no x tile, no dense0 phase and no a3 hand-off.  In the classic training step the
+// forward kernel also computes everything down to dz3 (all of it row-separable), and dense_tail_kernel runs from dz3: P5 (dx) only.
 //
 // Shapes are compile-time (D0 -> D1 -> D2 -> C<=16, batch <= 32): the demo CNN's 512 -> 256 -> 128 -> 10.  Other shapes use the wgmma GEMMs.
 #include <cooperative_groups.h>
@@ -54,6 +55,7 @@ struct MlpChainParams {
   // (dense_tail_kernel: a3 is its input, x and b0 are unused)
   float* a3; float* a4; float* dz4; float* dz3; float* dl;
   int B, C;
+  int from_dz3;              // dense_tail_kernel: dz3 is the input (cnn_fwd_dense0_kernel's training head computed it) and dx the only output
   unsigned long long* dbg;   // optional %globaltimer stamps of cluster CTA 0 (tools/kernel_times.py)
 };
 
@@ -245,6 +247,26 @@ struct TailSmem {
 // both kernels' shared memory, with the 1 KB the runtime reserves per CTA, has to fit into the SM's 228 KB
 static_assert(TailSmem<512, 256, 128, 16>::BYTES + CNN_FWD_DENSE0_SMEM_BYTES + 2048 <= 233472, "dense_tail_kernel fits beside cnn_fwd_dense0_kernel");
 
+// P5 of the chain: dx[:, slice of D0] = dz3 * W0[:, slice], with dz3 (rows >= B zero) whole in the A3 buffer and the W0 column slice staged.
+// NC = KS0, K = D1, split over all 16 warps.
+template <class L, int D0, int D1, class Stamp>
+__device__ __forceinline__ void dense_dx(float* sm, const MlpChainParams& p, const int cr, Stamp&& stamp) {
+  constexpr int KS0 = L::KS0, PER = 2 * KS0, KS = MC_THREADS / PER;
+  const float* sDZ3 = sm + L::A3; const float* sW0 = sm + L::W0;
+  float* scratch = sm + L::SCRATCH;
+  const int tid = threadIdx.x, ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
+  float acc[4][4] = {};
+  prod_nn<D1, KS0, KS>(sDZ3, sW0, tb, tn, ks, acc);
+  stamp(14);
+  put_partial<KS0>(scratch, tb, tn, ks, acc);
+  __syncthreads();
+  for (int e = tid; e < MC_B * KS0 / 4; e += MC_THREADS) {
+    const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
+    if (b < p.B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(scratch, b, n4);
+  }
+  stamp(9);
+}
+
 // P2 .. P5 of the chain, the part both cluster kernels share: a4 = relu(a3 W1^T + b1) with the a4 hand-off, the classifier, softmax-CE and
 // the whole dz4, dz3 with its hand-off, and dx.  On entry the weights are staged (W0 as the column slice for dx still in flight, W1 as the
 // row slice), a3 is in the A3 buffer (FROM_X: as it lands from the peers) and in A3OWN (this CTA's columns), the labels and biases are
@@ -259,7 +281,7 @@ __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams
   float* sW0 = sm + L::W0; float* sW1 = sm + L::W1; float* sA3 = sm + L::A3; float* sA4 = sm + L::A4;
   float* sDZ4 = sm + L::DZ4; float* sW2 = sm + L::W2; float* sDL = sm + L::DL; float* sA3own = sm + L::A3OWN;
   float* sB1 = sm + L::MISC + NS1; float* sB2 = sB1 + NS2; float* sLab = sB2 + 16;
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   const int B = p.B, C = p.C;
   // ---------------- P2: a4[:, slice] = relu(a3 * W1[slice]^T + b1)         NC = 16, K = D1, KS = 8
   {
@@ -311,27 +333,13 @@ __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams
       const int b = tid >> 2, n4 = tid & 3, c0 = 4 * n4;
       const float4 s4 = sum_partials<MC_CMAX, KS>(sDZ4, b, n4);
       const float lg[4] = {s4.x + sB2[c0], s4.y + sB2[c0 + 1], s4.z + sB2[c0 + 2], s4.w + sB2[c0 + 3]};
-      float mx = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) if (c0 + j < C) mx = fmaxf(mx, lg[j]);
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      float e[4], s = 0.f;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { e[j] = c0 + j < C ? __expf(lg[j] - mx) : 0.f; s += e[j]; }
-      s += __shfl_xor_sync(0xffffffffu, s, 1);
-      s += __shfl_xor_sync(0xffffffffu, s, 2);
-      const int l = (int)sLab[b];
       float dl[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) dl[j] = (c0 + j < C && b < B) ? e[j] / s - (c0 + j == l ? 1.f : 0.f) : 0.f;
+      const float loss = softmax_ce_quad(lg, C, (int)sLab[b], dl);
+      if (b >= B) dl[0] = dl[1] = dl[2] = dl[3] = 0.f;
       *reinterpret_cast<float4*>(sDL + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
-      const int q = l & 3;
-      const float mine = q == 0 ? lg[0] : q == 1 ? lg[1] : q == 2 ? lg[2] : lg[3];
-      const float picked = __shfl_sync(0xffffffffu, mine, (lane & ~3) | ((l >> 2) & 3));
       if (cr == 0 && b < B) {
         *reinterpret_cast<float4*>(p.dl + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
-        if (n4 == 0) p.loss[b] = -(picked - mx - __logf(s));
+        if (n4 == 0) p.loss[b] = loss;
         if (p.logits != nullptr)
 #pragma unroll
           for (int j = 0; j < 4; ++j) if (c0 + j < C) p.logits[(long long)b * C + c0 + j] = lg[j];
@@ -399,23 +407,9 @@ __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams
     stamp(7);
     __syncthreads();                                     // own dz3 columns stored, the P4 partials read
   }
-  // ---------------- P5: dx[:, slice of D0] = dz3 * W0[:, slice]                      NC = KS0, K = D1, split over all 16 warps
-  {
-    wait_landed(bar_dz3);                                // the peers' columns
-    stamp(8);
-    constexpr int PER = 2 * KS0, KS = MC_THREADS / PER;
-    const int ks = tid / PER, tile = tid % PER, tb = tile & 7, tn = tile >> 3;
-    float acc[4][4] = {};
-    prod_nn<D1, KS0, KS>(sDZ3, sW0, tb, tn, ks, acc);
-    stamp(14);
-    put_partial<KS0>(scratch, tb, tn, ks, acc);
-    __syncthreads();
-    for (int e = tid; e < MC_B * KS0 / 4; e += MC_THREADS) {
-      const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
-      if (b < B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(scratch, b, n4);
-    }
-  }
-  stamp(9);
+  wait_landed(bar_dz3);                                  // the peers' columns
+  stamp(8);
+  dense_dx<L, D0, D1>(sm, p, cr, stamp);
 }
 
 // CS = CTAs per cluster: 8 (portable) or 16 (non-portable size, one GPC): every layer is cut into CS column slices
@@ -533,6 +527,27 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dens
     if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
   };
   stamp(0);
+  if (p.from_dz3) {
+    // dx = dz3 W0 only: the W0 column slice before the grid dependency, then dz3 (rows >= B zero) into the buffer P5 reads.  Nothing is
+    // exchanged between the CTAs in this mode.
+    stage_plain_async(sW0, p.w0 + cr * L::KS0, D1, L::KS0, D0);
+    cp_async_commit();
+    stamp(1);
+    pdl_wait();
+    pdl_launch();
+    stamp(2);
+    for (int c = tid; c < MC_B * (D1 >> 2); c += MC_THREADS) {
+      const int r = c / (D1 >> 2), q = c - r * (D1 >> 2);
+      if (r < B) cp_async16(sA3 + sw_off(r, q << 2, D1), p.dz3 + (long long)r * D1 + (q << 2));
+      else *reinterpret_cast<float4*>(sA3 + sw_off(r, q << 2, D1)) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncthreads();
+    stamp(3);
+    dense_dx<L, D0, D1>(sm, p, cr, stamp);
+    return;
+  }
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) mbar_init(bar + i, 1);
     mbar_arrive_expect_tx(bar_a4, MC_B * D2 * 4);
@@ -676,14 +691,16 @@ GX_API int gx_mlp_chain(const float* x, const float* w0, const float* b0, const 
 }
 
 // the same data path from a3 [B][D1] (computed by gx_cnn_fwd_dense0): loss, logits, dx; stores a4, dz4, dz3 and the dlogits for
-// gx_dense_wgrad.  w0 is read only as the column slices of dx.  Returns -1 for unsupported shapes.
+// gx_dense_wgrad.  w0 is read only as the column slices of dx.  from_dz3 != 0: dx = dz3 [B][D1] · w0 only (dz3 computed by gx_cnn_fwd_dense0's
+// training head); nothing else is read or written.  Returns -1 for unsupported shapes.
 GX_API int gx_dense_tail(const float* a3, const float* w0, const float* w1, const float* b1, const float* w2, const float* b2, const float* label,
                          float* loss, float* logits, float* dx, float* a4, float* dz4, float* dz3, float* dl, int B, int D0, int D1, int D2, int C,
-                         cudaStream_t stream) {
+                         int from_dz3, cudaStream_t stream) {
   if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
   MlpChainParams p = {};
   p.w0 = w0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
   p.a3 = const_cast<float*>(a3); p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
+  p.from_dz3 = from_dz3 != 0;
   return mlp_launch_any<true>(p, stream);
 }
 

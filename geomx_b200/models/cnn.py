@@ -7,10 +7,11 @@
 plus the HiPS push/pull of all 10 keys (``dist_sync``: party aggregation → global aggregation + optimizer → broadcast), captured ONCE
 into a CUDA graph and replayed per step.  At the reference's batch size (32 per worker) the step is 5-6 hand-written sm_90a launches:
 
-  cnn_fwd      conv0+bias+ReLU+pool → conv1+bias+ReLU+pool → dense0+bias+ReLU, fp32 FMA, the conv0 map never leaves shared memory; clusters
-               of two images, whose 8 CTAs exchange a2 and compute a3 (cnn_fwd_dense0_kernel, csrc/kernels/cnn_direct.cu)
-  mlp_chain    dense1 → classifier → softmax-CE forward and the data gradients down to da2, from a3, one 16-CTA cluster
-               (dense_tail_kernel, csrc/kernels/mlp_chain.cu)
+  cnn_fwd      conv0+bias+ReLU+pool → conv1+bias+ReLU+pool → dense0 → dense1 → classifier → softmax-CE, and the data gradients dz4 and
+               dz3, fp32 FMA, the conv0 map never leaves shared memory; clusters of two images, whose 8 CTAs exchange a2, a3 and a4
+               (cnn_fwd_dense0_kernel, csrc/kernels/cnn_direct.cu)
+  mlp_chain    da2 = dz3 · W0, one 16-CTA cluster (dense_tail_kernel, csrc/kernels/mlp_chain.cu).  With look-ahead the forward kernel stops
+               at a3 and the cluster kernel runs the chain from a3 to da2.
   dense_wgrad  the three dense weight gradients and bias gradients, on a parallel branch: in the dense channel's step on the
                high-priority stream when there is one, otherwise on the side stream, joined before the exchange   (csrc/kernels/mlp_chain.cu)
   cnn_bwd_all  conv1 data gradient + pool/ReLU routing + conv0 weight gradient ‖ conv1 weight gradient, one grid      (csrc/kernels/cnn_direct.cu)
@@ -313,10 +314,16 @@ class HipsCNNTrainStep:
         # even B <= 32 (paths with both the direct convolutions and the cluster kernel): dense0 is row-separable, so the forward kernel
         # computes a3 on its 128 SMs and the cluster kernel starts from a3
         self._fwd_dense0 = fwd_dense0 = self.direct_conv and self.fused_mlp
+        # ... and so is the rest of the chain down to dz3: in the classic step the forward kernel also runs dense1, the classifier, softmax-CE,
+        # dz4 and dz3, and the cluster kernel computes only da2 = dz3 W0.  A look-ahead launch ends with the NEXT batch's forward kernel, which
+        # would overwrite this batch's loss and logits before the host reads them: it keeps the forward kernel that stops at a3.
+        self._fwd_head = fwd_head = fwd_dense0 and not self.lookahead
+        head_out = dict(wd1=P[6], bd1=P[7], wd2=P[8], bd2=P[9], label=self.label_cur, loss=self.loss, logits=self.logits, a4=self.a4, dz4=self.dz4,
+                        dz3=self.dz3, dl=self.dl) if fwd_head else {}
         if fwd_dense0:
             def fwd():
                 if not n.cnn_fwd_dense0(self.x, P[0], P[1], P[2], P[3], P[4], P[5], self.a1, self.idx1, self.a2, self.idx2, self.a3, carry=carry,
-                                        x_keep=self.x_cur if self.lookahead else None):
+                                        x_keep=self.x_cur if self.lookahead else None, **head_out):
                     raise RuntimeError("cnn_fwd_dense0 does not cover batch %d" % B)
         else:
             fwd = lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry,
@@ -326,7 +333,7 @@ class HipsCNNTrainStep:
             # backward pass waits for) and one weight-gradient launch on a parallel branch, instead of the seven above
             if fwd_dense0:
                 chain = lambda: n.dense_tail(self.a3, P[4], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2, self.a4,
-                                             self.dz4, self.dz3, self.dl)
+                                             self.dz4, self.dz3, self.dl, from_dz3=fwd_head)
             else:
                 chain = lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2,
                                                  self.a3, self.a4, self.dz4, self.dz3, self.dl)

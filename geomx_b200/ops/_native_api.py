@@ -117,15 +117,17 @@ def mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, d
     return True
 
 
-def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl):
+def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl, from_dz3=False):
     """The data path of the dense chain from a3 [B,D1] on (what :func:`cnn_fwd_dense0` computed), in ONE cluster launch: per-sample loss,
     logits and dx [B,D0]; it also stores a4, dz4, dz3 and the dlogits dl [B,16] for :func:`dense_wgrad` (a3 is already in memory).  ``w0``
-    [D1,D0] is read for dx only.  Returns False for shapes other than 512 -> 256 -> 128 -> C<=16, batch <= 32."""
-    B, D1 = a3.shape
+    [D1,D0] is read for dx only.  ``from_dz3=True``: dz3 [B,D1] is the input (what :func:`cnn_fwd_dense0`'s training head computed) and the
+    launch computes dx = dz3 · w0 only; the other buffers are neither read nor written.  Returns False for shapes other than
+    512 -> 256 -> 128 -> C<=16, batch <= 32."""
+    B, D1 = dz3.shape
     D0, D2, C = w0.shape[1], w1.shape[0], w2.shape[0]
-    assert w0.shape[0] == D1 and dx.shape == (B, D0) and dl.shape == (B, 16)
+    assert w0.shape[0] == D1 and dx.shape == (B, D0) and dl.shape == (B, 16) and dz3.is_contiguous()
     rc = _lib().gx_dense_tail(_p(a3), _p(w0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dx), _p(a4), _p(dz4), _p(dz3),
-                              _p(dl), B, D0, D1, D2, C, _s())
+                              _p(dl), B, D0, D1, D2, C, int(bool(from_dz3)), _s())
     if rc == -1:
         return False
     _ck(rc, "dense_tail")
@@ -153,15 +155,28 @@ def cnn_fwd(x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry=None, x_keep=None):
                           0 if src is None else src.numel(), _p(x_keep), x.shape[0], _s()), "cnn_fwd")
 
 
-def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None, x_keep=None):
+def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None, x_keep=None, *, wd1=None, bd1=None, wd2=None, bd2=None,
+                   label=None, loss=None, logits=None, a4=None, dz4=None, dz3=None, dl=None):
     """:func:`cnn_fwd` followed by the first dense layer in the same launch: also a3 [B,256] = relu(a2.view(B,512) · wdᵀ + bd), with
     wd [256,512].  ``carry`` / ``x_keep`` as in :func:`cnn_fwd`.  Runs clusters of two images: returns False without launching for odd B or
-    B > 32."""
+    B > 32.
+
+    With ``a4`` given, the same launch also runs the rest of the dense chain's row-separable part (the training head): dense1 (``wd1``
+    [128,256], ``bd1``), the classifier (``wd2`` [10,128], ``bd2``) and softmax-CE against ``label`` [B] (float class ids), and the data
+    gradients down to dz3.  It writes loss [B], logits [B,10] (skipped when None), a4 [B,128], dz4 [B,128], dz3 [B,256] and the dlogits
+    dl [B,16] (classes >= 10 zero): what :func:`dense_tail` with ``from_dz3=True`` and :func:`dense_wgrad` read."""
     B = x.shape[0]
     assert wd.shape == (256, 512) and a3.shape == (B, 256) and a3.is_contiguous()
+    head = (wd1, bd1, wd2, bd2, label, loss, logits, a4, dz4, dz3, dl)
+    if a4 is not None:
+        assert wd1.shape == (128, 256) and wd2.shape == (10, 128) and label.numel() == B and loss.numel() == B
+        assert all(t.is_contiguous() for t in (wd1, wd2, a4, dz4, dz3, dl))
+        assert a4.shape == (B, 128) and dz4.shape == (B, 128) and dz3.shape == (B, 256) and dl.shape == (B, 16)
+        assert logits is None or (logits.shape == (B, 10) and logits.is_contiguous())
     src, dst = carry if carry is not None else (None, None)
     rc = _lib().gx_cnn_fwd_dense0(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(wd), _p(bd), _p(a1), _p(idx1), _p(a2), _p(idx2), _p(a3), _p(src),
-                                  _p(dst), 0 if src is None else src.numel(), _p(x_keep), B, _s())
+                                  _p(dst), 0 if src is None else src.numel(), _p(x_keep),
+                                  *(_p(t) if a4 is not None else None for t in head), B, _s())
     if rc == -1:
         return False
     _ck(rc, "cnn_fwd_dense0")

@@ -9,9 +9,9 @@ SIGS = {
     "gx_gemm_tf32_pool": [P, L, I, P, L, I, I, I, I, P, P, I, I, I, P, F, P],
     "gx_mlp_chain": [P] * 16 + [I] * 5 + [P],
     "gx_dense_wgrad": [P] * 12 + [I] * 5 + [P],
-    "gx_dense_tail": [P] * 14 + [I] * 5 + [P],
+    "gx_dense_tail": [P] * 14 + [I] * 6 + [P],
     "gx_cnn_fwd": [P] * 11 + [I, P, I, P],
-    "gx_cnn_fwd_dense0": [P] * 14 + [I, P, I, P],
+    "gx_cnn_fwd_dense0": [P] * 14 + [I] + [P] * 12 + [I, P],
     "gx_cnn_bwd": [P] * 9 + [I, P],
     "gx_cnn_wgrad1": [P] * 6 + [I, P],
     "gx_cnn_bwd_all": [P] * 11 + [I, P],

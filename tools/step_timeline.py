@@ -26,6 +26,9 @@ CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
                     "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
                     "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
 FWD_DENSE0_PHASES, FWD_DENSE0_LABELS = (0, 1, 2, 3, 5, 6), ("staging", "conv0", "conv1", "a2 landed", "dense0 -> a3 stored")
+# with its training head (the classic step) it goes on: 7 a3 landed | 14 a4 landed | 15 dz3 stored
+FWD_HEAD_PHASES = FWD_DENSE0_PHASES + (7, 14, 15)
+FWD_HEAD_LABELS = FWD_DENSE0_LABELS + ("a3 landed", "dense1 -> a4 landed", "head -> dz4 -> dz3 stored")
 # the same for the dense-chain cluster kernel (gx_mlp_chain_set_debug slots of cluster CTA 0): 0 start | 3 inputs landed | 4 a3 landed |
 # 5 a4 landed | 6 dz4 computed | 7 dz3 pushed | 8 dz3 landed | 9 end (da2 stored); and of the dense weight-gradient kernel: 16 start of its
 # CTA 0 | 17 its grid dependency resolved | 18 end of its last CTA.  The kernel that starts from a3 (dense_tail_kernel) has no slot 4.
@@ -33,6 +36,8 @@ MLP_PHASES = (0, 3, 4, 5, 6, 7, 8, 9)
 MLP_PHASE_LABELS = ("staging+pdl-wait", "dense0 -> a3", "dense1 -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
 TAIL_PHASES = (0, 3, 5, 6, 7, 8, 9)
 TAIL_PHASE_LABELS = ("staging+pdl-wait", "a3 staged -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
+# ... and from dz3 (after the forward kernel's training head): 0 start | 3 dz3 staged | 9 end (da2 stored)
+TAIL_DZ3_PHASES, TAIL_DZ3_LABELS = (0, 3, 9), ("staging+pdl-wait+dz3 staged", "dz3 staged -> da2")
 
 
 def main():
@@ -57,11 +62,11 @@ def main():
         eng.step(X, y)
     fab = eng.fabric
     chans = list(fab.channels) or ["fsa"]
-    tail = getattr(eng, "_fwd_dense0", False)
+    tail, head = getattr(eng, "_fwd_dense0", False), getattr(eng, "_fwd_head", False)
     cnn_phases, cnn_labels = dict(CNN_PHASES), dict(CNN_PHASE_LABELS)
     if tail:
-        cnn_phases["cnn_fwd"], cnn_labels["cnn_fwd"] = FWD_DENSE0_PHASES, FWD_DENSE0_LABELS
-    mlp_phases, mlp_labels = (TAIL_PHASES, TAIL_PHASE_LABELS) if tail else (MLP_PHASES, MLP_PHASE_LABELS)
+        cnn_phases["cnn_fwd"], cnn_labels["cnn_fwd"] = (FWD_HEAD_PHASES, FWD_HEAD_LABELS) if head else (FWD_DENSE0_PHASES, FWD_DENSE0_LABELS)
+    mlp_phases, mlp_labels = ((TAIL_DZ3_PHASES, TAIL_DZ3_LABELS) if head else (TAIL_PHASES, TAIL_PHASE_LABELS)) if tail else (MLP_PHASES, MLP_PHASE_LABELS)
     for c in chans:
         fab.state[c][3] = 1
     # cnn_bwd_all: weight-gradient CTAs [0, 256) (pairs that split the batch), data-gradient CTAs [256, grid); its last `stamped_ctas` CTAs
