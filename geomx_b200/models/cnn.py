@@ -24,6 +24,10 @@ Without the direct convolutions (odd batches, ``GEOMX_DIRECT_CONV=0``) the clust
 bias / ReLU / max-pool / mask / column-sum epilogues (3xTF32 = fp32-accurate by default), weight-gradient GEMMs on a parallel graph branch.
 With one rank and one party both PS tiers collapse into the arena optimizer inside the exchange kernels.
 
+Which of these kernel paths a step takes is decided once, when the engine is constructed: ``step_path()`` maps the batch size, the
+engine's arguments and the step switches (``STEP_SWITCHES``, read from the environment at that moment) to a ``StepPath`` record, and
+``_steps()`` binds the launches of that record.  Changing a switch afterwards does not change the engine; construct a new one.
+
 The reference runs the same step as ~200 engine ops (per-image im2col+SGEMM) + 20 ZMQ round trips (SURVEY §3.3-3.4).
 The public API a user calls is ``step(X_host, y_host) -> loss`` (H2D of the batch from pinned memory, graph replay, D2H of the loss).
 
@@ -35,6 +39,7 @@ buffers of their own, ordered on the current stream after the steps enqueued bef
 from __future__ import annotations
 
 import os
+from typing import NamedTuple
 
 import torch
 
@@ -45,9 +50,98 @@ from ..ops import native
 from ..parallel.arena import ArenaLayout
 from ..parallel.fabric import HipsFabric, Topology
 
-__all__ = ["build_cnn", "CNN_PARAM_SHAPES", "HipsCNNTrainStep"]
+__all__ = ["build_cnn", "CNN_PARAM_SHAPES", "HipsCNNTrainStep", "StepPath", "step_path", "STEP_SWITCHES"]
 
 CNN_PARAM_SHAPES = [(16, 1, 5, 5), (16,), (32, 16, 5, 5), (32,), (256, 512), (256,), (128, 256), (128,), (10, 128), (10,)]
+
+# The environment variables that select the training step's kernel path; HipsCNNTrainStep reads them once, when it is constructed.
+STEP_SWITCHES = ("GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_CNN_BWD_ONE_LAUNCH",
+                 "GEOMX_NO_POOL_FUSION", "GEOMX_FUSED_EXCHANGE", "GEOMX_E2E_DIRECT_INPUT")
+
+# Names of the step's launches that more than one stage or caller refers to (tests, tools and bench.py key on the names).
+DIRECT_FWD = "conv0+conv1 fwd (direct, relu+pool fused)"
+GEMM_FWD = ("conv0+relu+pool+im2col", "conv1 gemm (bias,relu,maxpool fused)")
+MLP = "mlp chain fwd+bwd (cluster)"
+DENSE_WGRAD = "dense weight gradients"
+DENSE_KV = "hips push+opt+pull (dense keys, overlapped)"
+ONE_GRID = "conv bwd: conv1 wgrad + dgrad + conv0 wgrad (direct, one grid)"
+FUSED_BWD = "conv bwd (one grid) + conv-key exchange in its tail"
+EXCH = "hips push+opt+pull"
+LOCAL = "local optimizer (fused arena Adam)"
+
+
+class StepPath(NamedTuple):
+    """The kernel path of one engine's training step (see :func:`step_path`)."""
+    direct_conv: bool       # convolutions: direct fp32 kernels (True) or im2col + wgmma GEMMs
+    pool_fusion: bool       # GEMM convolutions: conv1's max-pool in the GEMM epilogue (where the kernel can express it)
+    dense: str              # where the dense chain's cluster kernel starts: 'a2' (mlp_chain), 'a3' (dense_tail; the forward kernel computes
+                            # dense0), 'dz3' (dense_tail from dz3; the forward kernel also runs the head), or 'gemm' (seven GEMM / head launches)
+    wgrad: str | None       # the cluster path's dense weight gradients: 'side' stream or 'comm' stream (in the dense channel's step)
+    bwd: str                # convolution backward: 'one_grid', 'exchange_tail' (one grid, conv keys' exchange in its tail), 'two_launch', 'gemm'
+    exchange: str           # the exchange: 'fsa', 'async', 'conv' (channel), 'all' (single channel), 'local_opt' (HFA: local optimizer only)
+    local_tail: bool        # update='local': the arena optimizer applies the exchanged aggregate after the exchange
+    overlap: bool           # key-group channels: the dense keys' exchange on the comm stream underneath the convolution backward
+    single: str | None      # the one direct-protocol channel of all keys ('all') when not overlapping
+    n_fwd: int              # leading launches that need only the batch and the weights (a look-ahead launch runs them for the next batch)
+    lookahead: bool
+    lookahead_join: str     # how a look-ahead launch joins before the next batch's forward launches: 'join' (side) or 'join_comm' (side + comm)
+    direct_input: bool      # the host pipeline captures one graph per input buffer instead of copying staging -> input
+
+
+def step_path(B, *, mode="dist_sync", hfa=False, update="server", lookahead=False, world=1, direct_protocol=False, conv_tail_capable=False,
+              env=None):
+    """Choose the training step's kernel path from plain values: the per-worker batch ``B``, the engine's ``mode`` / ``hfa`` / ``update`` /
+    ``lookahead``, the number of ranks, whether the fabric has the direct-protocol buffers, whether the conv keys' channel can run in a
+    compute kernel's tail, and the step switches in ``env`` (a mapping of :data:`STEP_SWITCHES` names to strings; missing = default)."""
+    env = env or {}
+    on = lambda k, default: env.get(k, default) == "1"
+    sync = mode == "dist_sync" and not hfa
+    # One rank -> channels (their exchange is local arithmetic); several ranks -> one exchange after the backward pass (the overlapped
+    # two-hop channel's polling slows the backward pass down, and at 8 ranks it outlasts the pass it hides behind).  Hence the default.
+    overlap = sync and on("GEOMX_STEP_OVERLAP", "1" if world == 1 else "0") and (world == 1 or direct_protocol)
+    single = "all" if (sync and not overlap and world > 1 and direct_protocol
+                       and env.get("GEOMX_STEP_EXCHANGE", "ll") in ("sharded", "replicated")) else None
+    lookahead = bool(lookahead) and sync
+    fused_mlp = B <= 32 and on("GEOMX_FUSED_MLP", "1")
+    # small-batch regime: both convolutions forward / backward as direct fp32-FMA kernels (csrc/kernels/cnn_direct.cu) instead of im2col +
+    # wgmma GEMMs; their conv1 weight-gradient body splits the batch in halves, so odd batches and batches > 64 use the GEMMs
+    direct_conv = B <= 64 and B % 2 == 0 and on("GEOMX_DIRECT_CONV", "1")
+    # even B <= 32: dense0 is row-separable, so the forward kernel computes a3 on its 128 SMs; in the classic step it also runs the chain
+    # down to dz3.  A look-ahead launch ends with the NEXT batch's forward kernel, which would overwrite this batch's loss and logits before
+    # the host reads them: it keeps the forward kernel that stops at a3.
+    if not fused_mlp:
+        dense = "gemm"
+    elif not direct_conv:
+        dense = "a2"
+    else:
+        dense = "a3" if lookahead else "dz3"
+    if not direct_conv:
+        bwd = "gemm"
+    elif not on("GEOMX_CNN_BWD_ONE_LAUNCH", "1"):
+        bwd = "two_launch"
+    elif overlap and conv_tail_capable and on("GEOMX_FUSED_EXCHANGE", "0"):
+        bwd = "exchange_tail"
+    else:
+        bwd = "one_grid"
+    if overlap:
+        exchange = "conv"
+    elif single:
+        exchange = single
+    elif hfa:
+        exchange = "local_opt"
+    else:
+        exchange = "async" if mode == "dist_async" else "fsa"
+    return StepPath(
+        direct_conv=direct_conv, pool_fusion=not on("GEOMX_NO_POOL_FUSION", "0"), dense=dense,
+        # the dense channel reads these gradients: with one, they are issued in its comm-stream step.  A look-ahead launch ends with the
+        # next batch's forward convolutions, which overwrite the x this kernel reads: it keeps them on the side stream, joined before those
+        wgrad=None if dense == "gemm" else ("comm" if overlap and not lookahead else "side"),
+        bwd=bwd, exchange=exchange, local_tail=update == "local" and not hfa, overlap=overlap, single=single,
+        n_fwd=1 if direct_conv else 2, lookahead=lookahead,
+        # the next batch's forward convolutions overwrite a2 (and a3), which the side branch may still be reading; a forward kernel that
+        # also computes dense0 reads W0 / b0, which the dense keys' exchange (comm) updates
+        lookahead_join="join_comm" if dense in ("a3", "dz3") else "join",
+        direct_input=not lookahead and on("GEOMX_E2E_DIRECT_INPUT", "1"))
 
 
 def build_cnn():
@@ -163,25 +257,18 @@ class HipsCNNTrainStep:
         # exchange runs underneath it on its own stream (two-hop, optimizer sharded over all ranks); the conv keys come last and use the
         # one-hop replicated mode — the only communication left on the critical path (reference ordering: push(idx, priority=-idx),
         # examples/cnn.py:121-125).  GEOMX_STEP_OVERLAP=0 selects the single fused exchange at the end of the step, =1 the channels.
-        # One rank -> channels (their exchange is local arithmetic); several ranks -> the single LL exchange after the backward pass (the
-        # overlapped two-hop channel's polling slows the backward pass down, and at 8 ranks it outlasts the pass it hides behind).  Hence the
-        # default by world size.
-        want_overlap = os.environ.get("GEOMX_STEP_OVERLAP", "1" if self.topo.world == 1 else "0") == "1"
-        self.overlap = mode == "dist_sync" and not self.hfa and want_overlap and (self.topo.world == 1 or f.ll_d is not None)
-        if self.overlap:
+        # The step switches are read here, once: the engine's kernel path does not change after construction.
+        env = {k: os.environ[k] for k in STEP_SWITCHES if k in os.environ}
+        choose = lambda tail_capable: step_path(B, mode=mode, hfa=bool(self.hfa), update=self.update, lookahead=lookahead, world=self.topo.world,
+                                                direct_protocol=f.ll_d is not None, conv_tail_capable=tail_capable, env=env)
+        path = choose(False)
+        if path.overlap:
             f.add_channel("dense", [4, 5, 6, 7, 8, 9], replicate=False, grid=int(os.environ.get("GEOMX_DENSE_CHANNEL_GRID", 40)) or None)
             f.add_channel("conv", [0, 1, 2, 3], replicate=True)
-        # GEOMX_STEP_OVERLAP=0: ONE exchange of all keys after the backward pass.  GEOMX_STEP_EXCHANGE picks its protocol: `ll` (three-hop
-        # hierarchy walk), `sharded` / `replicated` (direct protocol, two hops / one hop)
-        self.single = None
-        one = os.environ.get("GEOMX_STEP_EXCHANGE", "ll")
-        if not self.overlap and mode == "dist_sync" and not self.hfa and one in ("sharded", "replicated") and self.topo.world > 1 and f.ll_d is not None:
-            f.add_channel("all", list(range(10)), replicate=one == "replicated")
-            self.single = "all"
-        self.fused_mlp = B <= 32 and os.environ.get("GEOMX_FUSED_MLP", "1") == "1"
-        # small-batch regime: both convolutions forward / backward as direct fp32-FMA kernels (3 launches, csrc/kernels/cnn_direct.cu) instead
-        # of im2col + wgmma GEMMs (GEOMX_DIRECT_CONV=0 selects the GEMM path; batches > 64 always use it)
-        self.direct_conv = B <= 64 and B % 2 == 0 and os.environ.get("GEOMX_DIRECT_CONV", "1") == "1"
+        if path.single:
+            # GEOMX_STEP_OVERLAP=0: ONE exchange of all keys after the backward pass.  GEOMX_STEP_EXCHANGE picks its protocol: `ll` (three-hop
+            # hierarchy walk), `sharded` / `replicated` (direct protocol, two hops / one hop)
+            f.add_channel(path.single, list(range(10)), replicate=env.get("GEOMX_STEP_EXCHANGE") == "replicated")
         self.P = [f.param_view(i) for i in range(10)]
         self.G = [f.grad_view(i) for i in range(10)]
         if self.update == "local":
@@ -208,12 +295,10 @@ class HipsCNNTrainStep:
         self.dl = e(B, 16)          # dlogits, classes padded to 16 (cluster kernel -> dense weight-gradient kernel)
         self.dz2rows, self.dcol1, self.da1 = e(B * 64, 32), e(B * 64, 400), e(B, 16, 12, 12)
         self.loss_host = torch.empty(B, dtype=f32).pin_memory()
-        self.lookahead = bool(lookahead) and mode == "dist_sync" and not self.hfa
         # look-ahead: the head of the launch belongs to the PREVIOUS batch, whose labels must outlive the arrival of the next batch in `xin`
-        self.label_cur = torch.empty_like(self.label) if self.lookahead else self.label
-        self.x_cur = torch.empty_like(self.x) if self.lookahead else self.x        # ... and so must its images (conv0's weight gradient reads them)
+        self.label_cur = torch.empty_like(self.label) if path.lookahead else self.label
+        self.x_cur = torch.empty_like(self.x) if path.lookahead else self.x        # ... and so must its images (conv0's weight gradient reads them)
         self._primed = False
-        self.fused_exchange = False
         self.graph = None
         self._graph_alt = None
         self._xbufs = [self.xin, None]
@@ -225,6 +310,14 @@ class HipsCNNTrainStep:
         self.steps_done = 0
         self.kernels_per_step = 0
         self._ev = None             # evaluate / predict buffers (never shared with the step), grown to the largest N seen
+        # whether the conv keys' exchange can run in the backward grid's tail is a property of their channel.  Asked last: the answer
+        # allocates the channel's tile list, which would otherwise shift the step's buffers in the allocator.
+        if path.overlap and f.channel_fused_args("conv") is not None:
+            path = choose(True)
+        self.path = path
+        self.direct_conv, self.overlap, self.single, self.lookahead = path.direct_conv, path.overlap, path.single, path.lookahead
+        self.fused_mlp, self.fused_exchange = path.dense != "gemm", path.bwd == "exchange_tail"
+        self._fwd_dense0, self._fwd_head, self._n_fwd = path.dense in ("a3", "dz3"), path.dense == "dz3", path.n_fwd
 
     # ------------------------------------------------------------------------------------------------------------
     def _init_params(self, net):
@@ -260,137 +353,125 @@ class HipsCNNTrainStep:
         self.net = net
 
     # ------------------------------------------------------------------------------------------------------------
+    def _local_opt(self, grad_tensor, zero=None):
+        """update='local': the worker's arena optimizer (spec ``self._local_spec``) applied to ``grad_tensor``; ``zero`` is cleared."""
+        sp, f = self._local_spec, self.fabric
+        clip = sp.get("clip_gradient", -1.0)
+        # HFA applies the optimizer to the worker's own gradient arena, a sum over the batch: the reference's cnn_hfa.py steps the trainer
+        # with `trainer.step(num_samples)`, i.e. rescale_grad / B.  The pulled aggregate of the other local mode is already averaged.
+        rescale = sp["rescale_grad"] / self.B if self.hfa else sp["rescale_grad"]
+        native.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], rescale,
+                         -1.0 if clip is None else clip, sp.get("momentum", 0.0), sp.get("beta1", 0.9), sp.get("beta2", 0.999),
+                         sp.get("epsilon", 1e-8), sp.get("lamda", 0.04), self.opt_state, zero)
+
     def _steps(self):
-        """The training step as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch for weight
-        gradients), 'comm' (a key group's exchange on the high-priority stream), 'join' (main, after the side branch) or 'join_comm' (main,
-        after the side branch and the comm stream)."""
-        n = native
+        """The training step of ``self.path`` as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch
+        for weight gradients), 'comm' (a key group's exchange on the high-priority stream), 'join' (main, after the side branch) or 'join_comm'
+        (main, after the side branch and the comm stream).  The launches look their kernels, buffers and parameter blocks up when they run."""
+        n, path = native, self.path
         B, P, G, f = self.B, self.P, self.G, self.fabric
         a2f = self.a2.view(B, 512)
         Wc1, Gc1 = P[2].view(32, 400), G[2].view(32, 400)
-        kv = (lambda: (f.async_step(), f.grad.tensor.zero_() if self.fused_zero_grad else None)) if self.mode == "dist_async" else \
-            (lambda: f.fsa_step(zero_grad=self.fused_zero_grad))
-        if self.overlap:
-            kv = lambda: f.channel_step("conv", zero_grad=self.fused_zero_grad)
-        elif self.single:
-            kv = lambda: f.channel_step(self.single, zero_grad=self.fused_zero_grad)
-        kv_dense = [("hips push+opt+pull (dense keys, overlapped)", "comm", lambda: f.channel_step("dense", zero_grad=self.fused_zero_grad))] if self.overlap else []
-        carry = (self.label, self.label_cur) if self.lookahead else None
-        self._tail = []
-        if self.update == "local":
-            sp = self._local_spec
-            clip = sp.get("clip_gradient", -1.0)
-            # HFA applies the optimizer to the worker's own gradient arena, a sum over the batch: the reference's cnn_hfa.py steps the
-            # trainer with `trainer.step(num_samples)`, i.e. rescale_grad / B.  The pulled aggregate of the other local mode is already averaged.
-            rescale = sp["rescale_grad"] / B if self.hfa else sp["rescale_grad"]
+        carry = (self.label, self.label_cur) if path.lookahead else None
 
-            def local_opt(grad_tensor, zero=None):
-                n.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], rescale,
-                            -1.0 if clip is None else clip, sp.get("momentum", 0.0), sp.get("beta1", 0.9), sp.get("beta2", 0.999), sp.get("epsilon", 1e-8),
-                            sp.get("lamda", 0.04), self.opt_state, zero)
-            if self.hfa:
-                # HFA: no exchange inside the step; the optimizer consumes (and clears) the worker's own gradient arena
-                kv_dense = []
-                kv = lambda: local_opt(f.grad.tensor, f.grad.tensor if self.fused_zero_grad else None)
-            else:
-                # the exchange delivered the aggregated gradient into the fabric's parameter arena: one fused arena-optimizer launch applies it
-                self._tail = [("local optimizer (fused arena Adam)", "main", lambda: local_opt(f.param.tensor))]
-        def conv1_fwd():
-            # bias + ReLU + 2x2 max-pool in the GEMM epilogue (only the pooled map and its arg-max leave the SM); the two-kernel form is
-            # the fallback for geometries the in-warp pooling cannot express
-            if os.environ.get("GEOMX_NO_POOL_FUSION", "0") == "1" or not n.gemm_pool(self.col1, Wc1, self.a2, self.idx2, 8, 8, bias=P[3], relu=True):
-                n.gemm(self.col1, Wc1, self.z2, bias=P[3], relu=True, store_nchw_hw=64)
-                n.maxpool2x2_fwd(self.z2, self.a2, self.idx2)
-
-        head = [
-            ("dense0 gemm", "main", lambda: n.gemm(a2f, P[4], self.a3, bias=P[5], relu=True)),
-            ("dense1 gemm", "main", lambda: n.gemm(self.a3, P[6], self.a4, bias=P[7], relu=True)),
-            ("head fwd+bwd", "main", lambda: n.head_fwd_bwd(self.a4, P[8], P[9], self.label_cur, self.loss, self.logits, G[8], G[9], self.dz4, G[7], True)),
-            ("dW1 gemm", "side", lambda: n.gemm(self.dz4, self.a3, G[6], a_mn=True, b_mn=True)),
-            ("dz3 gemm (mask,colsum)", "main", lambda: n.gemm(self.dz4, P[6], self.dz3, b_mn=True, mask=self.a3, colsum=G[5])),
-            ("dW0 gemm", "side", lambda: n.gemm(self.dz3, a2f, G[4], a_mn=True, b_mn=True)),
-            ("da2 gemm", "main", lambda: n.gemm(self.dz3, P[4], self.da2, b_mn=True)),
-        ]
-        # even B <= 32 (paths with both the direct convolutions and the cluster kernel): dense0 is row-separable, so the forward kernel
-        # computes a3 on its 128 SMs and the cluster kernel starts from a3
-        self._fwd_dense0 = fwd_dense0 = self.direct_conv and self.fused_mlp
-        # ... and so is the rest of the chain down to dz3: in the classic step the forward kernel also runs dense1, the classifier, softmax-CE,
-        # dz4 and dz3, and the cluster kernel computes only da2 = dz3 W0.  A look-ahead launch ends with the NEXT batch's forward kernel, which
-        # would overwrite this batch's loss and logits before the host reads them: it keeps the forward kernel that stops at a3.
-        self._fwd_head = fwd_head = fwd_dense0 and not self.lookahead
-        head_out = dict(wd1=P[6], bd1=P[7], wd2=P[8], bd2=P[9], label=self.label_cur, loss=self.loss, logits=self.logits, a4=self.a4, dz4=self.dz4,
-                        dz3=self.dz3, dl=self.dl) if fwd_head else {}
-        if fwd_dense0:
-            def fwd():
+        # forward convolutions (the part a look-ahead launch runs for the NEXT batch)
+        if path.dense in ("a3", "dz3"):
+            def conv_fwd():
+                head = dict(wd1=P[6], bd1=P[7], wd2=P[8], bd2=P[9], label=self.label_cur, loss=self.loss, logits=self.logits, a4=self.a4,
+                            dz4=self.dz4, dz3=self.dz3, dl=self.dl) if path.dense == "dz3" else {}
                 if not n.cnn_fwd_dense0(self.x, P[0], P[1], P[2], P[3], P[4], P[5], self.a1, self.idx1, self.a2, self.idx2, self.a3, carry=carry,
-                                        x_keep=self.x_cur if self.lookahead else None, **head_out):
+                                        x_keep=self.x_cur if path.lookahead else None, **head):
                     raise RuntimeError("cnn_fwd_dense0 does not cover batch %d" % B)
+            fwd = [(DIRECT_FWD, "main", conv_fwd)]
+        elif path.direct_conv:
+            fwd = [(DIRECT_FWD, "main", lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry,
+                                                          x_keep=self.x_cur if path.lookahead else None))]
         else:
-            fwd = lambda: n.cnn_fwd(self.x, P[0], P[1], P[2], P[3], self.a1, self.idx1, self.a2, self.idx2, carry=carry,
-                                    x_keep=self.x_cur if self.lookahead else None)
-        if self.fused_mlp:
+            def conv1_fwd():
+                # bias + ReLU + 2x2 max-pool in the GEMM epilogue (only the pooled map and its arg-max leave the SM); the two-kernel form is
+                # the fallback for geometries the in-warp pooling cannot express
+                if not (path.pool_fusion and n.gemm_pool(self.col1, Wc1, self.a2, self.idx2, 8, 8, bias=P[3], relu=True)):
+                    n.gemm(self.col1, Wc1, self.z2, bias=P[3], relu=True, store_nchw_hw=64)
+                    n.maxpool2x2_fwd(self.z2, self.a2, self.idx2)
+                if path.lookahead:
+                    self.label_cur.copy_(self.label); self.x_cur.copy_(self.x)
+            fwd = [(GEMM_FWD[0], "main", lambda: n.conv_relu_pool_im2col_fwd(self.x, P[0], P[1], self.a1, self.idx1, self.col1, 5, 5)),
+                   (GEMM_FWD[1], "main", conv1_fwd)]
+
+        # dense chain: forward and backward down to da2, the input of the convolution backward pass
+        wgrad = lambda: n.dense_wgrad(a2f, self.a3, self.a4, self.dz4, self.dz3, self.dl, G[4], G[5], G[6], G[7], G[8], G[9])
+        if path.dense == "gemm":
+            dense = [
+                ("dense0 gemm", "main", lambda: n.gemm(a2f, P[4], self.a3, bias=P[5], relu=True)),
+                ("dense1 gemm", "main", lambda: n.gemm(self.a3, P[6], self.a4, bias=P[7], relu=True)),
+                ("head fwd+bwd", "main", lambda: n.head_fwd_bwd(self.a4, P[8], P[9], self.label_cur, self.loss, self.logits, G[8], G[9], self.dz4, G[7],
+                                                                True)),
+                ("dW1 gemm", "side", lambda: n.gemm(self.dz4, self.a3, G[6], a_mn=True, b_mn=True)),
+                ("dz3 gemm (mask,colsum)", "main", lambda: n.gemm(self.dz4, P[6], self.dz3, b_mn=True, mask=self.a3, colsum=G[5])),
+                ("dW0 gemm", "side", lambda: n.gemm(self.dz3, a2f, G[4], a_mn=True, b_mn=True)),
+                ("da2 gemm", "main", lambda: n.gemm(self.dz3, P[4], self.da2, b_mn=True)),
+            ]
+        elif path.dense == "a2":
             # dense0 -> dense1 -> classifier -> softmax-CE forward and backward: one cluster launch for the data path (what the convolution
             # backward pass waits for) and one weight-gradient launch on a parallel branch, instead of the seven above
-            if fwd_dense0:
-                chain = lambda: n.dense_tail(self.a3, P[4], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2, self.a4,
-                                             self.dz4, self.dz3, self.dl, from_dz3=fwd_head)
-            else:
-                chain = lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2,
-                                                 self.a3, self.a4, self.dz4, self.dz3, self.dl)
-            head = [("mlp chain fwd+bwd (cluster)", "main", chain)]
-            wgrad = lambda: n.dense_wgrad(a2f, self.a3, self.a4, self.dz4, self.dz3, self.dl, G[4], G[5], G[6], G[7], G[8], G[9])
-            if kv_dense and not self.lookahead:
-                # the dense channel reads these gradients: issued in the same comm-stream step, only a programmatic edge separates the two
-                name, _, chan = kv_dense[0]
-                kv_dense = [("dense weight gradients + " + name, "comm", lambda: (wgrad(), chan()))]
-            else:
-                # side stream, joined before the exchange (a dense channel's comm step waits for it too).  A look-ahead launch ends with
-                # the next batch's forward convolutions, which overwrite the x this kernel reads: _body joins the side branch before them
-                head.append(("dense weight gradients", "side", wgrad))
-        # number of leading steps that only need the batch and the weights (the part a look-ahead launch runs for the NEXT batch)
-        self._n_fwd = 1 if self.direct_conv else 2
-        if self.direct_conv:
-            da2v = self.da2
-            if os.environ.get("GEOMX_CNN_BWD_ONE_LAUNCH", "1") == "1" and B % 2 == 0 and B <= 64:
-                # both backward jobs in one heterogeneous grid: no side-stream fork / join around the convolution backward
-                fused = f.channel_fused_args("conv", zero_grad=self.fused_zero_grad) if self.overlap else None
-                self.fused_exchange = fused is not None
-                if fused is not None:
-                    # ... and the conv keys' exchange in the tail of the same launch (the CTAs that finish last serve one tile each)
-                    blk, tiles, n_act = fused
-                    return [
-                        ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
-                    ] + head + kv_dense + [
-                        ("conv bwd (one grid) + conv-key exchange in its tail", "main",
-                         lambda: n.cnn_bwd_exchange(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1], G[2], G[3], blk, tiles, n_act)),
-                    ] + self._tail
-                return [
-                    ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
-                ] + head + kv_dense + [
-                    ("conv bwd: conv1 wgrad + dgrad + conv0 wgrad (direct, one grid)", "main",
-                     lambda: n.cnn_bwd_all(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1], G[2], G[3])),
-                    ("hips push+opt+pull", "join", kv),
-                ] + self._tail
-            return [
-                ("conv0+conv1 fwd (direct, relu+pool fused)", "main", fwd),
-            ] + head + kv_dense + [
-                ("conv1 wgrad (direct, sparse)", "side", lambda: n.cnn_wgrad1(self.a1, self.a2, self.idx2, da2v, G[2], G[3])),
-                ("conv1 dgrad + conv0 wgrad (direct)", "main", lambda: n.cnn_bwd(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, da2v, G[0], G[1])),
-                ("hips push+opt+pull", "join", kv),
-            ] + self._tail
-        if self.lookahead:
-            conv1 = conv1_fwd
-            conv1_fwd = lambda: (conv1(), self.label_cur.copy_(self.label), self.x_cur.copy_(self.x))
-        return [
-            ("conv0+relu+pool+im2col", "main", lambda: n.conv_relu_pool_im2col_fwd(self.x, P[0], P[1], self.a1, self.idx1, self.col1, 5, 5)),
-            ("conv1 gemm (bias,relu,maxpool fused)", "main", conv1_fwd),
-        ] + head + kv_dense + [
-            ("pool+relu bwd -> rows", "main", lambda: n.pool_relu_bwd_rows(self.da2.view(B, 32, 4, 4), self.a2, self.idx2, self.dz2rows, G[3])),
-            ("dWc1 gemm (split-K)", "side", lambda: n.gemm(self.dz2rows, self.col1, Gc1, a_mn=True, b_mn=True, split_k=16, accumulate=True)),
-            ("dcol1 gemm", "main", lambda: n.gemm(self.dz2rows, Wc1, self.dcol1, b_mn=True)),
-            ("conv0 wgrad + col2im", "main", lambda: n.conv_relu_pool_wgrad_col2im(self.x_cur, self.dcol1, self.a1, self.idx1, G[0], G[1], CNN_PARAM_SHAPES[0], 5, 5)),
-            ("hips push+opt+pull", "join", kv),
-        ] + self._tail
+            dense = [(MLP, "main", lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits,
+                                                            self.da2, self.a3, self.a4, self.dz4, self.dz3, self.dl))]
+        else:
+            dense = [(MLP, "main", lambda: n.dense_tail(self.a3, P[4], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2,
+                                                        self.a4, self.dz4, self.dz3, self.dl, from_dz3=path.dense == "dz3"))]
+        if path.wgrad == "side":
+            dense.append((DENSE_WGRAD, "side", wgrad))
+
+        # the dense keys' exchange on the comm stream; the dense weight gradients go in the same step when they are issued there (only a
+        # programmatic edge separates the two)
+        dense_kv = lambda: f.channel_step("dense", zero_grad=self.fused_zero_grad)
+        if path.wgrad == "comm":
+            comm = [(DENSE_WGRAD + " + " + DENSE_KV, "comm", lambda: (wgrad(), dense_kv()))]
+        else:
+            comm = [(DENSE_KV, "comm", dense_kv)] if path.overlap else []
+
+        # convolution backward
+        if path.bwd == "exchange_tail":
+            # both backward jobs in one heterogeneous grid, and the conv keys' exchange in its tail (the CTAs that finish last serve one tile each)
+            def bwd_exchange():
+                fused = f.channel_fused_args("conv", zero_grad=self.fused_zero_grad)
+                if fused is None:
+                    raise RuntimeError("the conv keys' channel can no longer run in the backward grid's tail")
+                n.cnn_bwd_exchange(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, self.da2, G[0], G[1], G[2], G[3], *fused)
+            bwd = [(FUSED_BWD, "main", bwd_exchange)]
+        elif path.bwd == "one_grid":
+            # both backward jobs in one heterogeneous grid: no side-stream fork / join around the convolution backward
+            bwd = [(ONE_GRID, "main", lambda: n.cnn_bwd_all(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2, self.da2, G[0], G[1], G[2],
+                                                            G[3]))]
+        elif path.bwd == "two_launch":
+            bwd = [("conv1 wgrad (direct, sparse)", "side", lambda: n.cnn_wgrad1(self.a1, self.a2, self.idx2, self.da2, G[2], G[3])),
+                   ("conv1 dgrad + conv0 wgrad (direct)", "main", lambda: n.cnn_bwd(self.x_cur, P[2], self.a1, self.idx1, self.a2, self.idx2,
+                                                                                    self.da2, G[0], G[1]))]
+        else:
+            bwd = [
+                ("pool+relu bwd -> rows", "main", lambda: n.pool_relu_bwd_rows(self.da2.view(B, 32, 4, 4), self.a2, self.idx2, self.dz2rows, G[3])),
+                ("dWc1 gemm (split-K)", "side", lambda: n.gemm(self.dz2rows, self.col1, Gc1, a_mn=True, b_mn=True, split_k=16, accumulate=True)),
+                ("dcol1 gemm", "main", lambda: n.gemm(self.dz2rows, Wc1, self.dcol1, b_mn=True)),
+                ("conv0 wgrad + col2im", "main", lambda: n.conv_relu_pool_wgrad_col2im(self.x_cur, self.dcol1, self.a1, self.idx1, G[0], G[1],
+                                                                                       CNN_PARAM_SHAPES[0], 5, 5)),
+            ]
+
+        # the exchange, after the backward pass and the side branch (unless it runs in the backward grid's tail)
+        if path.bwd == "exchange_tail":
+            exchange = []
+        elif path.exchange in ("conv", "all"):
+            exchange = [(EXCH, "join", lambda: f.channel_step(path.exchange, zero_grad=self.fused_zero_grad))]
+        elif path.exchange == "local_opt":
+            # HFA: no exchange inside the step; the optimizer consumes (and clears) the worker's own gradient arena
+            exchange = [(EXCH, "join", lambda: self._local_opt(f.grad.tensor, f.grad.tensor if self.fused_zero_grad else None))]
+        elif path.exchange == "async":
+            exchange = [(EXCH, "join", lambda: (f.async_step(), f.grad.tensor.zero_() if self.fused_zero_grad else None))]
+        else:
+            exchange = [(EXCH, "join", lambda: f.fsa_step(zero_grad=self.fused_zero_grad))]
+
+        # update='local': the exchange delivered the aggregated gradient into the fabric's parameter arena; one arena-optimizer launch applies it
+        tail = [(LOCAL, "main", lambda: self._local_opt(f.param.tensor))] if path.local_tail else []
+        return fwd + dense + comm + bwd + exchange + tail
 
     def _body(self, stop_after=None, part="all"):
         """Issue the step (``part='all'``), only its forward convolutions (``'fwd'``), everything after them (``'rest'``), or the look-ahead
@@ -403,10 +484,7 @@ class HipsCNNTrainStep:
         main, side, comm = torch.cuda.current_stream(), self._side, self._comm
         forked = comm_forked = False
         steps = self._steps()
-        nf = self._n_fwd
-        # rotated: the next batch's forward convolutions overwrite a2 (and a3), which the side branch (dense weight gradients) may still be
-        # reading; a forward kernel that also computes dense0 reads W0 / b0, which the dense keys' exchange (comm) updates
-        join = "join_comm" if self._fwd_dense0 else "join"
+        nf, join = self.path.n_fwd, self.path.lookahead_join
         rotated = steps[nf:] + [(name, join if where == "main" else where, fn) for name, where, fn in steps[:nf]]
         steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": rotated}[part]
         for i, (name, where, fn) in enumerate(steps):
@@ -551,10 +629,9 @@ class HipsCNNTrainStep:
     def _pipeline(self):
         if not hasattr(self, "_pl"):
             dev, B = self.device, self.B
-            # direct mode: the two H2D targets ARE the step's two input buffers (one captured graph each); look-ahead steps and DGT runs
-            # keep the single-graph form with a staging -> compute copy
-            self._direct_inputs = not self.lookahead and os.environ.get("GEOMX_E2E_DIRECT_INPUT", "1") == "1"
-            if self._direct_inputs:
+            # direct mode: the two H2D targets ARE the step's two input buffers (one captured graph each); look-ahead steps keep the
+            # single-graph form with a staging -> compute copy
+            if self.path.direct_input:
                 self._xbufs[1] = torch.empty_like(self.xin)
                 stage = [self._xbufs[0], self._xbufs[1]]
             else:
@@ -595,7 +672,7 @@ class HipsCNNTrainStep:
                 pl["sy"][b].copy_(y.reshape(self.label.shape), non_blocking=True)
                 pl["ready"][b].record(h2d)
             main.wait_event(pl["ready"][b])
-            if not self._direct_inputs:
+            if not self.path.direct_input:
                 self.xin.copy_(pl["stage"][b], non_blocking=True)
         if pl["last_loss"] is not None:
             main.wait_event(pl["last_loss"])                # the loss buffer of the previous step has been read out
@@ -607,7 +684,7 @@ class HipsCNNTrainStep:
             self._prime()
             pl["done"][b].record(main)
             return LossHandle(None, None)
-        self.run_device(buf=b if (not X.is_cuda and self._direct_inputs) else 0)
+        self.run_device(buf=b if (not X.is_cuda and self.path.direct_input) else 0)
         pl["done"][b].record(main)
         host, ev = pl["ring"][i % 4]
         d2h = pl["d2h"]

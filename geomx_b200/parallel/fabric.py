@@ -538,10 +538,11 @@ class HipsFabric:
     def channel_fused_args(self, name, zero_grad=False):
         """For compute kernels that perform a replicated channel's exchange in their own tail (cnn_bwd_exchange_kernel): the channel's
         parameter block, its tile list and tile count — or ``None`` when the channel needs a launch of its own (sharded mode, Bi-Sparse
-        tiles, DGT bookkeeping, or a multi-rank job without the direct-protocol buffers)."""
+        tiles, DGT bookkeeping, or a multi-rank job without the direct-protocol buffers).  Whether a step uses a capable channel this way
+        is the step's choice."""
         ch = self.channels[name]
         single = self.topo.world == 1 and not self.loopback
-        if not ch["replicate"] or self.dgt_contrib is not None or os.environ.get("GEOMX_FUSED_EXCHANGE", "0") != "1":
+        if not ch["replicate"] or self.dgt_contrib is not None:
             return None
         if not single and (self.ll_d is None or not self._channel_formats_direct_ok(ch)):
             return None

@@ -8,12 +8,11 @@ import pytest
 import torch
 
 import geomx_b200 as mx
+from geomx_b200.models.cnn import STEP_SWITCHES
 
 pytestmark = pytest.mark.gpu
 
 D0, D1, D2 = 512, 256, 128
-STEP_SWITCHES = ("GEOMX_CNN_BWD_ONE_LAUNCH", "GEOMX_FUSED_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_NO_POOL_FUSION",
-                 "GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE")
 
 
 @pytest.fixture(scope="module")

@@ -13,13 +13,13 @@ import torch
 import torch.nn.functional as F
 
 import geomx_b200 as mx
+from geomx_b200.models.cnn import STEP_SWITCHES
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 D0, D1, D2 = 512, 256, 128
-STEP_SWITCHES = ("GEOMX_CNN_BWD_ONE_LAUNCH", "GEOMX_FUSED_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_NO_POOL_FUSION",
-                 "GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE", "GEOMX_MLP_CLUSTER")
+SWITCHES = STEP_SWITCHES + ("GEOMX_MLP_CLUSTER",)
 
 
 @pytest.fixture(scope="module")
@@ -187,7 +187,7 @@ def test_dense_tail_cluster8_matches_fp64():
 # ---------------------------------------------------------------------------------------------------------------- in the step
 def test_captured_step_runs_the_new_pair(nat, monkeypatch):
     from geomx_b200.parallel import Topology
-    for k in STEP_SWITCHES:
+    for k in SWITCHES:
         monkeypatch.delenv(k, raising=False)
     B = 32
     g = torch.Generator().manual_seed(900)

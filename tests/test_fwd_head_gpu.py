@@ -10,12 +10,12 @@ import torch
 import torch.nn.functional as F
 
 import geomx_b200 as mx
+from geomx_b200.models.cnn import STEP_SWITCHES
 
 pytestmark = pytest.mark.gpu
 
 D0, D1, D2, C = 512, 256, 128, 10
-STEP_SWITCHES = ("GEOMX_CNN_BWD_ONE_LAUNCH", "GEOMX_FUSED_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_NO_POOL_FUSION",
-                 "GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE", "GEOMX_MLP_CLUSTER")
+SWITCHES = STEP_SWITCHES + ("GEOMX_MLP_CLUSTER",)
 HEAD_OUT = ("loss", "logits", "a4", "dz4", "dz3", "dl")
 
 
@@ -160,7 +160,7 @@ def test_captured_step_pair(nat, monkeypatch, lookahead):
     """B = 32: the classic step runs the forward kernel with its head and the tail from dz3; the look-ahead step keeps the pair through a3
     (its launch ends with the next batch's forward kernel, which would overwrite the loss and logits the host has not read yet)."""
     from geomx_b200.parallel import Topology
-    for k in STEP_SWITCHES:
+    for k in SWITCHES:
         monkeypatch.delenv(k, raising=False)
     seen = {"fwd": [], "tail": []}
     fwd, tail = nat.cnn_fwd_dense0, nat.dense_tail

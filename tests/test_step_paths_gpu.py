@@ -10,6 +10,9 @@
   F  E with GEMM (NCHW store) + separate max-pool kernel          GEOMX_NO_POOL_FUSION=1
   G  GEMM convolutions and GEMM dense part                        B = 33, B > 64
 
+``tests/test_step_path.py`` checks the choice of path (``step_path``) without a GPU; this file checks that each path's launches run, in the
+recorded order and on the recorded streams, and compute the step.
+
 The reference takes the two max-pool arg-max decisions from the kernels (``idx1`` / ``idx2``): a window whose two largest candidates agree to
 fp32 rounding can legitimately go either way.  Those decisions are checked separately against the fp64 first maximum, wherever the window is
 not such a near-tie.  Exact ties (the zero background of the demo's images makes every conv0 window there a four-way tie) must resolve to the
@@ -26,11 +29,9 @@ import torch
 import torch.nn.functional as F
 
 import geomx_b200 as mx
+from geomx_b200.models.cnn import DENSE_KV, DENSE_WGRAD, DIRECT_FWD, EXCH, FUSED_BWD, GEMM_FWD, MLP, ONE_GRID, STEP_SWITCHES
 
 pytestmark = pytest.mark.gpu
-
-STEP_SWITCHES = ("GEOMX_CNN_BWD_ONE_LAUNCH", "GEOMX_FUSED_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_NO_POOL_FUSION",
-                 "GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE")
 
 
 @pytest.fixture(scope="module")
@@ -166,22 +167,23 @@ def step_params(g):
 
 
 # ---------------------------------------------------------------------------------------------------------------- 1. the step, per path
-ONE_GRID = "conv bwd: conv1 wgrad + dgrad + conv0 wgrad (direct, one grid)"
-DIRECT_FWD = "conv0+conv1 fwd (direct, relu+pool fused)"
-GEMM_CONV = ["conv0+relu+pool+im2col", "conv1 gemm (bias,relu,maxpool fused)", "pool+relu bwd -> rows", "dWc1 gemm (split-K)", "dcol1 gemm",
-             "conv0 wgrad + col2im"]
-MLP = ["mlp chain fwd+bwd (cluster)"]
-GEMM_HEAD = ["dense0 gemm", "dense1 gemm", "head fwd+bwd", "dW1 gemm", "dz3 gemm (mask,colsum)", "dW0 gemm", "da2 gemm"]
+# the ordered (launch, stream) lists of the step on one rank (overlapped channels: the dense keys' exchange on the comm stream)
+WGRAD_KV = (DENSE_WGRAD + " + " + DENSE_KV, "comm")
+GEMM_CONV_FWD = [(GEMM_FWD[0], "main"), (GEMM_FWD[1], "main")]
+GEMM_CONV_BWD = [("pool+relu bwd -> rows", "main"), ("dWc1 gemm (split-K)", "side"), ("dcol1 gemm", "main"), ("conv0 wgrad + col2im", "main")]
+GEMM_HEAD = [("dense0 gemm", "main"), ("dense1 gemm", "main"), ("head fwd+bwd", "main"), ("dW1 gemm", "side"), ("dz3 gemm (mask,colsum)", "main"),
+             ("dW0 gemm", "side"), ("da2 gemm", "main")]
 
-# path -> (direct_conv, fused_mlp, fused_exchange, step names that must be present)
+# path -> (direct_conv, fused_mlp, fused_exchange, the step's (launch, stream) list)
 PATHS = {
-    "A": (True, True, False, [DIRECT_FWD, ONE_GRID] + MLP),
-    "B": (True, True, False, [DIRECT_FWD, "conv1 wgrad (direct, sparse)", "conv1 dgrad + conv0 wgrad (direct)"] + MLP),
-    "C": (True, True, True, [DIRECT_FWD, "conv bwd (one grid) + conv-key exchange in its tail"] + MLP),
-    "D": (True, False, False, [DIRECT_FWD, ONE_GRID] + GEMM_HEAD),
-    "E": (False, True, False, GEMM_CONV + MLP),
-    "F": (False, True, False, GEMM_CONV + MLP),
-    "G": (False, False, False, GEMM_CONV + GEMM_HEAD),
+    "A": (True, True, False, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, (ONE_GRID, "main"), (EXCH, "join")]),
+    "B": (True, True, False, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, ("conv1 wgrad (direct, sparse)", "side"),
+                              ("conv1 dgrad + conv0 wgrad (direct)", "main"), (EXCH, "join")]),
+    "C": (True, True, True, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, (FUSED_BWD, "main")]),
+    "D": (True, False, False, [(DIRECT_FWD, "main")] + GEMM_HEAD + [(DENSE_KV, "comm"), (ONE_GRID, "main"), (EXCH, "join")]),
+    "E": (False, True, False, GEMM_CONV_FWD + [(MLP, "main"), WGRAD_KV] + GEMM_CONV_BWD + [(EXCH, "join")]),
+    "F": (False, True, False, GEMM_CONV_FWD + [(MLP, "main"), WGRAD_KV] + GEMM_CONV_BWD + [(EXCH, "join")]),
+    "G": (False, False, False, GEMM_CONV_FWD + GEMM_HEAD + [(DENSE_KV, "comm")] + GEMM_CONV_BWD + [(EXCH, "join")]),
 }
 CASES = [("A", 2, {}), ("A", 32, {}),
          ("B", 32, {"GEOMX_CNN_BWD_ONE_LAUNCH": "0"}),
@@ -220,10 +222,9 @@ def test_step_path_matches_fp64(nat, monkeypatch, path, B, env, data):
         eng._body(); torch.cuda.synchronize()
         # the intended kernels ran (otherwise a case would quietly test another path)
         direct, fused_mlp, fused_exchange, want = PATHS[path]
-        names = [n for n, _, _ in eng._steps()]
-        assert (eng.direct_conv, eng.fused_mlp, eng.fused_exchange) == (direct, fused_mlp, fused_exchange), (path, B, names)
-        missing = [n for n in want if n not in names]
-        assert not missing, (path, B, missing, names)
+        steps = [(n, s) for n, s, _ in eng._steps()]
+        assert (eng.direct_conv, eng.fused_mlp, eng.fused_exchange) == (direct, fused_mlp, fused_exchange), (path, B, steps)
+        assert steps == want, (path, B, steps)
         if not direct:        # the pooled conv1 GEMM leaves z2 untouched; the unfused form writes it and pools it separately
             assert bool(torch.isnan(eng.z2).all()) == (path != "F"), path
         loss, logits = eng.loss.clone(), eng.logits.clone()
@@ -241,6 +242,34 @@ def test_step_path_matches_fp64(nat, monkeypatch, path, B, env, data):
         assert max(again) < 1e-6 and rel_err(eng.loss, loss) < 1e-6, (path, B, data, again)
         for i, (p, p0) in enumerate(zip(eng.P, P0)):
             assert torch.equal(p, p0), "parameter %d changed by an lr = 0 step (path %s)" % (i, path)
+    finally:
+        del eng
+        gc.collect()
+        torch.cuda.empty_cache()
+
+
+def test_switches_are_read_at_construction(nat, monkeypatch):
+    """The kernel path is chosen when the engine is constructed: step switches changed afterwards change neither the step's launches nor the
+    graph that the host pipeline captures later on its second input buffer."""
+    from geomx_b200.parallel import Topology
+    for k in STEP_SWITCHES:
+        monkeypatch.delenv(k, raising=False)
+    B = 32
+    eng = mx.models.HipsCNNTrainStep(batch_size=B, optimizer=mx.optimizer.SGD(learning_rate=0.0), topo=Topology(1, 0, 1, 1), use_graph=True)
+    try:
+        g = torch.Generator().manual_seed(77)
+        eng.x.copy_(images(g, B, "rand")); eng.label.copy_(torch.randint(0, 10, (B,), generator=g).float().to(dev()))
+        steps = [(n, s) for n, s, _ in eng._steps()]
+        assert steps == PATHS["A"][3], steps
+        eng.capture(); torch.cuda.synchronize()
+        assert eng.kernels_per_step == 6, eng.kernels_per_step
+        for k, v in (("GEOMX_CNN_BWD_ONE_LAUNCH", "0"), ("GEOMX_FUSED_EXCHANGE", "1"), ("GEOMX_DIRECT_CONV", "0"), ("GEOMX_FUSED_MLP", "0"),
+                     ("GEOMX_E2E_DIRECT_INPUT", "0")):
+            monkeypatch.setenv(k, v)
+        assert [(n, s) for n, s, _ in eng._steps()] == steps
+        eng._pipeline()
+        eng._alt_graph(); torch.cuda.synchronize()
+        assert eng.kernels_per_step == 6, eng.kernels_per_step
     finally:
         del eng
         gc.collect()

@@ -24,14 +24,16 @@ import torch
 import torch.nn.functional as F
 
 import geomx_b200 as mx
+from geomx_b200.models.cnn import DENSE_WGRAD, DIRECT_FWD, EXCH, LOCAL, MLP, ONE_GRID, STEP_SWITCHES
 
 import _update_ref as R
+from test_step_paths_gpu import PATHS
 
 pytestmark = pytest.mark.gpu
 
-STEP_SWITCHES = ("GEOMX_CNN_BWD_ONE_LAUNCH", "GEOMX_FUSED_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_NO_POOL_FUSION",
-                 "GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE", "GEOMX_FABRIC_PROTOCOL", "GEOMX_FABRIC_DIRECT", "GEOMX_PY_UPDATER",
-                 "GEOMX_WIRE_FP8", "ENABLE_DGT", "ENABLE_P3", "MXNET_KVSTORE_USE_HFA")
+# the step switches and the fabric's own
+SWITCHES = STEP_SWITCHES + ("GEOMX_FABRIC_PROTOCOL", "GEOMX_FABRIC_DIRECT", "GEOMX_PY_UPDATER", "GEOMX_WIRE_FP8", "ENABLE_DGT", "ENABLE_P3",
+                            "MXNET_KVSTORE_USE_HFA")
 
 TOL = R.DISP_TOL
 
@@ -47,7 +49,7 @@ def nat():
 
 @pytest.fixture
 def clean_env(monkeypatch):
-    for k in STEP_SWITCHES:
+    for k in SWITCHES:
         monkeypatch.delenv(k, raising=False)
     return monkeypatch
 
@@ -433,14 +435,10 @@ def test_fabric_dgt_contribution(nat, clean_env, path):
 
 
 # ============================================================================================================ c. the engine
-DIRECT_FWD = "conv0+conv1 fwd (direct, relu+pool fused)"
-ONE_GRID = "conv bwd: conv1 wgrad + dgrad + conv0 wgrad (direct, one grid)"
-MLP = "mlp chain fwd+bwd (cluster)"
-DENSE_CH = "dense weight gradients + hips push+opt+pull (dense keys, overlapped)"
-EXCH = "hips push+opt+pull"
-LOCAL = "local optimizer (fused arena Adam)"
-FUSED_BWD = "conv bwd (one grid) + conv-key exchange in its tail"
-GEMM_CONV = "conv0+relu+pool+im2col"
+# the step's (launch, stream) lists: paths A, C and G of test_step_paths_gpu.py; one exchange after the backward pass; local updates
+A, C, G = PATHS["A"][3], PATHS["C"][3], PATHS["G"][3]
+ONE = [(DIRECT_FWD, "main"), (MLP, "main"), (DENSE_WGRAD, "side"), (ONE_GRID, "main"), (EXCH, "join")]
+A_LOCAL = A + [(LOCAL, "main")]
 
 
 def _opt(kind, clip=None):
@@ -471,25 +469,25 @@ def _clip_for(P0, X, y, B, rescale):
     return float(torch.quantile(flat[flat > 0].cpu(), 0.8))
 
 
-# name -> (B, env, optimizer kind, engine kwargs, graph, step names that must run, attribute checks)
+# name -> (B, env, optimizer kind, engine kwargs, graph, the step's (launch, stream) list, attribute checks)
 ENGINE_CASES = {
-    "A-adam": (32, {}, "adam", {}, False, [DIRECT_FWD, ONE_GRID, MLP, DENSE_CH], dict(overlap=True)),
-    "A-adam-graph": (32, {}, "adam", {}, True, [DIRECT_FWD, ONE_GRID, MLP, DENSE_CH], dict(overlap=True)),
-    "A-sgd": (32, {}, "sgd", {}, False, [DIRECT_FWD, ONE_GRID, MLP], dict(overlap=True)),
-    "A-dcasgd": (32, {}, "dcasgd", {}, False, [DIRECT_FWD, ONE_GRID, MLP], dict(overlap=True)),
-    "C-adam": (32, {"GEOMX_FUSED_EXCHANGE": "1"}, "adam", {}, False, [DIRECT_FWD, FUSED_BWD, MLP], dict(fused_exchange=True)),
-    "G-sgd": (96, {}, "sgd", {}, False, [GEMM_CONV, EXCH], dict(direct_conv=False, fused_mlp=False)),
-    "single-adam": (32, {"GEOMX_STEP_OVERLAP": "0"}, "adam", {}, False, [DIRECT_FWD, ONE_GRID, EXCH], dict(overlap=False)),
-    "loopback-ov1-adam": (32, {"GEOMX_STEP_OVERLAP": "1"}, "adam", dict(loopback=True), False, [DENSE_CH], dict(overlap=True)),
-    "loopback-ov1-sgd": (32, {"GEOMX_STEP_OVERLAP": "1"}, "sgd", dict(loopback=True), False, [DENSE_CH], dict(overlap=True)),
-    "loopback-ov0-adam": (32, {"GEOMX_STEP_OVERLAP": "0"}, "adam", dict(loopback=True), False, [EXCH], dict(overlap=False)),
-    "loopback-ov0-sgd": (32, {"GEOMX_STEP_OVERLAP": "0"}, "sgd", dict(loopback=True), False, [EXCH], dict(overlap=False)),
-    "loopback-fp16": (32, {"GEOMX_STEP_OVERLAP": "1"}, "adam", dict(loopback=True, wire_dtype="fp16"), False, [DENSE_CH], dict(overlap=True)),
-    "loopback-fp8": (32, {"GEOMX_STEP_OVERLAP": "0"}, "sgd", dict(loopback=True, wire_dtype="fp8"), False, [EXCH], dict(overlap=False)),
-    "async-adam": (32, {}, "adam", dict(mode="dist_async"), False, [EXCH], dict(overlap=False, mode="dist_async")),
-    "local-adam": (32, {}, "adam", dict(update="local"), False, [EXCH, LOCAL], dict(update="local")),
-    "local-dcasgd": (32, {}, "dcasgd", dict(update="local"), False, [EXCH, LOCAL], dict(update="local")),
-    "hfa-sgd": (32, {}, "sgd", dict(hfa=(2, 2)), False, [EXCH], dict(update="local", hfa=(2, 2))),
+    "A-adam": (32, {}, "adam", {}, False, A, dict(overlap=True)),
+    "A-adam-graph": (32, {}, "adam", {}, True, A, dict(overlap=True)),
+    "A-sgd": (32, {}, "sgd", {}, False, A, dict(overlap=True)),
+    "A-dcasgd": (32, {}, "dcasgd", {}, False, A, dict(overlap=True)),
+    "C-adam": (32, {"GEOMX_FUSED_EXCHANGE": "1"}, "adam", {}, False, C, dict(fused_exchange=True)),
+    "G-sgd": (96, {}, "sgd", {}, False, G, dict(direct_conv=False, fused_mlp=False)),
+    "single-adam": (32, {"GEOMX_STEP_OVERLAP": "0"}, "adam", {}, False, ONE, dict(overlap=False)),
+    "loopback-ov1-adam": (32, {"GEOMX_STEP_OVERLAP": "1"}, "adam", dict(loopback=True), False, A, dict(overlap=True)),
+    "loopback-ov1-sgd": (32, {"GEOMX_STEP_OVERLAP": "1"}, "sgd", dict(loopback=True), False, A, dict(overlap=True)),
+    "loopback-ov0-adam": (32, {"GEOMX_STEP_OVERLAP": "0"}, "adam", dict(loopback=True), False, ONE, dict(overlap=False)),
+    "loopback-ov0-sgd": (32, {"GEOMX_STEP_OVERLAP": "0"}, "sgd", dict(loopback=True), False, ONE, dict(overlap=False)),
+    "loopback-fp16": (32, {"GEOMX_STEP_OVERLAP": "1"}, "adam", dict(loopback=True, wire_dtype="fp16"), False, A, dict(overlap=True)),
+    "loopback-fp8": (32, {"GEOMX_STEP_OVERLAP": "0"}, "sgd", dict(loopback=True, wire_dtype="fp8"), False, ONE, dict(overlap=False)),
+    "async-adam": (32, {}, "adam", dict(mode="dist_async"), False, ONE, dict(overlap=False, mode="dist_async")),
+    "local-adam": (32, {}, "adam", dict(update="local"), False, A_LOCAL, dict(update="local")),
+    "local-dcasgd": (32, {}, "dcasgd", dict(update="local"), False, A_LOCAL, dict(update="local")),
+    "hfa-sgd": (32, {}, "sgd", dict(hfa=(2, 2)), False, ONE, dict(update="local", hfa=(2, 2))),
 }
 
 
@@ -518,9 +516,8 @@ def _engine_run(name, clean_env, steps=6, seed=0, fused_zero_grad=False):
             eng._local_spec = dict(eng._local_spec, clip_gradient=spec["clip_gradient"])
         else:
             eng.fabric.set_optimizer(dict(eng.fabric.opt_spec, clip_gradient=spec["clip_gradient"]))
-    names = [n for n, _, _ in eng._steps()]
-    missing = [n for n in want if n not in names]
-    assert not missing, (name, missing, names)
+    steps = [(n, s) for n, s, _ in eng._steps()]
+    assert steps == want, (name, steps)
     for a, v in attrs.items():
         assert getattr(eng, a) == v, (name, a, getattr(eng, a))
     if graph:
