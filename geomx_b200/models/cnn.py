@@ -585,8 +585,11 @@ class HipsCNNTrainStep:
     def run_device(self, buf=0):
         """One step on whatever is currently in input buffer ``buf`` (0: ``self.x`` / ``self.label``; device-only, used by the kernel-time
         bench and by the host pipeline)."""
-        if self._dgt_every and self.steps_done and self.steps_done % self._dgt_every == 0 and self.graph is not None:
-            self.fabric.dgt_rerank()          # outside the captured graph; order / formats are updated in place
+        # DGT: re-rank before every step whose count of steps already taken (graph warm-up steps included) is a positive multiple of
+        # dgt_rerank_every, eager or graphed; capture() also ranks once after its warm-up.  Outside any captured graph: the order and the
+        # formats are updated in place
+        if self._dgt_every and self.steps_done and self.steps_done % self._dgt_every == 0:
+            self.fabric.dgt_rerank()
         if self.use_graph:
             if self.graph is None:
                 self.capture()

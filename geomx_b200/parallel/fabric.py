@@ -212,10 +212,11 @@ def dgt_num_important(sorted_contrib, k, adaptive=False, k_min=0.2):
         return 0
     if not adaptive:
         return max(1, int(round(k * n)))
-    total = float(sorted_contrib.sum())
+    c = sorted_contrib.double()           # the total in the precision of the running sum: a tile below fp32 resolution still counts
+    total = float(c.sum())
     if total <= 0.0:
         return max(1, int(round(k_min * n)))
-    cum = torch.cumsum(sorted_contrib.double(), 0) / total
+    cum = torch.cumsum(c, 0) / total
     need = int(torch.searchsorted(cum, torch.tensor([k - 1e-12], dtype=cum.dtype, device=cum.device))[0]) + 1
     return max(1, min(n, max(need, int(round(k_min * n)))))
 

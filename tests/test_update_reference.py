@@ -5,6 +5,8 @@ that the reference computes what ``geomx_b200.optimizer``'s SGD / Adam / DCASGD 
 plausible kernel bug) moves the result by at least 100x the tolerance the GPU tests allow, on gradient sequences of the demo CNN's
 magnitudes — so those tolerances can catch each of those bugs.
 """
+import math
+
 import pytest
 import torch
 
@@ -134,3 +136,152 @@ def test_mutations_are_far_outside_the_gpu_tolerance():
     assert got == set(R.MUTATIONS), set(R.MUTATIONS) - got
     for c in checked:
         print("  %-7s mults=%-5s %-20s displacement error %.2e" % c)
+
+
+# ---------------------------------------------------------------------------------------------------------- Bi-Sparse tiles and DGT
+def test_bsc_stage_hand_made_tiles():
+    """The Bi-Sparse stage on hand-made tiles: the K largest |v| go, ties at the K-th magnitude to the lowest index; sent entries are
+    cleared in u and v, the rest carries over (u = 0.9u + g, v += u); the aggregate is what ``bsc_decompress`` makes of the (value, index)
+    list, and the pull (``bsc_pull_compress`` of the aggregate, then zero + scatter with ``-1`` padding) returns its non-zeros."""
+    from geomx_b200.kvstore import compression as gc
+    g1 = torch.zeros(1024, dtype=torch.float64)
+    g1[[5, 100, 700]] = 3.0
+    g1[[9, 400]] = -3.0
+    g1[50] = 7.0
+    g1[[2, 3]] = 0.5
+    K = 3
+    u, v = torch.zeros(1024, dtype=torch.float64), torch.zeros(1024, dtype=torch.float64)
+    agg, sels = R.bsc_round(u, v, g1, K)
+    assert sels[0].tolist() == [5, 9, 50]
+    zipped = torch.cat([g1[sels[0]], sels[0].double()]).float()
+    assert torch.equal(agg.float(), gc.bsc_decompress(zipped, 1024))
+    assert R.selection_slack(g1, sels[0], K) == 0.0
+    rest = g1.clone()
+    rest[sels[0]] = 0.0
+    assert torch.equal(u, rest) and torch.equal(v, rest)
+    # pull: the aggregate's non-zeros in index order, padded with index -1, scattered into a zeroed (here: dirty) tile
+    pulled = gc.bsc_pull_compress(agg.float(), K / 1024, 1)
+    assert pulled[K:].tolist() == [5.0, 9.0, 50.0]
+    assert torch.equal(gc.bsc_decompress(pulled, 1024, out=torch.full((1024,), 9.0), accumulate=False), agg.float())
+    # second round: momentum on what was not sent
+    g2 = torch.zeros(1024, dtype=torch.float64)
+    g2[700] = 1.0
+    agg2, sels2 = R.bsc_round(u, v, g2, K)
+    u_exp = rest * R.BSC_MOMENTUM + g2
+    v_exp = rest + u_exp
+    assert sels2[0].tolist() == [100, 400, 700]         # |v| = 3 + 0.9*3 (100, 400) and 3 + 0.9*3 + 1 (700)
+    assert torch.equal(agg2[[100, 400, 700]], v_exp[[100, 400, 700]])
+    # the mutations on the same tiles
+    u, v = torch.zeros(1024, dtype=torch.float64), torch.zeros(1024, dtype=torch.float64)
+    assert R.bsc_round(u, v, g1, K, mutation="bsc_ties_high_index")[1][0].tolist() == [50, 400, 700]
+    u, v = torch.zeros(1024, dtype=torch.float64), torch.zeros(1024, dtype=torch.float64)
+    R.bsc_round(u, v, g1, K, mutation="bsc_residual_kept")
+    assert torch.equal(v, g1)
+    # fewer than K non-zeros: every non-zero goes, the rest of the K packets carry zeros of the lowest indices
+    u, v = torch.zeros(1024, dtype=torch.float64), torch.zeros(1024, dtype=torch.float64)
+    g3 = torch.zeros(1024, dtype=torch.float64)
+    g3[[600, 601]] = -2.0
+    agg3, sels3 = R.bsc_round(u, v, g3, 5)
+    assert sels3[0].tolist() == [0, 1, 2, 600, 601] and torch.equal(agg3, g3)
+    # the slack of a selection that is not a top-K
+    assert R.selection_slack(g1, torch.tensor([5, 9, 2]), K) > 0.5
+    assert R.selection_slack(g1, torch.tensor([5, 9, 50, 100]), K) == float("inf")
+    assert R.selection_slack(g3, torch.tensor([600]), 5) == float("inf")
+    assert R.bsc_k(0.01) == 10 and R.bsc_k(1e-6) == 1 and R.bsc_k(0.5) == 512
+
+
+def test_per_tile_formats_match_per_key_formats():
+    """A key whose formats are given per tile computes what the per-key format computes when every tile has it; a mixed key rounds each
+    tile by its own format."""
+    gen = torch.Generator().manual_seed(21)
+    shapes = [(3000,), (1025,)]
+    W0 = [torch.randn(s, generator=gen) * 0.1 for s in shapes]
+    grads = R.cnn_like_grads(gen, shapes, 3)
+    spec = R.CASE_SPECS["adam"]
+    for after in (False, True):
+        a = R.UpdateRef(spec, W0, push_scale=1 / 32, fmts=["fp8", "fp16"], round_after_scale=after)
+        b = R.UpdateRef(spec, W0, push_scale=1 / 32, fmts=[["fp8"] * 3, ["fp16"] * 2], round_after_scale=after)
+        for gs in grads:
+            a.step(gs)
+            b.step(gs)
+        assert all(torch.equal(x, y) for x, y in zip(a.w, b.w))
+        assert all(torch.equal(x, y) for x, y in zip(a.params(), b.params()))
+    m = R.UpdateRef(None, W0, push_scale=1 / 32, fmts=[["fp32", "fp8", "fp16"], "fp32"], round_after_scale=True)
+    m.step(grads[0])
+    s = grads[0][0].float() * (1 / 32)
+    assert torch.equal(m.w[0][:1024], s[:1024].double())
+    assert torch.equal(m.w[0][1024:2048], R.fp8_wire(s[1024:2048]).double())
+    assert torch.equal(m.w[0][2048:], R.fp16_wire(s[2048:]).double())
+
+
+def test_num_important_matches_the_fabric():
+    """The reference's size of the important set equals ``dgt_num_important`` of the fabric, fixed and adaptive, on random and degenerate
+    contributions."""
+    from geomx_b200.parallel.fabric import dgt_num_important
+    gen = torch.Generator().manual_seed(4)
+    for n in (1, 2, 7, 100, 333):
+        for c in (torch.rand(n, generator=gen) ** 4, torch.zeros(n), torch.ones(n)):
+            c = c.sort(descending=True).values
+            for k in (0.1, 0.5, 0.8, 1.0):
+                for adaptive, k_min in ((False, 0.2), (True, 0.2), (True, 0.05), (True, 0.6)):
+                    assert R.num_important(c, k, adaptive, k_min) == dgt_num_important(c, k, adaptive, k_min), (n, k, adaptive, k_min)
+
+
+def _stage_case():
+    """The CNN's keys, Bi-Sparse on those >= 1000 elements (the bench's ``bsc`` configuration), Adam on the aggregate; CNN-like gradient
+    sums on a grid of 2^-4 so that tiles have exact ties at their K-th magnitude (as quantised gradients do)."""
+    gen = torch.Generator().manual_seed(12)
+    W0 = [torch.randn(s, generator=gen) * 0.1 for s in CNN_SHAPES]
+    grads = [[torch.round(g / 0.0625) * 0.0625 for g in gs] for gs in R.cnn_like_grads(gen, CNN_SHAPES, 6, batch=32)]
+    fmts = ["bsc" if math.prod(s) >= 1000 else "fp32" for s in CNN_SHAPES]
+    return W0, grads, fmts
+
+
+def test_stage_mutations_are_far_outside_the_gpu_tolerance():
+    """Every Bi-Sparse mutation moves the weights' displacement (or, for the scale applied after the selection, which is linear and so only
+    visible in the carried state, ``u`` / ``v``) by at least 100x the GPU tests' tolerance; so does skipping the DGT demotion."""
+    W0, grads, fmts = _stage_case()
+    spec = R.CASE_SPECS["adam"]
+    run = lambda mut: _run(R.UpdateRef(spec, W0, push_scale=1 / 32, fmts=fmts, round_after_scale=True, mutation=mut), grads)
+    good = run(None)
+    out = {}
+    for mut in ("bsc_no_momentum", "bsc_residual_kept", "bsc_ties_high_index", "bsc_scale_after_select"):
+        bad = run(mut)
+        e = R.displacement_err(bad.w, W0, good.w)
+        if mut == "bsc_scale_after_select":
+            assert e < 1e-6, e                   # linear: the aggregate is the same
+            e = max(R.rel(b, a) for a, b in zip(good.u + good.v, bad.u + bad.v) if a.norm() > 0)
+        out[mut] = e
+    # DGT: fp16 keys, re-ranked after two rounds by the reference's own contribution EMA; half the tiles demoted
+    fm16 = ["fp16" if math.prod(s) >= 1000 else "fp32" for s in CNN_SHAPES]
+    res = {}
+    for mut in (None, "dgt_no_demotion"):
+        ref = R.UpdateRef(spec, W0, push_scale=1 / 32, fmts=list(fm16), round_after_scale=True, mutation=mut)
+        ema = None
+        for k, gs in enumerate(grads):
+            ref.step(gs)
+            mean = torch.cat(ref.agg).abs().view(-1, 1024).mean(1)
+            ema = mean if ema is None else R.dgt_ema(ema, mean, 0.3)
+            if k == 1:
+                base = [f for i in range(len(W0)) for f in ref.tile_fmts(i)]
+                _, n_imp, new = R.dgt_formats(base, ema, 0.5, mutation=mut)
+                assert n_imp == round(0.5 * len(base))
+                pos = 0
+                for i in range(len(W0)):
+                    T = len(ref.tile_fmts(i))
+                    ref.fmts[i] = new[pos:pos + T]
+                    pos += T
+        res[mut] = ref
+    assert any("fp8" in f for f in res[None].fmts if isinstance(f, list))
+    out["dgt_no_demotion"] = R.displacement_err(res["dgt_no_demotion"].w, W0, res[None].w)
+    for m, e in out.items():
+        print("  %-24s %.2e" % (m, e))
+    assert set(out) == set(R.STAGE_MUTATIONS)
+    weak = {m: e for m, e in out.items() if not e >= 100 * R.DISP_TOL}
+    assert not weak, weak
+
+
+def _run(ref, grads):
+    for gs in grads:
+        ref.step(gs)
+    return ref
