@@ -919,45 +919,19 @@ __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, c
   stamp(21);
   const int t = tile_list[s_ticket - first];
   const uint32_t epoch = (round << 3) | (uint32_t)(p.channel_id & 7);
-  const int S = p.party_size, P = p.num_parties;
-  const long long n2 = 2 * p.n;
   int* err = p.state + 5;
-  int f = p.tile_fmt ? (int)p.tile_fmt[t] : FMT_F32;
-  if (f != FMT_F16 && f != FMT_F8) f = FMT_F32;
+  const int f = grad_fmt(fmt_of(p, t));
   const long long off = (long long)t * TILE + threadIdx.x * 4;
   float* g = p.grad[p.rank] + off;
   const float4 v = __ldcg(reinterpret_cast<const float4*>(g));  // written by other CTAs of this launch: read at L2
   if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
   const bool wire = p.ll_d[p.rank] != nullptr;                   // false: single rank without loop-back — nothing to exchange
-  if (wire) {
-    const long long slot = (long long)p.rank * n2 + 2 * off;
-    if (p.ll_d_mc != nullptr) ll_send_dense_mc(p.ll_d_mc + slot, v, f, epoch);
-    else for (int r = 0; r < p.world; ++r) ll_send_dense(p.ll_d[r] + slot, v, f, epoch);
-  }
+  if (wire) direct_send_all(p, off, v, f, epoch);
   stamp(22);
-  float lr = adam_lr(p.h, opt_t), wd = p.h.wd;
-  if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
-  float4 W = *reinterpret_cast<float4*>(p.w + off);             // state loads overlap the flight of the packets
-  float4 A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
-  float4 Bm = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
-  float4 agg = f4_scale(v, p.push_scale);
-  if (wire) {
-    const float* in = p.ll_d[p.rank] + 2 * off;
-    for (int gq = 0; gq < P; ++gq) {
-      float4 ps = ll_recv_dense(in + (long long)(gq * S) * n2, f, epoch, err);
-      for (int j = 1; j < S; ++j) ps = f4_add(ps, ll_recv_dense(in + (long long)(gq * S + j) * n2, f, epoch, err));
-      ps = f4_scale(ps, p.push_scale);
-      agg = gq == 0 ? ps : f4_add(agg, ps);
-    }
-  }
+  TileState s = tile_state_load(p, t, off, adam_lr(p.h, opt_t));  // state loads overlap the flight of the packets
+  const float4 agg = wire ? direct_recv_sum(p, off, f, epoch, err) : f4_scale(v, p.push_scale);
   stamp(23);
-  opt_apply(W.x, agg.x, A.x, Bm.x, p.h, lr, wd);
-  opt_apply(W.y, agg.y, A.y, Bm.y, p.h, lr, wd);
-  opt_apply(W.z, agg.z, A.z, Bm.z, p.h, lr, wd);
-  opt_apply(W.w, agg.w, A.w, Bm.w, p.h, lr, wd);
-  *reinterpret_cast<float4*>(p.w + off) = W;
-  if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = A;
-  if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = Bm;
+  const float4 W = tile_state_apply(p, off, s, agg);
   *reinterpret_cast<float4*>(p.param[p.rank] + off) = W;        // the pull is a local store: every rank holds the fresh replica
   if (threadIdx.x == 0) {
     const int done = atomicAdd(p.state + 1, 1);

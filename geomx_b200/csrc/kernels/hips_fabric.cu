@@ -28,18 +28,8 @@ namespace gx {
 // Global-owner side of one tile: optimizer + broadcast + per-key completion/flag.  `agg` is this thread's float4 of the summed gradient.
 __device__ __forceinline__ void global_apply_tile(const FabricParams& p, int t, float4 agg, uint32_t epoch, float lr_t) {
   const long long off = (long long)t * TILE + threadIdx.x * 4;
-  float lr = lr_t, wd = p.h.wd;
-  if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
-  float4 W = *reinterpret_cast<float4*>(p.w + off);
-  float4 A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
-  float4 B = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
-  opt_apply(W.x, agg.x, A.x, B.x, p.h, lr, wd);
-  opt_apply(W.y, agg.y, A.y, B.y, p.h, lr, wd);
-  opt_apply(W.z, agg.z, A.z, B.z, p.h, lr, wd);
-  opt_apply(W.w, agg.w, A.w, B.w, p.h, lr, wd);
-  *reinterpret_cast<float4*>(p.w + off) = W;
-  if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = A;
-  if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = B;
+  TileState s = tile_state_load(p, t, off, lr_t);
+  const float4 W = tile_state_apply(p, off, s, agg);
   if (p.world == 1) {  // degenerate single-rank HiPS: the arena optimizer, no cross-GPU traffic, flags or fences
     *reinterpret_cast<float4*>(p.param[0] + off) = W;
     return;
@@ -88,20 +78,9 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
       const long long off = (long long)t * TILE + threadIdx.x * 4;
       float* g = p.grad[0] + off;
       const float4 G = *reinterpret_cast<const float4*>(g);
-      float4 W = *reinterpret_cast<float4*>(p.w + off);
-      float4 A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
-      float4 B = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
-      float lr = lr_t, wd = p.h.wd;
-      if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
-      const float4 agg = f4_scale(G, p.push_scale);
-      opt_apply(W.x, agg.x, A.x, B.x, p.h, lr, wd);
-      opt_apply(W.y, agg.y, A.y, B.y, p.h, lr, wd);
-      opt_apply(W.z, agg.z, A.z, B.z, p.h, lr, wd);
-      opt_apply(W.w, agg.w, A.w, B.w, p.h, lr, wd);
+      TileState s = tile_state_load(p, t, off, lr_t);
+      const float4 W = tile_state_apply(p, off, s, f4_scale(G, p.push_scale));
       if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
-      *reinterpret_cast<float4*>(p.w + off) = W;
-      if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = A;
-      if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = B;
       *reinterpret_cast<float4*>(p.param[0] + off) = W;
     }
     if (threadIdx.x == 0) {
@@ -272,8 +251,6 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
   const long long n2 = 2 * p.n;
   const int K = p.bsc_k;
   int* err = p.state + 5;
-  auto fmt_of = [&](int t) -> int { return p.tile_fmt ? (int)p.tile_fmt[t] : FMT_F32; };
-  auto grad_fmt = [](int f) -> int { return (f == FMT_F16 || f == FMT_F8) ? f : FMT_F32; };     // Bi-Sparse tiles travel dense inside a party
 
   // ---- phase 1: push my gradient tiles to their party owners (tiles I own myself are read in place in phase 2).  Inside a party the
   //      transport is dense (reference: worker -> local server is never sparsified), fp16 tiles travel as halves.
@@ -285,7 +262,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
     float* g = p.grad[p.rank] + off;
     const float4 v = *reinterpret_cast<const float4*>(g);
     if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
-    ll_send_dense(p.ll_a[party_base + t % S] + (long long)p.local * n2 + 2 * off, v, grad_fmt(fmt_of(t)), epoch);
+    ll_send_dense(p.ll_a[party_base + t % S] + (long long)p.local * n2 + 2 * off, v, grad_fmt(fmt_of(p, t)), epoch);
   }
   stamp(1);
   // ---- phase 2: LOCAL PS TIER: the party owner sums the party's gradients of its tiles and forwards the aggregate to the global owner
@@ -293,7 +270,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
     const int t = p.tile_order ? p.tile_order[ti] : ti;   // DGT: important tiles first
     if (t % S != p.local) continue;
     if (p.tile_active != nullptr && !p.tile_active[t]) continue;
-    const int fmt = fmt_of(t);
+    const int fmt = fmt_of(p, t);
     const long long off = (long long)t * TILE + threadIdx.x * 4;
     float* g = p.grad[p.rank] + off;
     float4 acc = *reinterpret_cast<const float4*>(g);
@@ -350,13 +327,9 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
     const int t = p.tile_order ? p.tile_order[ti] : ti;   // DGT: important tiles first
     if (owner_of(t) != p.rank) continue;
     if (p.tile_active != nullptr && !p.tile_active[t]) continue;
-    const int fmt = fmt_of(t);
+    const int fmt = fmt_of(p, t);
     const long long off = (long long)t * TILE + threadIdx.x * 4;
-    float lr = lr_t, wd = p.h.wd;
-    if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
-    float4 W = *reinterpret_cast<float4*>(p.w + off);   // issued before the poll: the state loads overlap the wait
-    float4 A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
-    float4 B = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
+    TileState s = tile_state_load(p, t, off, lr_t);   // issued before the poll: the state loads overlap the wait
     float4 agg;
     if (fmt != FMT_BSC) {
       agg = ll_recv_dense(p.ll_b[p.rank] + 2 * off, fmt, epoch, err);
@@ -374,30 +347,8 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
       __syncthreads();
       agg = *reinterpret_cast<const float4*>(s_tile + threadIdx.x * 4);
     }
-    if (p.dgt_contrib != nullptr) {
-      // DGT contribution of this tile (kv_app.h:853-876 EvalMsgContribution): EMA of the mean |aggregated gradient| — ranks the tiles for the
-      // next re-ordering (important first) and decides which tiles keep full precision (HipsFabric.dgt_rerank)
-      float a = fabsf(agg.x) + fabsf(agg.y) + fabsf(agg.z) + fabsf(agg.w);
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
-      __syncthreads();
-      if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = a;
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        float sum = 0.f;
-#pragma unroll
-        for (int i = 0; i < FAB_THREADS / 32; ++i) sum += s_red[i];
-        const float mean = sum * (1.f / TILE), old = p.dgt_contrib[t];
-        p.dgt_contrib[t] = old == 0.f ? mean : p.dgt_alpha * old + (1.f - p.dgt_alpha) * mean;
-      }
-    }
-    opt_apply(W.x, agg.x, A.x, B.x, p.h, lr, wd);
-    opt_apply(W.y, agg.y, A.y, B.y, p.h, lr, wd);
-    opt_apply(W.z, agg.z, A.z, B.z, p.h, lr, wd);
-    opt_apply(W.w, agg.w, A.w, B.w, p.h, lr, wd);
-    *reinterpret_cast<float4*>(p.w + off) = W;
-    if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = A;
-    if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = B;
+    if (p.dgt_contrib != nullptr) dgt_update_contrib(p, t, agg, s_red);
+    const float4 W = tile_state_apply(p, off, s, agg);
     if (fmt == FMT_BSC && p.h.kind < 0) {
       // BSCPullCompress (:271-308): the aggregated gradient goes back sparse — its non-zeros in index order, at most P*K of them
       const float ww[4] = {W.x, W.y, W.z, W.w};
@@ -430,7 +381,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
   for (int ti = blockIdx.x; ti < p.tiles; ti += gridDim.x) {
     const int t = p.tile_order ? p.tile_order[ti] : ti;   // DGT: important tiles first
     if (p.tile_active != nullptr && !p.tile_active[t]) continue;
-    const int fmt = fmt_of(t);
+    const int fmt = fmt_of(p, t);
     const long long off = (long long)t * TILE + threadIdx.x * 4;
     if (fmt == FMT_BSC && p.h.kind < 0) {   // BSCDecompress on the worker side: zero + scatter
       __syncthreads();
@@ -507,11 +458,8 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
   const uint32_t epoch = (round << 3) | (uint32_t)(p.channel_id & 7);
   const int opt_t = (*reinterpret_cast<volatile int*>(p.state + 2)) + 1;
   const float lr_t = adam_lr(p.h, opt_t);
-  const int S = p.party_size, P = p.num_parties;
-  const long long n2 = 2 * p.n;
   const bool rep = p.direct_replicate != 0;
   int* err = p.state + 5;
-  auto fmt_of = [&](int t) -> int { const int f = p.tile_fmt ? (int)p.tile_fmt[t] : FMT_F32; return (f == FMT_F16 || f == FMT_F8) ? f : FMT_F32; };
 
   // ---- phase 1: push my gradient tiles to the rank(s) that apply them (my own slot included: the reducer reads all slots the same way)
   for (int ti = blockIdx.x; ti < p.tiles; ti += gridDim.x) {
@@ -521,11 +469,9 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
     float* g = p.grad[p.rank] + off;
     const float4 v = *reinterpret_cast<const float4*>(g);
     if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
-    const long long slot = (long long)p.rank * n2 + 2 * off;
-    const int f = fmt_of(t);
-    if (!rep) ll_send_dense(p.ll_d[p.tile_owner[t]] + slot, v, f, epoch);
-    else if (p.ll_d_mc != nullptr) ll_send_dense_mc(p.ll_d_mc + slot, v, f, epoch);
-    else for (int r = 0; r < p.world; ++r) ll_send_dense(p.ll_d[r] + slot, v, f, epoch);
+    const int f = grad_fmt(fmt_of(p, t));
+    if (rep) direct_send_all(p, off, v, f, epoch);
+    else ll_send_dense(p.ll_d[p.tile_owner[t]] + (long long)p.rank * 2 * p.n + 2 * off, v, f, epoch);
   }
   stamp(1);
   // ---- phase 2: both server tiers on the applying rank: party sums, scale, sum over parties, optimizer
@@ -533,43 +479,12 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
     const int t = p.tile_order ? p.tile_order[ti] : ti;
     if (p.tile_active != nullptr && !p.tile_active[t]) continue;
     if (!rep && p.tile_owner[t] != p.rank) continue;
-    const int f = fmt_of(t);
+    const int f = grad_fmt(fmt_of(p, t));
     const long long off = (long long)t * TILE + threadIdx.x * 4;
-    float lr = lr_t, wd = p.h.wd;
-    if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
-    float4 W = *reinterpret_cast<float4*>(p.w + off);   // issued before the polls: the state loads overlap the wait
-    float4 A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
-    float4 B = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
-    const float* in = p.ll_d[p.rank] + 2 * off;
-    float4 agg = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int g = 0; g < P; ++g) {
-      float4 ps = ll_recv_dense(in + (long long)(g * S) * n2, f, epoch, err);
-      for (int j = 1; j < S; ++j) ps = f4_add(ps, ll_recv_dense(in + (long long)(g * S + j) * n2, f, epoch, err));
-      ps = f4_scale(ps, p.push_scale);
-      agg = g == 0 ? ps : f4_add(agg, ps);
-    }
-    if (p.dgt_contrib != nullptr && (!rep || p.tile_owner[t] == p.rank)) {   // DGT contribution EMA (kv_app.h:853-876), as in the LL kernel
-      float a = fabsf(agg.x) + fabsf(agg.y) + fabsf(agg.z) + fabsf(agg.w);
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
-      __syncthreads();
-      if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = a;
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        float sum = 0.f;
-#pragma unroll
-        for (int i = 0; i < FAB_THREADS / 32; ++i) sum += s_red[i];
-        const float mean = sum * (1.f / TILE), old = p.dgt_contrib[t];
-        p.dgt_contrib[t] = old == 0.f ? mean : p.dgt_alpha * old + (1.f - p.dgt_alpha) * mean;
-      }
-    }
-    opt_apply(W.x, agg.x, A.x, B.x, p.h, lr, wd);
-    opt_apply(W.y, agg.y, A.y, B.y, p.h, lr, wd);
-    opt_apply(W.z, agg.z, A.z, B.z, p.h, lr, wd);
-    opt_apply(W.w, agg.w, A.w, B.w, p.h, lr, wd);
-    *reinterpret_cast<float4*>(p.w + off) = W;
-    if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = A;
-    if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = B;
+    TileState s = tile_state_load(p, t, off, lr_t);   // issued before the polls: the state loads overlap the wait
+    const float4 agg = direct_recv_sum(p, off, f, epoch, err);
+    if (p.dgt_contrib != nullptr && (!rep || p.tile_owner[t] == p.rank)) dgt_update_contrib(p, t, agg, s_red);
+    const float4 W = tile_state_apply(p, off, s, agg);
     if (rep) {
       *reinterpret_cast<float4*>(p.param[p.rank] + off) = W;   // the pull is a local store: every rank holds the fresh replica
     } else {
@@ -585,7 +500,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
       const int t = p.tile_order ? p.tile_order[ti] : ti;
       if (p.tile_active != nullptr && !p.tile_active[t]) continue;
       const long long off = (long long)t * TILE + threadIdx.x * 4;
-      const int bf = fmt_of(t) == FMT_F32 ? FMT_F32 : FMT_F16;
+      const int bf = grad_fmt(fmt_of(p, t)) == FMT_F32 ? FMT_F32 : FMT_F16;
       *reinterpret_cast<float4*>(p.param[p.rank] + off) = ll_recv_dense(p.ll_e[p.rank] + 2 * off, bf, epoch, err);
     }
   }
@@ -648,10 +563,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_async_step_kernel(const F
     float4 W = ld_f4_sys(wp);
     float4 A = s0_peer[owner] ? ld_f4_sys(s0_peer[owner] + off) : make_float4(0, 0, 0, 0);
     float4 B = s1_peer[owner] ? ld_f4_sys(s1_peer[owner] + off) : make_float4(0, 0, 0, 0);
-    opt_apply(W.x, acc.x, A.x, B.x, p.h, lr, wd);
-    opt_apply(W.y, acc.y, A.y, B.y, p.h, lr, wd);
-    opt_apply(W.z, acc.z, A.z, B.z, p.h, lr, wd);
-    opt_apply(W.w, acc.w, A.w, B.w, p.h, lr, wd);
+    opt_apply4(W, acc, A, B, p.h, lr, wd);
     st_f4_sys(wp, W);
     if (s0_peer[owner]) st_f4_sys(s0_peer[owner] + off, A);
     if (s1_peer[owner]) st_f4_sys(s1_peer[owner] + off, B);

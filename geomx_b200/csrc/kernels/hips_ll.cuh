@@ -1,10 +1,10 @@
-// Shared device-side pieces of the HiPS fabric kernels: the launch parameter block, the optimizer step and the LL ("low latency") packet
-// protocol.  Included by hips_fabric.cu (the exchange kernels) and by cnn_direct.cu (the convolution backward kernel whose tail performs the
-// conv keys' exchange itself).
+// Shared device-side pieces of the HiPS fabric kernels: the launch parameter block, the per-tile server update, the LL ("low latency") packet
+// protocol and the replicated direct-protocol exchange of one tile.  Included by hips_fabric.cu (the exchange kernels) and by cnn_direct.cu
+// (the convolution backward kernel whose tail performs the conv keys' exchange itself).  The optimizer rules are in optim.cuh.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
-#include "common.cuh"
+#include "optim.cuh"
 
 namespace gx {
 
@@ -12,11 +12,6 @@ constexpr int MAX_RANKS = 16;
 constexpr int TILE = 1024;           // floats per tile (= 4 KiB = one 256-thread float4 sweep)
 constexpr int FAB_THREADS = 256;
 
-
-struct OptHyperF {
-  float lr, wd, rescale, clip, momentum, beta1, beta2, eps, lamda;
-  int kind;  // 0 sgd, 1 adam, 2 dcasgd, -1 none (store aggregated gradient: Bi-Sparse / local-optimizer modes)
-};
 
 struct FabricParams {
   int world, rank, party_size, num_parties, party, local;
@@ -42,7 +37,7 @@ struct FabricParams {
   const float2* tile_mult;     // per-tile (lr_mult, wd_mult) or nullptr
   int* key_done;               // [num_keys] cumulative completion counters on this rank (global owner side)
   int* state;                  // [0]=epoch completed, [1]=CTA completion counter, [2]=optimizer step t
-  OptHyperF h;
+  OptHyper h;
   float push_scale;            // the script-level  grad / num_samples
   int defer_pull_wait;
   int param_ready_off;         // uint32 offset of param_ready[num_keys] in the flag pad
@@ -80,37 +75,46 @@ __device__ __forceinline__ void wait_flag_ge(const uint32_t* p, uint32_t v) {
 __device__ __forceinline__ float4 f4_add(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
 __device__ __forceinline__ float4 f4_scale(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
 
-__device__ __forceinline__ void opt_apply(float& w, float g, float& a, float& b, const OptHyperF& h, float lr, float wd) {
-  if (h.kind == 1) {
-    g = fmaf(wd, w, g * h.rescale);            // adam_update: the regularised gradient is what gets clipped (optimizer_op-inl.h:840-873)
-    if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-    a = h.beta1 * a + (1.f - h.beta1) * g;
-    b = h.beta2 * b + (1.f - h.beta2) * g * g;
-    w -= lr * a / (sqrtf(b) + h.eps);
-  } else if (h.kind == 0) {
-    g *= h.rescale;
-    if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-    g = fmaf(wd, w, g);
-    if (h.momentum != 0.f) { a = h.momentum * a - lr * g; w += a; }
-    else w -= lr * g;
-  } else if (h.kind == 2) {
-    g *= h.rescale;
-    if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-    const float upd = g + wd * w + h.lamda * g * g * (w - b);
-    const float prev = w;
-    if (h.momentum != 0.f) { a = h.momentum * a - lr * upd; w += a; }
-    else w -= lr * upd;
-    b = prev;
-  } else {
-    w = g;  // no optimizer on the server: store the aggregate (reference ApplyUpdates without updater_, :547-550)
+// ---- per-tile server update, in two steps so that callers can issue the state loads before they wait for the aggregate
+struct TileState {
+  float4 W, A, B;    // master weights and optimizer state of this thread's float4 of the tile
+  float lr, wd;      // after the tile's (lr_mult, wd_mult)
+};
+__device__ __forceinline__ TileState tile_state_load(const FabricParams& p, int t, long long off, float lr_t) {
+  TileState s;
+  s.lr = lr_t; s.wd = p.h.wd;
+  if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); s.lr *= mm.x; s.wd *= mm.y; }
+  s.W = *reinterpret_cast<float4*>(p.w + off);
+  s.A = p.s0 ? *reinterpret_cast<float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
+  s.B = p.s1 ? *reinterpret_cast<float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
+  return s;
+}
+// optimizer step on `agg`, state stored back; returns the fresh weights
+__device__ __forceinline__ float4 tile_state_apply(const FabricParams& p, long long off, TileState& s, float4 agg) {
+  opt_apply4(s.W, agg, s.A, s.B, p.h, s.lr, s.wd);
+  *reinterpret_cast<float4*>(p.w + off) = s.W;
+  if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = s.A;
+  if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = s.B;
+  return s.W;
+}
+
+// DGT contribution of tile t (kv_app.h:853-876 EvalMsgContribution): EMA of the mean |aggregated gradient| — ranks the tiles for the next
+// re-ordering (important first) and decides which tiles keep full precision (HipsFabric.dgt_rerank).  All FAB_THREADS threads call it.
+__device__ __forceinline__ void dgt_update_contrib(const FabricParams& p, int t, float4 agg, float* s_red) {
+  float a = fabsf(agg.x) + fabsf(agg.y) + fabsf(agg.z) + fabsf(agg.w);
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) a += __shfl_xor_sync(0xffffffffu, a, d);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = a;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < FAB_THREADS / 32; ++i) sum += s_red[i];
+    const float mean = sum * (1.f / TILE), old = p.dgt_contrib[t];
+    p.dgt_contrib[t] = old == 0.f ? mean : p.dgt_alpha * old + (1.f - p.dgt_alpha) * mean;
   }
 }
-
-__device__ __forceinline__ float adam_lr(const OptHyperF& h, int t) {
-  if (h.kind != 1) return h.lr;
-  return h.lr * sqrtf(1.f - powf(h.beta2, (float)t)) / (1.f - powf(h.beta1, (float)t));
-}
-
 
 // ------------------------------------------------------------------------------------------------------------------ LL protocol
 // The flag protocol above costs one fence.acq_rel.sys per hand-off and tools/fabric_probe.py measures 2.4-7 us for each of them on
@@ -175,6 +179,9 @@ constexpr int FMT_F16 = 1;   // {h0h1,e,h2h3,e}: half the bytes on every hop (gr
 constexpr int FMT_BSC = 2;   // Bi-Sparse between the tiers: k {value, e, index, e} packets per tile instead of 1024 values
 constexpr int FMT_F8 = 3;    // block-scaled fp8 gradients: e4m3 with one fp32 scale per 128 values (a warp), 8 values per packet => 1/4 of the
                              // fp32 bytes on the two gradient hops; parameters of such tiles return as fp16
+__device__ __forceinline__ int fmt_of(const FabricParams& p, int t) { return p.tile_fmt ? (int)p.tile_fmt[t] : FMT_F32; }
+// format of a tile's dense gradient packets: Bi-Sparse tiles travel as fp32 wherever their gradients go dense
+__device__ __forceinline__ int grad_fmt(int f) { return (f == FMT_F16 || f == FMT_F8) ? f : FMT_F32; }
 
 // ---- block-scaled fp8 (warp-collective: all 32 lanes of a warp call these together; a lane owns 4 consecutive values)
 __device__ __forceinline__ uint32_t pack_f8x4(float4 v, float inv) {
@@ -230,6 +237,28 @@ __device__ __forceinline__ float4 ll_recv_dense(const float* src, int fmt, uint3
     return make_float4(a.x, a.y, b.x, b.y);
   }
   return ll_load(src, epoch, err);
+}
+
+// ------------------------------------------------------------------------------------------------------------------ direct protocol
+// replicated mode: this rank's gradient float4 `v` at arena offset `off` into its own slot on every rank (one multicast store, or one per rank)
+__device__ __forceinline__ void direct_send_all(const FabricParams& p, long long off, float4 v, int f, uint32_t epoch) {
+  const long long slot = (long long)p.rank * 2 * p.n + 2 * off;
+  if (p.ll_d_mc != nullptr) ll_send_dense_mc(p.ll_d_mc + slot, v, f, epoch);
+  else for (int r = 0; r < p.world; ++r) ll_send_dense(p.ll_d[r] + slot, v, f, epoch);
+}
+// the aggregate of every rank's packets at `off`, summed in the hierarchy's order: inside each party, push_scale, then across parties
+__device__ __forceinline__ float4 direct_recv_sum(const FabricParams& p, long long off, int f, uint32_t epoch, int* err) {
+  const int S = p.party_size;
+  const long long n2 = 2 * p.n;
+  const float* in = p.ll_d[p.rank] + 2 * off;
+  float4 agg = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int g = 0; g < p.num_parties; ++g) {
+    float4 ps = ll_recv_dense(in + (long long)(g * S) * n2, f, epoch, err);
+    for (int j = 1; j < S; ++j) ps = f4_add(ps, ll_recv_dense(in + (long long)(g * S + j) * n2, f, epoch, err));
+    ps = f4_scale(ps, p.push_scale);
+    agg = g == 0 ? ps : f4_add(agg, ps);
+  }
+  return agg;
 }
 
 }  // namespace gx

@@ -8,54 +8,15 @@
 //     Per-key lr/wd multipliers come from a per-tile table (tile = 1024 floats; keys are tile-aligned in the arena).
 //   * multi_tensor_* : one launch over a pointer table (Trainer path for tensors that do not live in an arena).
 //   * n-ary sum (CommDevice reduce), scale+cast (the script-level `grad / num_samples` and `.astype('float16')`).
+// The update rules themselves (OptHyper, opt_elem / opt_apply, adam_lr) are in optim.cuh, shared with the HiPS fabric kernels.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
-#include "common.cuh"
+#include "optim.cuh"
 
 namespace gx {
 
-enum OptKind { OPT_SGD = 0, OPT_ADAM = 1, OPT_DCASGD = 2 };
-
-struct OptHyper {
-  float lr, wd, rescale, clip;      // clip < 0 -> off
-  float momentum;                   // sgd / dcasgd
-  float beta1, beta2, eps;          // adam
-  float lamda;                      // dcasgd
-};
-
 constexpr int ARENA_TILE = 1024;
-
-__device__ __forceinline__ float prep_grad(float g, float w, const OptHyper& h, float wd) {
-  g *= h.rescale;
-  if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-  return fmaf(wd, w, g);
-}
-
-// one element of each optimizer (s0/s1 = state slots: sgd: s0=mom; adam: s0=m, s1=v; dcasgd: s0=mom, s1=prev_weight)
-template <int KIND>
-__device__ __forceinline__ void opt_elem(float& w, float g, float& s0, float& s1, const OptHyper& h, float lr, float wd) {
-  if (KIND == OPT_SGD) {
-    g = prep_grad(g, w, h, wd);
-    if (h.momentum != 0.f) { s0 = h.momentum * s0 - lr * g; w += s0; }
-    else w -= lr * g;
-  } else if (KIND == OPT_ADAM) {
-    // adam_update clips the REGULARISED gradient: rescale, + wd*w, then clip (src/operator/optimizer_op-inl.h:840-873)
-    g = fmaf(wd, w, g * h.rescale);
-    if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-    s0 = h.beta1 * s0 + (1.f - h.beta1) * g;
-    s1 = h.beta2 * s1 + (1.f - h.beta2) * g * g;
-    w -= lr * s0 / (sqrtf(s1) + h.eps);
-  } else {
-    g *= h.rescale;
-    if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
-    const float upd = g + wd * w + h.lamda * g * g * (w - s1);
-    const float prev = w;
-    if (h.momentum != 0.f) { s0 = h.momentum * s0 - lr * upd; w += s0; }
-    else w -= lr * upd;
-    s1 = prev;
-  }
-}
 
 // step_state[0] = number of completed updates t, step_state[1] = CTA completion counter (self-resetting)
 template <int KIND>
@@ -64,9 +25,9 @@ __global__ void __launch_bounds__(256) arena_opt_kernel(float* __restrict__ w, c
                                                          float* __restrict__ g_zero) {
   gx::pdl_wait();
   gx::pdl_launch();
+  h.kind = KIND;  // a compile-time kind: adam_lr and opt_apply4 reduce to this kernel's rule
   const int t = step_state ? (*reinterpret_cast<volatile int*>(step_state)) + 1 : 1;
-  float lr_t = h.lr;
-  if (KIND == OPT_ADAM) lr_t = h.lr * sqrtf(1.f - powf(h.beta2, (float)t)) / (1.f - powf(h.beta1, (float)t));
+  const float lr_t = adam_lr(h, t);
   const long long n4 = n >> 2;  // arenas are tile-padded, n % 1024 == 0
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float lr = lr_t, wd = h.wd;
@@ -75,10 +36,7 @@ __global__ void __launch_bounds__(256) arena_opt_kernel(float* __restrict__ w, c
     const float4 G = reinterpret_cast<const float4*>(g)[i];
     float4 A = s0 ? reinterpret_cast<float4*>(s0)[i] : make_float4(0, 0, 0, 0);
     float4 Bv = s1 ? reinterpret_cast<float4*>(s1)[i] : make_float4(0, 0, 0, 0);
-    opt_elem<KIND>(W.x, G.x, A.x, Bv.x, h, lr, wd);
-    opt_elem<KIND>(W.y, G.y, A.y, Bv.y, h, lr, wd);
-    opt_elem<KIND>(W.z, G.z, A.z, Bv.z, h, lr, wd);
-    opt_elem<KIND>(W.w, G.w, A.w, Bv.w, h, lr, wd);
+    opt_apply4(W, G, A, Bv, h, lr, wd);
     reinterpret_cast<float4*>(w)[i] = W;
     if (s0) reinterpret_cast<float4*>(s0)[i] = A;
     if (s1) reinterpret_cast<float4*>(s1)[i] = Bv;
@@ -169,8 +127,9 @@ static inline int grid_for(long long n, int per_thread = 1) {
 
 using namespace gx;
 
-static OptHyper mk(float lr, float wd, float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda) {
+static OptHyper mk(int kind, float lr, float wd, float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda) {
   OptHyper h; h.lr = lr; h.wd = wd; h.rescale = rescale; h.clip = clip; h.momentum = momentum; h.beta1 = b1; h.beta2 = b2; h.eps = eps; h.lamda = lamda;
+  h.kind = kind;
   return h;
 }
 
@@ -178,7 +137,7 @@ static OptHyper mk(float lr, float wd, float rescale, float clip, float momentum
 GX_API int gx_arena_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, const void* tile_mult, float lr, float wd,
                         float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda, int* step_state, float* g_zero,
                         cudaStream_t s) {
-  const OptHyper h = mk(lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+  const OptHyper h = mk(kind, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
   const int grid = grid_for(n, 4);
   const float2* tm = reinterpret_cast<const float2*>(tile_mult);
   if (kind == OPT_SGD) launch_pdl(arena_opt_kernel<OPT_SGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, step_state, g_zero);
@@ -189,7 +148,7 @@ GX_API int gx_arena_opt(int kind, float* w, const float* g, float* s0, float* s1
 
 GX_API int gx_multi_tensor_opt(int kind, const void* table, int num_tensors, long long max_n, float lr_t, float wd, float rescale, float clip,
                                float momentum, float b1, float b2, float eps, float lamda, cudaStream_t s) {
-  const OptHyper h = mk(lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+  const OptHyper h = mk(kind, lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
   int gx_ = grid_for(max_n); if (gx_ > 64) gx_ = 64;
   dim3 grid(gx_, num_tensors);
   const TensorEntry* t = reinterpret_cast<const TensorEntry*>(table);
@@ -201,7 +160,7 @@ GX_API int gx_multi_tensor_opt(int kind, const void* table, int num_tensors, lon
 
 GX_API int gx_single_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, float lr_t, float wd, float rescale, float clip,
                          float momentum, float b1, float b2, float eps, float lamda, cudaStream_t s) {
-  const OptHyper h = mk(lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+  const OptHyper h = mk(kind, lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
   const int grid = grid_for(n);
   if (kind == OPT_SGD) launch_pdl(single_opt_kernel<OPT_SGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t);
   else if (kind == OPT_ADAM) launch_pdl(single_opt_kernel<OPT_ADAM>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t);

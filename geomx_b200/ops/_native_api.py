@@ -413,16 +413,17 @@ def head_fwd_bwd(a, W, bias, label, loss, logits, dW, db, da, dbias_prev, relu_m
 
 
 # --------------------------------------------------------------------------------------------------------------- optimizers
-_KIND = {"sgd": 0, "adam": 1, "dcasgd": 2}
+# optimizer kind codes of the kernels (OptKind in csrc/kernels/optim.cuh)
+OPT_KIND = {"sgd": 0, "adam": 1, "dcasgd": 2}
 
 
 def arena_opt(kind, w, g, s0, s1, n, tile_mult, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda, step_state, g_zero=None):
-    _ck(_lib().gx_arena_opt(_KIND[kind], _p(w), _p(g), _p(s0), _p(s1), n, _p(tile_mult), lr, wd, rescale, clip, momentum, b1, b2, eps,
+    _ck(_lib().gx_arena_opt(OPT_KIND[kind], _p(w), _p(g), _p(s0), _p(s1), n, _p(tile_mult), lr, wd, rescale, clip, momentum, b1, b2, eps,
                             lamda, _p(step_state), _p(g_zero), _s()), "arena_opt")
 
 
 def single_opt(kind, w, g, s0, s1, lr_t, wd, rescale, clip, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8, lamda=0.04):
-    _ck(_lib().gx_single_opt(_KIND[kind], _p(w), _p(g), _p(s0), _p(s1), w.numel(), lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda, _s()),
+    _ck(_lib().gx_single_opt(OPT_KIND[kind], _p(w), _p(g), _p(s0), _p(s1), w.numel(), lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda, _s()),
         "single_opt")
 
 
@@ -477,7 +478,7 @@ def multi_tensor_update(optimizer, updater, idxs, ws, gs):
         _mt_cache[key] = ent
     dev, max_n, cnt = ent
     clip = -1.0 if optimizer.clip_gradient is None else float(optimizer.clip_gradient)
-    _ck(_lib().gx_multi_tensor_opt(_KIND[kind], _p(dev), cnt, max_n, lr_t, float(optimizer.wd), float(optimizer.rescale_grad), clip,
+    _ck(_lib().gx_multi_tensor_opt(OPT_KIND[kind], _p(dev), cnt, max_n, lr_t, float(optimizer.wd), float(optimizer.rescale_grad), clip,
                                    float(spec.get("momentum", 0.0)), float(spec.get("beta1", 0.9)), float(spec.get("beta2", 0.999)),
                                    float(spec.get("epsilon", 1e-8)), float(spec.get("lamda", 0.04)), _s()), "multi_tensor_opt")
     return True

@@ -19,6 +19,7 @@ import torch
 
 from ..base import MXNetError, getenv_int
 from ..ops import native
+from ..ops._native_api import OPT_KIND
 from .arena import ArenaLayout
 
 MAX_RANKS = 16
@@ -200,7 +201,7 @@ class _FabricParams(ctypes.Structure):
     ]
 
 
-_KIND = {"sgd": 0, "adam": 1, "dcasgd": 2, None: -1, "none": -1}
+_KIND = {**OPT_KIND, None: -1, "none": -1}   # -1: no server optimizer, the kernels store the aggregated gradient
 
 
 def dgt_num_important(sorted_contrib, k, adaptive=False, k_min=0.2):
