@@ -53,6 +53,7 @@ __device__ __forceinline__ void global_apply_tile(const FabricParams& p, int t, 
   }
 }
 
+template <bool SCHED>
 __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const FabricParams p) {
   gx::pdl_wait();
   gx::pdl_launch();
@@ -63,7 +64,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
   const uint32_t epoch = (uint32_t)(*reinterpret_cast<volatile int*>(p.state)) + 1u;
   const int opt_t = (*reinterpret_cast<volatile int*>(p.state + 2)) + 1;
   __shared__ float s_lr;
-  if (threadIdx.x == 0) s_lr = adam_lr(p.h, opt_t);
+  if (threadIdx.x == 0) s_lr = step_lr<SCHED>(p.h, opt_t);
   __syncthreads();
   const float lr_t = s_lr;
   const int S = p.party_size, P = p.num_parties;
@@ -228,6 +229,7 @@ __device__ __forceinline__ uint32_t block_kth_largest(const uint32_t (&a)[4], in
   return prefix;
 }
 
+template <bool SCHED>
 __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const FabricParams p) {
   gx::pdl_wait();
   gx::pdl_launch();
@@ -241,7 +243,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
   __shared__ float s_red[FAB_THREADS / 32];
   const uint32_t epoch = (uint32_t)(*reinterpret_cast<volatile int*>(p.state)) + 1u;
   const int opt_t = (*reinterpret_cast<volatile int*>(p.state + 2)) + 1;
-  const float lr_t = adam_lr(p.h, opt_t);
+  const float lr_t = step_lr<SCHED>(p.h, opt_t);
   const int S = p.party_size, P = p.ll_party_mode ? 1 : p.num_parties;
   const int party_base = p.party * S;
   const int slot = p.ll_party_mode ? 0 : p.party;                       // this party's packet slot on a global owner
@@ -425,6 +427,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
 // sharded channel runs on a side stream underneath the convolution backward pass; the conv keys' replicated channel is the only exposed
 // communication).  Reference for the ordering idea: per-key push with priority = -index (examples/cnn.py:121-125, kvstore_dist.h:565-625).
 // Every channel owns its state block (epoch, CTA counter, optimizer step) and stamps its id into the packet epoch.
+template <bool SCHED>
 __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const FabricParams p) {
   // Before the grid dependency resolves (i.e. while the kernel that produces the gradients is still running): walk this CTA's tiles once and
   // pull everything that does NOT depend on that kernel towards L2 — the tile metadata, the optimizer state and master weights of the tiles
@@ -457,7 +460,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
   const uint32_t round = (uint32_t)(*reinterpret_cast<volatile int*>(p.state)) + 1u;
   const uint32_t epoch = (round << 3) | (uint32_t)(p.channel_id & 7);
   const int opt_t = (*reinterpret_cast<volatile int*>(p.state + 2)) + 1;
-  const float lr_t = adam_lr(p.h, opt_t);
+  const float lr_t = step_lr<SCHED>(p.h, opt_t);
   const bool rep = p.direct_replicate != 0;
   int* err = p.state + 5;
 
@@ -518,6 +521,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
 
 // One-sided MixedSync: the party's tile owner applies its aggregate directly on the global owner's HBM under a per-tile lock.
 // locks live in the global owner's flag pad at `lock_off` (uint32 per tile), per-tile optimizer step counts right after them.
+template <bool SCHED>
 __global__ void __launch_bounds__(FAB_THREADS, 1) hips_async_step_kernel(const FabricParams p, float* const* w_peer, float* const* s0_peer,
                                                                           float* const* s1_peer, int lock_off, int step_off) {
   gx::pdl_wait();
@@ -557,7 +561,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_async_step_kernel(const F
       s_step = (int)ld_relaxed_sys(stepc) + 1;
     }
     __syncthreads();
-    float lr = adam_lr(p.h, s_step), wd = p.h.wd;
+    float lr = step_lr<SCHED>(p.h, s_step), wd = p.h.wd;
     if (p.tile_mult) { const float2 mm = __ldg(p.tile_mult + t); lr *= mm.x; wd *= mm.y; }
     float* wp = w_peer[owner] + off;
     float4 W = ld_f4_sys(wp);
@@ -705,35 +709,40 @@ GX_API int gx_fabric_params_size() { return (int)sizeof(FabricParams); }
 GX_API int gx_hips_fsa_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(hips_fsa_step_kernel, dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_step_kernel<true> : hips_fsa_step_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
 // Largest co-resident grid of the fused kernels (they spin on each other: every CTA of a launch must be resident).
 GX_API int gx_hips_max_grid() {
-  int dev = 0, sms = 0, occ_a = 0, occ_b = 0;
+  int dev = 0, sms = 0, occ = 1 << 30;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_a, hips_fsa_ll_kernel, FAB_THREADS, 0);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_b, hips_fsa_step_kernel, FAB_THREADS, 0);
-  const int occ = occ_a < occ_b ? occ_a : occ_b;
+  for (const void* k : {(const void*)hips_fsa_ll_kernel<false>, (const void*)hips_fsa_ll_kernel<true>, (const void*)hips_fsa_step_kernel<false>,
+                        (const void*)hips_fsa_step_kernel<true>}) {   // both instances of each: constant and scheduled lr
+    int o = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k, FAB_THREADS, 0);
+    occ = o < occ ? o : occ;
+  }
   return sms * (occ < 1 ? 1 : (occ > 2 ? 2 : occ));
 }
 GX_API int gx_hips_fsa_ll_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(hips_fsa_ll_kernel, dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_ll_kernel<true> : hips_fsa_ll_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_hips_fsa_direct_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(hips_fsa_direct_kernel, dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_direct_kernel<true> : hips_fsa_direct_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s,
+             p);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_hips_async_step(const void* params, float* const* w_peer, float* const* s0_peer, float* const* s1_peer, int lock_off, int step_off,
                               int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
-  launch_pdl(hips_async_step_kernel, dim3(grid), dim3(FAB_THREADS), 0, s, p, w_peer, s0_peer, s1_peer, lock_off, step_off);
+  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_async_step_kernel<true> : hips_async_step_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p,
+             w_peer, s0_peer, s1_peer, lock_off, step_off);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_hips_party_allreduce(const void* params, float* const* src_peer, float* const* dst_peer, float scale, int mode, int flag_off, int grid,

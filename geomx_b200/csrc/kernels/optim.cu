@@ -8,7 +8,7 @@
 //     Per-key lr/wd multipliers come from a per-tile table (tile = 1024 floats; keys are tile-aligned in the arena).
 //   * multi_tensor_* : one launch over a pointer table (Trainer path for tensors that do not live in an arena).
 //   * n-ary sum (CommDevice reduce), scale+cast (the script-level `grad / num_samples` and `.astype('float16')`).
-// The update rules themselves (OptHyper, opt_elem / opt_apply, adam_lr) are in optim.cuh, shared with the HiPS fabric kernels.
+// The update rules themselves (OptHyper, opt_elem / opt_apply, sched_lr / step_lr) are in optim.cuh, shared with the HiPS fabric kernels.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -19,15 +19,15 @@ namespace gx {
 constexpr int ARENA_TILE = 1024;
 
 // step_state[0] = number of completed updates t, step_state[1] = CTA completion counter (self-resetting)
-template <int KIND>
+template <int KIND, bool SCHED>
 __global__ void __launch_bounds__(256) arena_opt_kernel(float* __restrict__ w, const float* __restrict__ g, float* __restrict__ s0, float* __restrict__ s1,
                                                          long long n, const float2* __restrict__ tile_mult, OptHyper h, int* __restrict__ step_state,
                                                          float* __restrict__ g_zero) {
   gx::pdl_wait();
   gx::pdl_launch();
-  h.kind = KIND;  // a compile-time kind: adam_lr and opt_apply4 reduce to this kernel's rule
+  h.kind = KIND;  // a compile-time kind: step_lr and opt_apply4 reduce to this kernel's rule
   const int t = step_state ? (*reinterpret_cast<volatile int*>(step_state)) + 1 : 1;
-  const float lr_t = adam_lr(h, t);
+  const float lr_t = step_lr<SCHED>(h, t);
   const long long n4 = n >> 2;  // arenas are tile-padded, n % 1024 == 0
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float lr = lr_t, wd = h.wd;
@@ -130,19 +130,26 @@ using namespace gx;
 static OptHyper mk(int kind, float lr, float wd, float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda) {
   OptHyper h; h.lr = lr; h.wd = wd; h.rescale = rescale; h.clip = clip; h.momentum = momentum; h.beta1 = b1; h.beta2 = b2; h.eps = eps; h.lamda = lamda;
   h.kind = kind;
+  h.sched = LrSchedule{};  // SCHED_NONE: the constant lr
   return h;
 }
 
 // kind: 0 sgd, 1 adam, 2 dcasgd.  n must be a multiple of 4 (arenas are 1024-padded).  step_state: int[2] device or null.
+// schedule: a host LrSchedule (lr is its base lr), or null for a constant lr.
 GX_API int gx_arena_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, const void* tile_mult, float lr, float wd,
                         float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda, int* step_state, float* g_zero,
-                        cudaStream_t s) {
-  const OptHyper h = mk(kind, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+                        const void* schedule, cudaStream_t s) {
+  OptHyper h = mk(kind, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+  if (schedule) h.sched = *reinterpret_cast<const LrSchedule*>(schedule);
   const int grid = grid_for(n, 4);
   const float2* tm = reinterpret_cast<const float2*>(tile_mult);
-  if (kind == OPT_SGD) launch_pdl(arena_opt_kernel<OPT_SGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, step_state, g_zero);
-  else if (kind == OPT_ADAM) launch_pdl(arena_opt_kernel<OPT_ADAM>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, step_state, g_zero);
-  else launch_pdl(arena_opt_kernel<OPT_DCASGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, step_state, g_zero);
+  const bool sched = h.sched.kind != SCHED_NONE;   // the constant-lr or the scheduled instance (step_lr<SCHED>)
+#define GX_ARENA(K) launch_pdl(sched ? arena_opt_kernel<K, true> : arena_opt_kernel<K, false>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, \
+                               step_state, g_zero)
+  if (kind == OPT_SGD) GX_ARENA(OPT_SGD);
+  else if (kind == OPT_ADAM) GX_ARENA(OPT_ADAM);
+  else GX_ARENA(OPT_DCASGD);
+#undef GX_ARENA
   return GX_CHECK_LAUNCH();
 }
 

@@ -193,8 +193,10 @@ class Trainer:
         from ..ops import native
         if len(self._contexts) != 1 or not native.available():
             return False
+        if self._optimizer.lr_scheduler is not None:
+            return False
         spec = self._optimizer.spec()
-        if spec is None or spec["name"] not in ("adam", "sgd") or self._optimizer.lr_scheduler is not None:
+        if spec is None or spec["name"] not in ("adam", "sgd"):
             return False
         ws, gs, idxs = [], [], []
         for i, p in self._trainable():

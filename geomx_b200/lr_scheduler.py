@@ -46,6 +46,36 @@ class LRScheduler:
     def __call__(self, num_update):
         return self.get_warmup_lr(num_update) if num_update < self.warmup_steps else self.decayed(num_update)
 
+    def device_spec(self):
+        """The schedule as a plain dict of fixed fields, for optimizers that evaluate it on the device from their step counter
+        (``sched_lr`` in ``csrc/kernels/optim.cuh``): ``kind`` ('factor', 'multifactor', 'poly' or 'cosine'), the warm-up fields and the
+        fields of that kind.  ``base_lr`` is not part of it: the optimizer passes it to the kernels as their ``lr``.
+
+        Raises ``ValueError`` for a scheduler whose values cannot be derived from these fields: a class other than the four above, a
+        subclass that overrides ``__call__`` / ``get_warmup_lr`` / ``decayed`` / ``shape`` / ``max_steps``, or a ``MultiFactorScheduler``
+        with more than :data:`DEVICE_MAX_MILESTONES` milestones (the size of the device struct's table)."""
+        name = type(self).__name__
+        base = next((c for c in type(self).__mro__ if c in _DEVICE_KINDS), None)
+        if base is None:
+            raise ValueError("%s cannot run on the device: only Factor / MultiFactor / Poly / Cosine schedules can" % name)
+        for attr in ("__call__", "get_warmup_lr", "decayed", "shape", "max_steps"):
+            if getattr(type(self), attr, None) is not getattr(base, attr, None):
+                raise ValueError("%s overrides %s: its values are no longer those of %s, so it cannot run on the device"
+                                 % (name, attr, base.__name__))
+        d = dict(kind=_DEVICE_KINDS[base], warmup_steps=int(self.warmup_steps), warmup_begin_lr=float(self.warmup_begin_lr),
+                 warmup_mode=self.warmup_mode, step=0, factor=1.0, stop_factor_lr=0.0, milestones=[], max_update=0, final_lr=0.0, pwr=1.0)
+        if base is FactorScheduler:
+            d.update(step=int(self.step), factor=float(self.factor), stop_factor_lr=float(self.stop_factor_lr))
+        elif base is MultiFactorScheduler:
+            if len(self.step) > DEVICE_MAX_MILESTONES:
+                raise ValueError("%s has %d milestones; the device schedule holds at most %d" % (name, len(self.step), DEVICE_MAX_MILESTONES))
+            d.update(milestones=[int(s) for s in self.step], factor=float(self.factor))
+        else:
+            d.update(max_update=int(self.max_update), final_lr=float(self.final_lr))
+            if base is PolyScheduler:
+                d.update(pwr=float(self.power))
+        return d
+
 
 class FactorScheduler(LRScheduler):
     """``base_lr * factor**k`` with one more factor every ``step`` updates (``k = (num_update - 1) // step``), never below ``stop_factor_lr``."""
@@ -118,3 +148,8 @@ class CosineScheduler(_Annealing):
 
     def shape(self, progress):
         return 0.5 * (1.0 + math.cos(math.pi * progress))
+
+
+# LRScheduler.device_spec: the classes the device evaluates, and the milestone table of its struct (LrSchedule::milestones)
+DEVICE_MAX_MILESTONES = 16
+_DEVICE_KINDS = {FactorScheduler: "factor", MultiFactorScheduler: "multifactor", PolyScheduler: "poly", CosineScheduler: "cosine"}

@@ -38,6 +38,7 @@ buffers of their own, ordered on the current stream after the steps enqueued bef
 """
 from __future__ import annotations
 
+import copy
 import os
 from typing import NamedTuple
 
@@ -190,6 +191,30 @@ class EvalHandle:
     item = wait
 
 
+def _key_mults(optimizer, net):
+    """Per-key ``(lr_mult, wd_mult)`` of the demo CNN's ten keys, resolved as ``Optimizer._get_lr`` / ``_get_wd`` resolve them for index
+    ``i``: the ``Parameter`` of ``net`` (what ``gluon.Trainer`` hands over through ``param_dict``) or the optimizer's ``param_dict``, then
+    ``optimizer.lr_mult`` / ``wd_mult`` by index, then by ``idx2name``."""
+    params = dict(optimizer.param_dict)
+    if net is not None:
+        params = dict(enumerate(net.collect_params().values()))
+    out = []
+    for i in range(len(CNN_PARAM_SHAPES)):
+        if i in params:
+            out.append((float(params[i].lr_mult), float(params[i].wd_mult)))
+            continue
+        m = []
+        for table in (optimizer.lr_mult, optimizer.wd_mult):
+            if i in table:
+                m.append(float(table[i]))
+            elif i in optimizer.idx2name:
+                m.append(float(table.get(optimizer.idx2name[i], 1.0)))
+            else:
+                m.append(1.0)
+        out.append(tuple(m))
+    return out
+
+
 class HipsCNNTrainStep:
     """Graph-captured training step of the demo CNN on the HiPS fabric.
 
@@ -198,7 +223,12 @@ class HipsCNNTrainStep:
     net : Gluon network from :func:`build_cnn` (initialised; its parameters are re-homed into the symmetric arena so
           ``net(x)`` / ``save_parameters`` keep working on the live weights) or ``None`` (Xavier init here).
     batch_size : per-worker batch (reference default 32).
-    optimizer : ``mx.optimizer.Optimizer`` with a native spec (Adam / SGD / DCASGD) — runs on the global-PS shard.
+    optimizer : ``mx.optimizer.Optimizer`` with a native spec (Adam / SGD / DCASGD) — runs on the global-PS shard.  Honoured in full:
+          its ``lr_scheduler`` (Factor / MultiFactor / Poly / Cosine, with warm-up) is evaluated by the update kernels from the device step
+          count, so every replay of the captured step takes the scheduled rate; per-key ``lr_mult`` / ``wd_mult`` (from ``net``'s
+          Parameters, else the optimizer's tables) scale each key's update; the step count starts at ``begin_num_update``.  An optimizer
+          whose schedule cannot run on the device (any other scheduler, or a subclass that changes a schedule's values) raises
+          ``ValueError`` here.  ``set_learning_rate`` changes a constant rate between steps; ``learning_rate`` is the rate of the next update.
     topo : :class:`Topology` (default: from ``WORLD_SIZE`` / ``RANK`` / ``GEOMX_NUM_PARTIES`` / ``DMLC_NUM_GLOBAL_SERVER``).
     """
 
@@ -231,8 +261,22 @@ class HipsCNNTrainStep:
         spec = optimizer.spec()
         if spec is None:
             raise ValueError("optimizer %s has no native spec; use Adam / SGD / DCASGD" % type(optimizer).__name__)
-        self.layout = ArenaLayout.build(list(enumerate(CNN_PARAM_SHAPES)))
+        sched = optimizer.lr_scheduler
+        if sched is not None:
+            if not hasattr(sched, "device_spec"):
+                raise ValueError("lr_scheduler %s cannot run on the device: only Factor / MultiFactor / Poly / Cosine schedules can"
+                                 % type(sched).__name__)
+            # raises ValueError for a schedule the kernels cannot evaluate.  The base lr is the scheduler's own, as Optimizer._get_lr
+            # applies it (the two differ only when the scheduler was attached after the optimizer was made); the engine keeps a copy of the
+            # scheduler as it was given, so that `learning_rate` reports what the kernels apply
+            spec = dict(spec, lr=float(sched.base_lr), lr_schedule=sched.device_spec())
+            sched = copy.copy(sched)
+        self.optimizer = optimizer
+        self._sched = sched
+        self._lr = float(spec["lr"])
+        self.layout = ArenaLayout.build(list(enumerate(CNN_PARAM_SHAPES)), mults=_key_mults(optimizer, net))
         self._local_spec = spec if self.update == "local" else None
+        self._local_sched = native.pack_schedule(spec["lr_schedule"]) if "lr_schedule" in spec else None   # packed once, for _local_opt
         self.fabric = HipsFabric(self.layout, self.topo, self.device, None if self.update == "local" else spec, use_multicast=use_multicast,
                                  loopback=loopback)
         # the script-level `grad / num_samples`, folded into the push kernel; with local updates the aggregate is also averaged over the workers
@@ -279,6 +323,16 @@ class HipsCNNTrainStep:
             self.s0l, self.s1l = torch.zeros_like(self.Wl), torch.zeros_like(self.Wl)
             self.opt_state = torch.zeros(4, dtype=torch.int32, device=self.device)
             self.P = [self.layout.view(self.Wl, i) for i in range(10)]
+        # resumed training: the device step count (schedule and Adam's bias correction) continues from begin_num_update, as the
+        # optimizer's own per-index count does
+        begin = int(optimizer.begin_num_update)
+        if begin:
+            if self.update == "local":
+                self.opt_state[0] = begin
+            elif mode == "dist_async":
+                f.flags.tensor[f.off["async_step"]: f.off["async_step"] + f.tiles] = begin      # the one-sided update counts per tile
+            else:
+                f.set_opt_step(begin)
         self._init_params(net)
         dev, f32 = self.device, torch.float32
         e = lambda *s, dt=f32: torch.empty(*s, dtype=dt, device=dev)
@@ -299,6 +353,7 @@ class HipsCNNTrainStep:
         self.label_cur = torch.empty_like(self.label) if path.lookahead else self.label
         self.x_cur = torch.empty_like(self.x) if path.lookahead else self.x        # ... and so must its images (conv0's weight gradient reads them)
         self._primed = False
+        self._warmed = False        # capture() has run its two eager warm-up steps
         self.graph = None
         self._graph_alt = None
         self._xbufs = [self.xin, None]
@@ -362,7 +417,7 @@ class HipsCNNTrainStep:
         rescale = sp["rescale_grad"] / self.B if self.hfa else sp["rescale_grad"]
         native.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], rescale,
                          -1.0 if clip is None else clip, sp.get("momentum", 0.0), sp.get("beta1", 0.9), sp.get("beta2", 0.999),
-                         sp.get("epsilon", 1e-8), sp.get("lamda", 0.04), self.opt_state, zero)
+                         sp.get("epsilon", 1e-8), sp.get("lamda", 0.04), self.opt_state, zero, schedule=self._local_sched)
 
     def _steps(self):
         """The training step of ``self.path`` as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch
@@ -516,28 +571,70 @@ class HipsCNNTrainStep:
             self.kernels_per_step = native.launch_count - before
 
     def capture(self):
-        """Warm up (2 eager steps on a side stream) and capture the step into a CUDA graph."""
+        """Warm up (2 eager steps on a side stream) and capture the step into a CUDA graph.  After ``set_learning_rate`` dropped the graphs,
+        only the capture runs: the warm-up steps are real updates and happen once per engine."""
         if self.graph is not None or not self.use_graph:
             return
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(2):
-                self._body()
-                self.steps_done += 1
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        if self._dgt_every:
-            self.fabric.dgt_rerank()      # first ranking now: the collective's lazy communicator set-up belongs to the warm-up, not to a timed step
-        if self.topo.world > 1:
-            import torch.distributed as dist
-            dist.barrier()
+        if not self._warmed:
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for _ in range(2):
+                    self._body()
+                    self.steps_done += 1
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            if self._dgt_every:
+                self.fabric.dgt_rerank()      # first ranking now: the collective's lazy communicator set-up belongs to the warm-up, not to a timed step
+            if self.topo.world > 1:
+                import torch.distributed as dist
+                dist.barrier()
+            self._warmed = True
         if self.lookahead:
             self._prime()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             self._body(part="rotated" if self.lookahead else "all")
         self.graph = g
+        self._graph_alt = None
+
+    # learning rate ---------------------------------------------------------------------------------------------------
+    @property
+    def opt_step(self):
+        """Number of optimizer updates applied so far (``begin_num_update`` included): the device step count that the schedule and
+        Adam's bias correction read.  Reading it synchronises with the device."""
+        if self.update == "local":
+            return int(self.opt_state[0])
+        f = self.fabric
+        if self.mode == "dist_async" and not self.hfa:
+            return int(f.flags.tensor[f.off["async_step"]: f.off["async_step"] + f.tiles].max())
+        return f.opt_step
+
+    @property
+    def learning_rate(self):
+        """The learning rate of the next update, before Adam's bias correction and the per-key ``lr_mult``: the schedule at
+        ``opt_step + 1``, or the constant lr."""
+        return self._sched(self.opt_step + 1) if self._sched is not None else self._lr
+
+    def set_learning_rate(self, lr):
+        """Set the constant learning rate of the following updates, as ``Optimizer.set_learning_rate`` / ``Trainer.set_learning_rate``
+        do (raises ``UserWarning`` when the optimizer has an ``lr_scheduler``: the schedule owns the rate).
+
+        The lr is part of the kernels' parameter blocks, which a captured graph holds: this waits for the device, drops the captured graphs
+        and lets the next step capture them again, without the warm-up steps of the first capture (a look-ahead engine keeps its primed
+        batch).  Several ranks: every rank calls it with the same value before the same step, as every worker calls its own
+        ``Trainer.set_learning_rate`` in the reference; in the replicated channels each rank updates its own replica of the server state
+        with the lr it was given."""
+        if self._sched is not None:
+            raise UserWarning("LRScheduler of the optimizer has already been defined.")
+        self.optimizer.set_learning_rate(lr)
+        self._lr = float(lr)
+        torch.cuda.synchronize(self.device)
+        if self.update == "local":
+            self._local_spec = dict(self._local_spec, lr=self._lr)
+        else:
+            self.fabric.set_optimizer(dict(self.fabric.opt_spec, lr=self._lr))
+        self.graph = None
         self._graph_alt = None
 
     def _prime(self):

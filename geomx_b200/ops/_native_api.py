@@ -416,10 +416,47 @@ def head_fwd_bwd(a, W, bias, label, loss, logits, dW, db, da, dbias_prev, relu_m
 # optimizer kind codes of the kernels (OptKind in csrc/kernels/optim.cuh)
 OPT_KIND = {"sgd": 0, "adam": 1, "dcasgd": 2}
 
+# learning-rate schedule kinds of the kernels (SchedKind in csrc/kernels/optim.cuh); the dicts come from LRScheduler.device_spec()
+SCHED_KIND = {None: 0, "none": 0, "factor": 1, "multifactor": 2, "poly": 3, "cosine": 4}
+SCHED_MAX_MILESTONES = 16
 
-def arena_opt(kind, w, g, s0, s1, n, tile_mult, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda, step_state, g_zero=None):
+
+class LrSchedule(ctypes.Structure):
+    """Mirror of ``LrSchedule`` (csrc/kernels/optim.cuh), the last member of ``OptHyper``."""
+    _fields_ = [("kind", ctypes.c_int), ("warmup_steps", ctypes.c_int), ("warmup_linear", ctypes.c_int), ("warmup_begin_lr", ctypes.c_float),
+                ("step", ctypes.c_int), ("factor", ctypes.c_float), ("stop_factor_lr", ctypes.c_float), ("num_milestones", ctypes.c_int),
+                ("milestones", ctypes.c_int * SCHED_MAX_MILESTONES), ("max_update", ctypes.c_int), ("final_lr", ctypes.c_float),
+                ("pwr", ctypes.c_float)]
+
+
+def pack_schedule(sched):
+    """``LRScheduler.device_spec()`` dict (or None: constant lr) -> :class:`LrSchedule`."""
+    s = LrSchedule()
+    if sched is None:
+        return s
+    ms = [int(m) for m in sched.get("milestones", [])]
+    if len(ms) > SCHED_MAX_MILESTONES:
+        raise ValueError("a device schedule holds at most %d milestones, got %d" % (SCHED_MAX_MILESTONES, len(ms)))
+    s.kind = SCHED_KIND[sched["kind"]]
+    s.warmup_steps, s.warmup_linear = int(sched["warmup_steps"]), int(sched["warmup_mode"] == "linear")
+    s.warmup_begin_lr = float(sched["warmup_begin_lr"])
+    s.step, s.factor, s.stop_factor_lr = int(sched["step"]), float(sched["factor"]), float(sched["stop_factor_lr"])
+    s.num_milestones = len(ms)
+    for i, m in enumerate(ms):
+        s.milestones[i] = m
+    s.max_update, s.final_lr, s.pwr = int(sched["max_update"]), float(sched["final_lr"]), float(sched["pwr"])
+    return s
+
+
+def arena_opt(kind, w, g, s0, s1, n, tile_mult, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda, step_state, g_zero=None, schedule=None):
+    """Fused arena optimizer; ``lr`` is the base lr of ``schedule`` (an ``LRScheduler.device_spec()`` dict, or an :class:`LrSchedule` that
+    :func:`pack_schedule` made from one), which the kernel evaluates at the device step count ``step_state[0] + 1``; ``schedule=None``:
+    constant lr."""
+    if schedule is not None and not isinstance(schedule, LrSchedule):
+        schedule = pack_schedule(schedule)
+    sched = None if schedule is None else ctypes.byref(schedule)
     _ck(_lib().gx_arena_opt(OPT_KIND[kind], _p(w), _p(g), _p(s0), _p(s1), n, _p(tile_mult), lr, wd, rescale, clip, momentum, b1, b2, eps,
-                            lamda, _p(step_state), _p(g_zero), _s()), "arena_opt")
+                            lamda, _p(step_state), _p(g_zero), sched, _s()), "arena_opt")
 
 
 def single_opt(kind, w, g, s0, s1, lr_t, wd, rescale, clip, momentum=0.0, b1=0.9, b2=0.999, eps=1e-8, lamda=0.04):

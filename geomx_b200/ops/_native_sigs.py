@@ -49,7 +49,7 @@ SIGS = {
     "gx_softmax_ce_bwd": [P, P, P, P, I, I, P],
     "gx_head_fwd_bwd": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
     # optim.cu
-    "gx_arena_opt": [I, P, P, P, P, L, P, F, F, F, F, F, F, F, F, F, P, P, P],
+    "gx_arena_opt": [I, P, P, P, P, L, P, F, F, F, F, F, F, F, F, F, P, P, P, P],
     "gx_multi_tensor_opt": [I, P, I, L, F, F, F, F, F, F, F, F, F, P],
     "gx_single_opt": [I, P, P, P, P, L, F, F, F, F, F, F, F, F, F, P],
     "gx_nary_sum": [P, P, I, L, P],

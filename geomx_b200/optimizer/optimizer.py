@@ -81,6 +81,14 @@ class Optimizer:
         d = dict(name=self.native_name, lr=float(self.lr), wd=float(self.wd), rescale_grad=float(self.rescale_grad),
                  clip_gradient=float(self.clip_gradient) if self.clip_gradient is not None else -1.0,
                  multi_precision=bool(self.multi_precision))
+        if self.lr_scheduler is not None:
+            # the schedule as the device evaluates it.  A schedule the device cannot evaluate leaves the key out (spec() itself must not
+            # raise: the KVStores and the Trainer call it for every optimizer); whoever needs the schedule on the device calls
+            # lr_scheduler.device_spec() for the reason.  spec_is_static() still says False, so the KVStores keep scheduled optimizers in Python.
+            try:
+                d["lr_schedule"] = self.lr_scheduler.device_spec()
+            except (ValueError, AttributeError):
+                pass
         d.update(kw)
         return d
 

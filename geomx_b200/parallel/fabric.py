@@ -19,7 +19,7 @@ import torch
 
 from ..base import MXNetError, getenv_int
 from ..ops import native
-from ..ops._native_api import OPT_KIND
+from ..ops._native_api import OPT_KIND, LrSchedule, pack_schedule
 from .arena import ArenaLayout
 
 MAX_RANKS = 16
@@ -175,7 +175,8 @@ class SymmetricHeap:
 
 # ------------------------------------------------------------------------------------------------------------ kernel parameter block
 class _OptHyperF(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_float) for n in ("lr", "wd", "rescale", "clip", "momentum", "beta1", "beta2", "eps", "lamda")] + [("kind", ctypes.c_int)]
+    _fields_ = ([(n, ctypes.c_float) for n in ("lr", "wd", "rescale", "clip", "momentum", "beta1", "beta2", "eps", "lamda")]
+                + [("kind", ctypes.c_int), ("sched", LrSchedule)])
 
 
 class _FabricParams(ctypes.Structure):
@@ -416,6 +417,7 @@ class HipsFabric:
         h.lr, h.wd, h.rescale, h.clip = s["lr"], s["wd"], s["rescale_grad"], s["clip_gradient"]
         h.momentum = s.get("momentum", 0.0); h.beta1 = s.get("beta1", 0.9); h.beta2 = s.get("beta2", 0.999)
         h.eps = s.get("epsilon", 1e-8); h.lamda = s.get("lamda", 0.04)
+        h.sched = pack_schedule(s.get("lr_schedule"))      # evaluated by the kernels at their step count; absent: constant lr
         return h
 
     def _block(self, channel, masked=False, zero_grad=False):
