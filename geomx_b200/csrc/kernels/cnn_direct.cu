@@ -885,7 +885,7 @@ __global__ void __launch_bounds__(288) __cluster_dims__(2, 1, 1)
 // the first packet: the tail CTAs are already running when the last gradient lands.
 //   state words of the channel (FabricParams::state): [0] round, [1] tail completion counter, [2] optimizer step, [5] protocol error, [6] tickets.
 // All 256 CTAs are co-resident (2 per SM on 132 SMs), so spinning on the ticket counter cannot starve the CTAs it waits for.
-template <bool SCHED>
+template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, const float* w1, const float* a1, const unsigned char* idx1, const float* a2,
                                                                 const unsigned char* idx2, const float* da2, float* dw0, float* db0, float* dw1, float* db1,
                                                                 int B, unsigned long long* dbg, const __grid_constant__ FabricParams p,
@@ -932,7 +932,7 @@ __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, c
   TileState s = tile_state_load(p, t, off, step_lr<SCHED>(p.h, opt_t));  // state loads overlap the flight of the packets
   const float4 agg = wire ? direct_recv_sum(p, off, f, epoch, err) : f4_scale(v, p.push_scale);
   stamp(23);
-  const float4 W = tile_state_apply(p, off, s, agg);
+  const float4 W = tile_state_apply<EXT>(p, off, s, agg);
   *reinterpret_cast<float4*>(p.param[p.rank] + off) = W;        // the pull is a local store: every rank holds the fresh replica
   if (threadIdx.x == 0) {
     const int done = atomicAdd(p.state + 1, 1);
@@ -1076,15 +1076,16 @@ GX_API int gx_cnn_bwd_exchange(const float* x, const float* w1, const float* a1,
   const size_t smem = smem_w > (size_t)CnnBwdSmem::BYTES ? smem_w : (size_t)CnnBwdSmem::BYTES;
   static size_t attr = 0;
   if (smem > attr) {
-    for (const void* k : {(const void*)cnn_bwd_exchange_kernel<false>, (const void*)cnn_bwd_exchange_kernel<true>}) {
+    for (const void* k : {(const void*)cnn_bwd_exchange_kernel<false, false>, (const void*)cnn_bwd_exchange_kernel<true, false>,
+                          (const void*)cnn_bwd_exchange_kernel<false, true>, (const void*)cnn_bwd_exchange_kernel<true, true>}) {
       cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return (int)e;
     }
     attr = smem;
   }
   const FabricParams p = *reinterpret_cast<const FabricParams*>(params);
-  // the constant-lr or the scheduled instance (step_lr<SCHED>)
-  launch_pdl(p.h.sched.kind != SCHED_NONE ? cnn_bwd_exchange_kernel<true> : cnn_bwd_exchange_kernel<false>, dim3(grid), dim3(288), smem, s, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1, B, g_cnn_dbg, p, tile_list,
+  // the constant-lr or the scheduled instance (step_lr<SCHED>), with the later optimizer kinds or without (opt_apply4<EXT>)
+  launch_pdl(GX_FAB_INSTANCE(cnn_bwd_exchange_kernel, p), dim3(grid), dim3(288), smem, s, x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1, B, g_cnn_dbg, p, tile_list,
              n_active);
   return GX_CHECK_LAUNCH();
 }

@@ -26,10 +26,11 @@
 namespace gx {
 
 // Global-owner side of one tile: optimizer + broadcast + per-key completion/flag.  `agg` is this thread's float4 of the summed gradient.
+template <bool EXT>
 __device__ __forceinline__ void global_apply_tile(const FabricParams& p, int t, float4 agg, uint32_t epoch, float lr_t) {
   const long long off = (long long)t * TILE + threadIdx.x * 4;
   TileState s = tile_state_load(p, t, off, lr_t);
-  const float4 W = tile_state_apply(p, off, s, agg);
+  const float4 W = tile_state_apply<EXT>(p, off, s, agg);
   if (p.world == 1) {  // degenerate single-rank HiPS: the arena optimizer, no cross-GPU traffic, flags or fences
     *reinterpret_cast<float4*>(p.param[0] + off) = W;
     return;
@@ -53,7 +54,7 @@ __device__ __forceinline__ void global_apply_tile(const FabricParams& p, int t, 
   }
 }
 
-template <bool SCHED>
+template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const FabricParams p) {
   gx::pdl_wait();
   gx::pdl_launch();
@@ -80,7 +81,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
       float* g = p.grad[0] + off;
       const float4 G = *reinterpret_cast<const float4*>(g);
       TileState s = tile_state_load(p, t, off, lr_t);
-      const float4 W = tile_state_apply(p, off, s, f4_scale(G, p.push_scale));
+      const float4 W = tile_state_apply<EXT>(p, off, s, f4_scale(G, p.push_scale));
       if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
       *reinterpret_cast<float4*>(p.param[0] + off) = W;
     }
@@ -124,7 +125,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
     if (p.zero_grad && p.world == 1) *reinterpret_cast<float4*>(p.grad[p.rank] + off) = make_float4(0.f, 0.f, 0.f, 0.f);
     const int owner = p.tile_owner[t];
     if (P == 1 && owner == p.rank) {
-      global_apply_tile(p, t, acc, epoch, lr_t);  // both tiers collapse: stay in registers
+      global_apply_tile<EXT>(p, t, acc, epoch, lr_t);  // both tiers collapse: stay in registers
       stamp(8);
     } else {
       st_f4_sys(p.stage[owner] + (long long)p.party * p.n + off, acc);
@@ -149,7 +150,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
     const long long off = (long long)t * TILE + threadIdx.x * 4;
     float4 acc = ld_f4_sys(p.stage[p.rank] + off);
     for (int g = 1; g < P; ++g) acc = f4_add(acc, ld_f4_sys(p.stage[p.rank] + (long long)g * p.n + off));
-    global_apply_tile(p, t, acc, epoch, lr_t);
+    global_apply_tile<EXT>(p, t, acc, epoch, lr_t);
     stamp(10);
   }
 
@@ -229,7 +230,7 @@ __device__ __forceinline__ uint32_t block_kth_largest(const uint32_t (&a)[4], in
   return prefix;
 }
 
-template <bool SCHED>
+template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const FabricParams p) {
   gx::pdl_wait();
   gx::pdl_launch();
@@ -350,7 +351,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
       agg = *reinterpret_cast<const float4*>(s_tile + threadIdx.x * 4);
     }
     if (p.dgt_contrib != nullptr) dgt_update_contrib(p, t, agg, s_red);
-    const float4 W = tile_state_apply(p, off, s, agg);
+    const float4 W = tile_state_apply<EXT>(p, off, s, agg);
     if (fmt == FMT_BSC && p.h.kind < 0) {
       // BSCPullCompress (:271-308): the aggregated gradient goes back sparse — its non-zeros in index order, at most P*K of them
       const float ww[4] = {W.x, W.y, W.z, W.w};
@@ -427,7 +428,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_ll_kernel(const Fabri
 // sharded channel runs on a side stream underneath the convolution backward pass; the conv keys' replicated channel is the only exposed
 // communication).  Reference for the ordering idea: per-key push with priority = -index (examples/cnn.py:121-125, kvstore_dist.h:565-625).
 // Every channel owns its state block (epoch, CTA counter, optimizer step) and stamps its id into the packet epoch.
-template <bool SCHED>
+template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const FabricParams p) {
   // Before the grid dependency resolves (i.e. while the kernel that produces the gradients is still running): walk this CTA's tiles once and
   // pull everything that does NOT depend on that kernel towards L2 — the tile metadata, the optimizer state and master weights of the tiles
@@ -487,7 +488,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
     TileState s = tile_state_load(p, t, off, lr_t);   // issued before the polls: the state loads overlap the wait
     const float4 agg = direct_recv_sum(p, off, f, epoch, err);
     if (p.dgt_contrib != nullptr && (!rep || p.tile_owner[t] == p.rank)) dgt_update_contrib(p, t, agg, s_red);
-    const float4 W = tile_state_apply(p, off, s, agg);
+    const float4 W = tile_state_apply<EXT>(p, off, s, agg);
     if (rep) {
       *reinterpret_cast<float4*>(p.param[p.rank] + off) = W;   // the pull is a local store: every rank holds the fresh replica
     } else {
@@ -521,7 +522,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 2) hips_fsa_direct_kernel(const F
 
 // One-sided MixedSync: the party's tile owner applies its aggregate directly on the global owner's HBM under a per-tile lock.
 // locks live in the global owner's flag pad at `lock_off` (uint32 per tile), per-tile optimizer step counts right after them.
-template <bool SCHED>
+template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(FAB_THREADS, 1) hips_async_step_kernel(const FabricParams p, float* const* w_peer, float* const* s0_peer,
                                                                           float* const* s1_peer, int lock_off, int step_off) {
   gx::pdl_wait();
@@ -567,7 +568,7 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_async_step_kernel(const F
     float4 W = ld_f4_sys(wp);
     float4 A = s0_peer[owner] ? ld_f4_sys(s0_peer[owner] + off) : make_float4(0, 0, 0, 0);
     float4 B = s1_peer[owner] ? ld_f4_sys(s1_peer[owner] + off) : make_float4(0, 0, 0, 0);
-    opt_apply4(W, acc, A, B, p.h, lr, wd);
+    opt_apply4<EXT>(W, acc, A, B, p.h, lr, wd);
     st_f4_sys(wp, W);
     if (s0_peer[owner]) st_f4_sys(s0_peer[owner] + off, A);
     if (s1_peer[owner]) st_f4_sys(s1_peer[owner] + off, B);
@@ -709,7 +710,7 @@ GX_API int gx_fabric_params_size() { return (int)sizeof(FabricParams); }
 GX_API int gx_hips_fsa_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_step_kernel<true> : hips_fsa_step_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  launch_pdl(GX_FAB_INSTANCE(hips_fsa_step_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
 // Largest co-resident grid of the fused kernels (they spin on each other: every CTA of a launch must be resident).
@@ -717,8 +718,11 @@ GX_API int gx_hips_max_grid() {
   int dev = 0, sms = 0, occ = 1 << 30;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  for (const void* k : {(const void*)hips_fsa_ll_kernel<false>, (const void*)hips_fsa_ll_kernel<true>, (const void*)hips_fsa_step_kernel<false>,
-                        (const void*)hips_fsa_step_kernel<true>}) {   // both instances of each: constant and scheduled lr
+  // every instance of each: constant and scheduled lr, with and without the later optimizer kinds
+  for (const void* k : {(const void*)hips_fsa_ll_kernel<false, false>, (const void*)hips_fsa_ll_kernel<true, false>,
+                        (const void*)hips_fsa_ll_kernel<false, true>, (const void*)hips_fsa_ll_kernel<true, true>,
+                        (const void*)hips_fsa_step_kernel<false, false>, (const void*)hips_fsa_step_kernel<true, false>,
+                        (const void*)hips_fsa_step_kernel<false, true>, (const void*)hips_fsa_step_kernel<true, true>}) {
     int o = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k, FAB_THREADS, 0);
     occ = o < occ ? o : occ;
@@ -728,20 +732,20 @@ GX_API int gx_hips_max_grid() {
 GX_API int gx_hips_fsa_ll_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_ll_kernel<true> : hips_fsa_ll_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  launch_pdl(GX_FAB_INSTANCE(hips_fsa_ll_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_hips_fsa_direct_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_fsa_direct_kernel<true> : hips_fsa_direct_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s,
+  launch_pdl(GX_FAB_INSTANCE(hips_fsa_direct_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s,
              p);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_hips_async_step(const void* params, float* const* w_peer, float* const* s0_peer, float* const* s1_peer, int lock_off, int step_off,
                               int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
-  launch_pdl(p.h.sched.kind != SCHED_NONE ? hips_async_step_kernel<true> : hips_async_step_kernel<false>, dim3(grid), dim3(FAB_THREADS), 0, s, p,
+  launch_pdl(GX_FAB_INSTANCE(hips_async_step_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p,
              w_peer, s0_peer, s1_peer, lock_off, step_off);
   return GX_CHECK_LAUNCH();
 }

@@ -67,6 +67,13 @@ struct FabricParams {
                                // 0: the tile's global owner does and pushes the result back (two hops)
   int channel_id;              // 0..7, folded into the packet epoch so that channels can never mistake each other's packets
 };
+// The instance of a fabric kernel (template <bool SCHED, bool EXT>) for a parameter block: the scheduled-lr instance when the block has a
+// schedule (step_lr<SCHED>), and the one with the later optimizer kinds compiled in only for those kinds (opt_apply4<EXT>).
+#define GX_FAB_INSTANCE(kern, p)                                                                                      \
+  ((p).h.sched.kind != SCHED_NONE ? ((p).h.kind > OPT_DCASGD ? kern<true, true> : kern<true, false>)                  \
+                                  : ((p).h.kind > OPT_DCASGD ? kern<false, true> : kern<false, false>))
+// parallel/fabric.py's _FabricParams mirrors this block and asserts the same size (FABRIC_PARAMS_BYTES); kernel parameters are limited to 4 KB
+static_assert(sizeof(FabricParams) == 1656 && offsetof(FabricParams, h) == 728, "FabricParams layout (parallel/fabric.py)");
 
 __device__ __forceinline__ void wait_flag_ge(const uint32_t* p, uint32_t v) {
   while (ld_acquire_sys(p) < v) { __nanosleep(20); }
@@ -90,8 +97,9 @@ __device__ __forceinline__ TileState tile_state_load(const FabricParams& p, int 
   return s;
 }
 // optimizer step on `agg`, state stored back; returns the fresh weights
+template <bool EXT>
 __device__ __forceinline__ float4 tile_state_apply(const FabricParams& p, long long off, TileState& s, float4 agg) {
-  opt_apply4(s.W, agg, s.A, s.B, p.h, s.lr, s.wd);
+  opt_apply4<EXT>(s.W, agg, s.A, s.B, p.h, s.lr, s.wd);
   *reinterpret_cast<float4*>(p.w + off) = s.W;
   if (p.s0) *reinterpret_cast<float4*>(p.s0 + off) = s.A;
   if (p.s1) *reinterpret_cast<float4*>(p.s1 + off) = s.B;

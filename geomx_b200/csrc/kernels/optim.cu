@@ -1,6 +1,6 @@
 // Fused optimizer / elementwise kernels for sm_90a.
 //
-// Reference: SGD / SGD-momentum / Adam / DCASGD are 1-3 mshadow MapPlanKernel passes *per parameter*
+// Reference: SGD / SGD-momentum / Adam / DCASGD and the other element-wise rules are 1-3 mshadow MapPlanKernel passes *per parameter*
 // (src/operator/optimizer_op-inl.h:86-103,305-326,840-873; DCASGD python/mxnet/optimizer/optimizer.py:872-925), driven by a
 // Python loop.  Here:
 //   * arena_* : ONE launch updates a whole flat parameter arena (all keys), 128-bit accesses, with the step counter and
@@ -8,7 +8,7 @@
 //     Per-key lr/wd multipliers come from a per-tile table (tile = 1024 floats; keys are tile-aligned in the arena).
 //   * multi_tensor_* : one launch over a pointer table (Trainer path for tensors that do not live in an arena).
 //   * n-ary sum (CommDevice reduce), scale+cast (the script-level `grad / num_samples` and `.astype('float16')`).
-// The update rules themselves (OptHyper, opt_elem / opt_apply, sched_lr / step_lr) are in optim.cuh, shared with the HiPS fabric kernels.
+// The update rules themselves (OptHyper, opt_elem / opt_apply4, sched_lr / step_lr) are in optim.cuh, shared with the HiPS fabric kernels.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -36,7 +36,7 @@ __global__ void __launch_bounds__(256) arena_opt_kernel(float* __restrict__ w, c
     const float4 G = reinterpret_cast<const float4*>(g)[i];
     float4 A = s0 ? reinterpret_cast<float4*>(s0)[i] : make_float4(0, 0, 0, 0);
     float4 Bv = s1 ? reinterpret_cast<float4*>(s1)[i] : make_float4(0, 0, 0, 0);
-    opt_apply4(W, G, A, Bv, h, lr, wd);
+    opt_apply4<(KIND > OPT_DCASGD)>(W, G, A, Bv, h, lr, wd);
     reinterpret_cast<float4*>(w)[i] = W;
     if (s0) reinterpret_cast<float4*>(s0)[i] = A;
     if (s1) reinterpret_cast<float4*>(s1)[i] = Bv;
@@ -128,51 +128,83 @@ static inline int grid_for(long long n, int per_thread = 1) {
 using namespace gx;
 
 static OptHyper mk(int kind, float lr, float wd, float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda) {
-  OptHyper h; h.lr = lr; h.wd = wd; h.rescale = rescale; h.clip = clip; h.momentum = momentum; h.beta1 = b1; h.beta2 = b2; h.eps = eps; h.lamda = lamda;
+  OptHyper h{};   // the fields of the later kinds 0; sched SCHED_NONE: the constant lr
+  h.lr = lr; h.wd = wd; h.rescale = rescale; h.clip = clip; h.momentum = momentum; h.beta1 = b1; h.beta2 = b2; h.eps = eps; h.lamda = lamda;
   h.kind = kind;
-  h.sched = LrSchedule{};  // SCHED_NONE: the constant lr
   return h;
 }
 
-// kind: 0 sgd, 1 adam, 2 dcasgd.  n must be a multiple of 4 (arenas are 1024-padded).  step_state: int[2] device or null.
-// schedule: a host LrSchedule (lr is its base lr), or null for a constant lr.
-GX_API int gx_arena_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, const void* tile_mult, float lr, float wd,
-                        float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda, int* step_state, float* g_zero,
-                        const void* schedule, cudaStream_t s) {
-  OptHyper h = mk(kind, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
-  if (schedule) h.sched = *reinterpret_cast<const LrSchedule*>(schedule);
+// one case per OptKind: the kernels are instantiated per kind, so that each instance compiles to its own rule only
+#define GX_OPT_DISPATCH(kind, LAUNCH)                     \
+  switch (kind) {                                         \
+    case OPT_SGD: LAUNCH(OPT_SGD); break;                 \
+    case OPT_ADAM: LAUNCH(OPT_ADAM); break;               \
+    case OPT_DCASGD: LAUNCH(OPT_DCASGD); break;           \
+    case OPT_NAG: LAUNCH(OPT_NAG); break;                 \
+    case OPT_SIGNUM: LAUNCH(OPT_SIGNUM); break;           \
+    case OPT_RMSPROP: LAUNCH(OPT_RMSPROP); break;         \
+    case OPT_ADAGRAD: LAUNCH(OPT_ADAGRAD); break;         \
+    case OPT_ADADELTA: LAUNCH(OPT_ADADELTA); break;       \
+    case OPT_FTRL: LAUNCH(OPT_FTRL); break;               \
+    default: return -1;                                   \
+  }
+
+// The entry points that take a packed OptHyper (ops/_native_api.py pack_hyper): every kind and all of its hyper-parameters.  The
+// schedule travels inside it (h.sched).  n must be a multiple of 4 (arenas are 1024-padded).  step_state: int[2] device or null.
+GX_API int gx_arena_opt_h(const void* hyper, float* w, const float* g, float* s0, float* s1, long long n, const void* tile_mult,
+                          int* step_state, float* g_zero, cudaStream_t s) {
+  const OptHyper h = *reinterpret_cast<const OptHyper*>(hyper);
   const int grid = grid_for(n, 4);
   const float2* tm = reinterpret_cast<const float2*>(tile_mult);
   const bool sched = h.sched.kind != SCHED_NONE;   // the constant-lr or the scheduled instance (step_lr<SCHED>)
 #define GX_ARENA(K) launch_pdl(sched ? arena_opt_kernel<K, true> : arena_opt_kernel<K, false>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, tm, h, \
                                step_state, g_zero)
-  if (kind == OPT_SGD) GX_ARENA(OPT_SGD);
-  else if (kind == OPT_ADAM) GX_ARENA(OPT_ADAM);
-  else GX_ARENA(OPT_DCASGD);
+  GX_OPT_DISPATCH(h.kind, GX_ARENA)
 #undef GX_ARENA
   return GX_CHECK_LAUNCH();
+}
+
+// lr_t: the step's lr (Adam: bias-corrected), the same for every tensor; tensors scale it by their lr_mult
+GX_API int gx_multi_tensor_opt_h(const void* hyper, const void* table, int num_tensors, long long max_n, float lr_t, cudaStream_t s) {
+  const OptHyper h = *reinterpret_cast<const OptHyper*>(hyper);
+  int gx_ = grid_for(max_n); if (gx_ > 64) gx_ = 64;
+  dim3 grid(gx_, num_tensors);
+  const TensorEntry* t = reinterpret_cast<const TensorEntry*>(table);
+#define GX_MT(K) launch_pdl(multi_tensor_opt_kernel<K>, dim3(grid), dim3(256), 0, s, t, h, lr_t)
+  GX_OPT_DISPATCH(h.kind, GX_MT)
+#undef GX_MT
+  return GX_CHECK_LAUNCH();
+}
+
+GX_API int gx_single_opt_h(const void* hyper, float* w, const float* g, float* s0, float* s1, long long n, float lr_t, cudaStream_t s) {
+  const OptHyper h = *reinterpret_cast<const OptHyper*>(hyper);
+  const int grid = grid_for(n);
+#define GX_SINGLE(K) launch_pdl(single_opt_kernel<K>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t)
+  GX_OPT_DISPATCH(h.kind, GX_SINGLE)
+#undef GX_SINGLE
+  return GX_CHECK_LAUNCH();
+}
+
+// The positional entry points of SGD / Adam / DCASGD (kind 0 / 1 / 2).  schedule: a host LrSchedule (lr is its base lr), or null for a
+// constant lr.
+GX_API int gx_arena_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, const void* tile_mult, float lr, float wd,
+                        float rescale, float clip, float momentum, float b1, float b2, float eps, float lamda, int* step_state, float* g_zero,
+                        const void* schedule, cudaStream_t s) {
+  OptHyper h = mk(kind, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda);
+  if (schedule) h.sched = *reinterpret_cast<const LrSchedule*>(schedule);
+  return gx_arena_opt_h(&h, w, g, s0, s1, n, tile_mult, step_state, g_zero, s);
 }
 
 GX_API int gx_multi_tensor_opt(int kind, const void* table, int num_tensors, long long max_n, float lr_t, float wd, float rescale, float clip,
                                float momentum, float b1, float b2, float eps, float lamda, cudaStream_t s) {
   const OptHyper h = mk(kind, lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
-  int gx_ = grid_for(max_n); if (gx_ > 64) gx_ = 64;
-  dim3 grid(gx_, num_tensors);
-  const TensorEntry* t = reinterpret_cast<const TensorEntry*>(table);
-  if (kind == OPT_SGD) launch_pdl(multi_tensor_opt_kernel<OPT_SGD>, dim3(grid), dim3(256), 0, s, t, h, lr_t);
-  else if (kind == OPT_ADAM) launch_pdl(multi_tensor_opt_kernel<OPT_ADAM>, dim3(grid), dim3(256), 0, s, t, h, lr_t);
-  else launch_pdl(multi_tensor_opt_kernel<OPT_DCASGD>, dim3(grid), dim3(256), 0, s, t, h, lr_t);
-  return GX_CHECK_LAUNCH();
+  return gx_multi_tensor_opt_h(&h, table, num_tensors, max_n, lr_t, s);
 }
 
 GX_API int gx_single_opt(int kind, float* w, const float* g, float* s0, float* s1, long long n, float lr_t, float wd, float rescale, float clip,
                          float momentum, float b1, float b2, float eps, float lamda, cudaStream_t s) {
   const OptHyper h = mk(kind, lr_t, wd, rescale, clip, momentum, b1, b2, eps, lamda);
-  const int grid = grid_for(n);
-  if (kind == OPT_SGD) launch_pdl(single_opt_kernel<OPT_SGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t);
-  else if (kind == OPT_ADAM) launch_pdl(single_opt_kernel<OPT_ADAM>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t);
-  else launch_pdl(single_opt_kernel<OPT_DCASGD>, dim3(grid), dim3(256), 0, s, w, g, s0, s1, n, h, lr_t);
-  return GX_CHECK_LAUNCH();
+  return gx_single_opt_h(&h, w, g, s0, s1, n, lr_t, s);
 }
 
 GX_API int gx_nary_sum(float* out, const float* const* inputs, int cnt, long long n, cudaStream_t s) {

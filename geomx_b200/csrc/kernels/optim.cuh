@@ -6,7 +6,10 @@
 
 namespace gx {
 
-enum OptKind { OPT_NONE = -1, OPT_SGD = 0, OPT_ADAM = 1, OPT_DCASGD = 2 };
+enum OptKind {
+  OPT_NONE = -1, OPT_SGD = 0, OPT_ADAM = 1, OPT_DCASGD = 2,
+  OPT_NAG = 3, OPT_SIGNUM = 4, OPT_RMSPROP = 5, OPT_ADAGRAD = 6, OPT_ADADELTA = 7, OPT_FTRL = 8
+};
 
 // The learning-rate schedules of lr_scheduler.py, as LRScheduler.device_spec() describes them; ops/_native_api.py packs that dict.
 enum SchedKind { SCHED_NONE = 0, SCHED_FACTOR = 1, SCHED_MULTIFACTOR = 2, SCHED_POLY = 3, SCHED_COSINE = 4 };
@@ -23,20 +26,75 @@ struct LrSchedule {
   float final_lr, pwr;
 };
 
-// Field order is part of the ABI: parallel/fabric.py's _OptHyperF mirrors it inside FabricParams.
+// Field order is part of the ABI: ops/_native_api.py's OptHyper mirrors it (also inside parallel/fabric.py's FabricParams); the
+// static_asserts below pin the offsets that the Python side asserts too.
 struct OptHyper {
   float lr, wd, rescale, clip;      // clip < 0 -> off; lr: the base lr of a schedule
-  float momentum;                   // sgd / dcasgd
-  float beta1, beta2, eps;          // adam
+  float momentum;                   // sgd / dcasgd / nag / signum
+  float beta1, beta2, eps;          // adam; eps also rmsprop / adagrad / adadelta
   float lamda;                      // dcasgd
+  float wd_lh;                      // signum: decoupled weight decay
+  float clip_weights;               // rmsprop: clamp of the new weight, < 0 -> off
+  float gamma1;                     // rmsprop: decay of the squared-gradient average
+  float rho;                        // adadelta
+  float beta, lamda1;               // ftrl
   int kind;                         // OptKind; OPT_NONE (fabric only): store the aggregated gradient (Bi-Sparse / local-optimizer modes)
   LrSchedule sched;
 };
+static_assert(sizeof(LrSchedule) == 108, "LrSchedule layout (ops/_native_api.py)");
+static_assert(offsetof(OptHyper, wd_lh) == 36 && offsetof(OptHyper, lamda1) == 56 && offsetof(OptHyper, kind) == 60 &&
+              offsetof(OptHyper, sched) == 64 && sizeof(OptHyper) == 172, "OptHyper layout (ops/_native_api.py)");
 
-// one element of each optimizer (s0/s1 = state slots: sgd: s0=mom; adam: s0=m, s1=v; dcasgd: s0=mom, s1=prev_weight)
+__device__ __forceinline__ float clip_to(float x, float c) { return c >= 0.f ? fminf(fmaxf(x, -c), c) : x; }
+__device__ __forceinline__ float sign_of(float x) { return (float)((x > 0.f) - (x < 0.f)); }
+
+// One element of each optimizer, written from the reference's update operators (src/operator/optimizer_op-inl.h) and optimizer.py.
+// State slots s0 / s1: sgd, nag, signum: s0 = mom; adam: s0 = m, s1 = v; dcasgd: s0 = mom, s1 = previous weight; rmsprop: s0 = n;
+// adagrad: s0 = history; adadelta: s0 = acc_g, s1 = acc_delta; ftrl: s0 = z, s1 = n.  Every state starts at 0 except dcasgd's s1.
 template <int KIND>
 __device__ __forceinline__ void opt_elem(float& w, float g, float& s0, float& s1, const OptHyper& h, float lr, float wd) {
-  if (KIND == OPT_SGD) {
+  if (KIND == OPT_NAG) {
+    // optimizer.py NAG: rescale, clip, then mom = mu*mom + (g + wd*w); w -= lr * (g + wd*w + mu*mom)
+    g = fmaf(wd, w, clip_to(g * h.rescale, h.clip));
+    if (h.momentum != 0.f) { s0 = fmaf(h.momentum, s0, g); g = fmaf(h.momentum, s0, g); }
+    w -= lr * g;
+  } else if (KIND == OPT_SIGNUM) {
+    if (h.momentum != 0.f) {
+      // SignumKernel: mom = mu*mom - (1-mu)*wd*w - (1-mu)*clip(rescale*g); w = (1 - lr*wd_lh)*w + lr*sign(mom)
+      s0 = h.momentum * s0 - (1.f - h.momentum) * fmaf(wd, w, clip_to(g * h.rescale, h.clip));
+      w = (1.f - lr * h.wd_lh) * w + lr * sign_of(s0);
+    } else {
+      // SignSGDKernel: decoupled wd, no clip, no wd_lh
+      w = (1.f - lr * wd) * w - lr * sign_of(g);
+    }
+  } else if (KIND == OPT_RMSPROP) {
+    // RMSPropUpdate: rescale, + wd*w, THEN clip; eps inside the sqrt; clip_weights clamps the new weight
+    g = clip_to(fmaf(wd, w, g * h.rescale), h.clip);
+    s0 = (1.f - h.gamma1) * g * g + h.gamma1 * s0;
+    w = clip_to(w - lr * (g / sqrtf(s0 + h.eps)), h.clip_weights);
+  } else if (KIND == OPT_ADAGRAD) {
+    // optimizer.py AdaGrad (dense): rescale, clip; history += g^2; w += (g / sqrt(history + eps) + wd*w) * -lr
+    g = clip_to(g * h.rescale, h.clip);
+    s0 = fmaf(g, g, s0);
+    w -= lr * (g / sqrtf(s0 + h.eps) + wd * w);
+  } else if (KIND == OPT_ADADELTA) {
+    // optimizer.py AdaDelta: no learning rate; wd outside the adaptive step
+    g = clip_to(g * h.rescale, h.clip);
+    s0 = h.rho * s0 + (1.f - h.rho) * g * g;
+    const float d = sqrtf(s1 + h.eps) / sqrtf(s0 + h.eps) * g;
+    s1 = h.rho * s1 + (1.f - h.rho) * d * d;
+    w -= d + wd * w;
+  } else if (KIND == OPT_FTRL) {
+    // FtrlUpdate: z += g - (sqrt(n + g^2) - sqrt(n)) * w / lr; n += g^2; w = (sign(z)*lamda1 - z) / ((beta + sqrt(n)) / lr + wd) masked by
+    // |z| > lamda1.  sqrt(n + g^2) - sqrt(n) is computed as g^2 / (sqrt(n + g^2) + sqrt(n)), the same value without the cancellation that
+    // the literal difference suffers in fp32 once n >> g^2 (it would lose every digit of the increment after a few hundred updates).
+    g = clip_to(g * h.rescale, h.clip);
+    const float g2 = g * g, sn = sqrtf(s1), sn1 = sqrtf(s1 + g2);
+    const float sigma = sn1 + sn > 0.f ? g2 / (sn1 + sn) : 0.f;
+    s0 += g - sigma * w / lr;
+    s1 += g2;
+    w = fabsf(s0) > h.lamda1 ? (sign_of(s0) * h.lamda1 - s0) / ((h.beta + sn1) / lr + wd) : 0.f;
+  } else if (KIND == OPT_SGD) {
     g *= h.rescale;
     if (h.clip >= 0.f) g = fminf(fmaxf(g, -h.clip), h.clip);
     g = fmaf(wd, w, g);
@@ -60,7 +118,7 @@ __device__ __forceinline__ void opt_elem(float& w, float g, float& s0, float& s1
   }
 }
 
-// the same, with the kind chosen at run time by h.kind
+// the run-time dispatch over SGD / Adam / DCASGD, one element
 __device__ __forceinline__ void opt_apply(float& w, float g, float& s0, float& s1, const OptHyper& h, float lr, float wd) {
   if (h.kind == OPT_ADAM) opt_elem<OPT_ADAM>(w, g, s0, s1, h, lr, wd);
   else if (h.kind == OPT_SGD) opt_elem<OPT_SGD>(w, g, s0, s1, h, lr, wd);
@@ -68,12 +126,32 @@ __device__ __forceinline__ void opt_apply(float& w, float g, float& s0, float& s
   else w = g;  // no optimizer on the server: store the aggregate (reference ApplyUpdates without updater_, :547-550)
 }
 
-// four consecutive elements (one float4 of each operand)
+template <int KIND>
+__device__ __forceinline__ void opt_elem4(float4& W, float4 G, float4& A, float4& B, const OptHyper& h, float lr, float wd) {
+  opt_elem<KIND>(W.x, G.x, A.x, B.x, h, lr, wd);
+  opt_elem<KIND>(W.y, G.y, A.y, B.y, h, lr, wd);
+  opt_elem<KIND>(W.z, G.z, A.z, B.z, h, lr, wd);
+  opt_elem<KIND>(W.w, G.w, A.w, B.w, h, lr, wd);
+}
+
+// The server update of the fabric kernels: four consecutive elements (one float4 of each operand), the kind chosen at run time by h.kind.
+// EXT: the instance also runs the kinds after DCASGD (NAG .. Ftrl).  The fabric kernels are instantiated with and without them and their
+// launchers pick EXT only for those kinds (GX_FAB_INSTANCE, hips_ll.cuh): the SGD / Adam / DCASGD instances compile to the code they had
+// before the later kinds existed, which keeps the training step's exchange kernels as short as they were.
+template <bool EXT>
 __device__ __forceinline__ void opt_apply4(float4& W, float4 G, float4& A, float4& B, const OptHyper& h, float lr, float wd) {
-  opt_apply(W.x, G.x, A.x, B.x, h, lr, wd);
-  opt_apply(W.y, G.y, A.y, B.y, h, lr, wd);
-  opt_apply(W.z, G.z, A.z, B.z, h, lr, wd);
-  opt_apply(W.w, G.w, A.w, B.w, h, lr, wd);
+  if (!EXT) {
+    opt_apply(W.x, G.x, A.x, B.x, h, lr, wd);
+    opt_apply(W.y, G.y, A.y, B.y, h, lr, wd);
+    opt_apply(W.z, G.z, A.z, B.z, h, lr, wd);
+    opt_apply(W.w, G.w, A.w, B.w, h, lr, wd);
+  } else if (h.kind == OPT_NAG) opt_elem4<OPT_NAG>(W, G, A, B, h, lr, wd);
+  else if (h.kind == OPT_SIGNUM) opt_elem4<OPT_SIGNUM>(W, G, A, B, h, lr, wd);
+  else if (h.kind == OPT_RMSPROP) opt_elem4<OPT_RMSPROP>(W, G, A, B, h, lr, wd);
+  else if (h.kind == OPT_ADAGRAD) opt_elem4<OPT_ADAGRAD>(W, G, A, B, h, lr, wd);
+  else if (h.kind == OPT_ADADELTA) opt_elem4<OPT_ADADELTA>(W, G, A, B, h, lr, wd);
+  else if (h.kind == OPT_FTRL) opt_elem4<OPT_FTRL>(W, G, A, B, h, lr, wd);
+  else opt_apply4<false>(W, G, A, B, h, lr, wd);
 }
 
 // learning rate of update t (1-based) before Adam's bias correction: the fp32 mirror of LRScheduler.__call__(t) with base_lr = h.lr.

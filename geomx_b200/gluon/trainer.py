@@ -196,7 +196,7 @@ class Trainer:
         if self._optimizer.lr_scheduler is not None:
             return False
         spec = self._optimizer.spec()
-        if spec is None or spec["name"] not in ("adam", "sgd"):
+        if spec is None or spec["name"] not in native.OPT_KINDS:
             return False
         ws, gs, idxs = [], [], []
         for i, p in self._trainable():

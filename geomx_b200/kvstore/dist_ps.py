@@ -40,6 +40,11 @@ def _pinned(numel, dtype):
     return t
 
 
+# the kinds the C++ host server executes from a spec (csrc/hips/server_optim.h, ServerOptSpec::valid); it aborts on any other name, so the
+# other native kinds ship the pickled optimizer like any Python optimizer
+HOST_SERVER_KINDS = ("sgd", "adam", "dcasgd")
+
+
 def spec_to_string(spec):
     return ";".join("%s=%s" % (k, v) for k, v in spec.items() if k != "multi_precision")
 
@@ -196,7 +201,8 @@ class KVStoreDist(KVStoreBase):
             import os
             # the declarative spec carries one scalar lr / wd: an lr_scheduler or per-parameter multipliers (e.g. wd_mult = 0 on biases) need the
             # optimizer object itself on the server, which is what the reference always ships (kvstore.py:452-499)
-            if spec is not None and optimizer.spec_is_static() and os.environ.get("GEOMX_PY_UPDATER", "0") != "1":
+            if (spec is not None and spec["name"] in HOST_SERVER_KINDS and optimizer.spec_is_static()
+                    and os.environ.get("GEOMX_PY_UPDATER", "0") != "1"):
                 self._kv.send_command_to_servers(CMD_OPT_SPEC, spec_to_string(spec))
             else:
                 self._kv.send_command_to_servers(CMD_CONTROLLER, pickle.dumps(optimizer, 0).decode("latin1"))

@@ -215,15 +215,29 @@ def _key_mults(optimizer, net):
     return out
 
 
+_NATIVE_OPTIMIZERS = "SGD, Adam, DCASGD, NAG, Signum, RMSProp (centered=False), AdaGrad, AdaDelta, Ftrl"
+# why the other optimizers of the library do not run in the update kernels
+_NOT_NATIVE = {
+    "RMSProp(centered=True)": "centered RMSProp keeps three state arrays, the kernels two",
+    "FTML": "it keeps three state arrays, the kernels two",
+    "Nadam": "its momentum schedule is one scalar shared by all keys and advanced once per key update",
+    "Adamax": "m / u is 0 / 0 wherever every gradient so far was exactly 0, where the reference writes NaN",
+    "SGLD": "it needs a device random-number generator",
+    "LBSGD": "it has its own warm-up strategy",
+}
+
+
 class HipsCNNTrainStep:
-    """Graph-captured training step of the demo CNN on the HiPS fabric.
+    """Graph-captured training step of the demo CNN on the HiPS fabric (SGD, Adam, DCASGD, NAG, Signum, RMSProp, AdaGrad, AdaDelta, Ftrl).
 
     Parameters
     ----------
     net : Gluon network from :func:`build_cnn` (initialised; its parameters are re-homed into the symmetric arena so
           ``net(x)`` / ``save_parameters`` keep working on the live weights) or ``None`` (Xavier init here).
     batch_size : per-worker batch (reference default 32).
-    optimizer : ``mx.optimizer.Optimizer`` with a native spec (Adam / SGD / DCASGD) — runs on the global-PS shard.  Honoured in full:
+    optimizer : ``mx.optimizer.Optimizer`` with a native spec — SGD, Adam, DCASGD, NAG, Signum, RMSProp (``centered=False``), AdaGrad,
+          AdaDelta or Ftrl — runs on the global-PS shard (or on every worker with local updates).  Centered RMSProp, FTML, Nadam, Adamax,
+          SGLD and LBSGD raise ``ValueError`` with the reason.  Honoured in full:
           its ``lr_scheduler`` (Factor / MultiFactor / Poly / Cosine, with warm-up) is evaluated by the update kernels from the device step
           count, so every replay of the captured step takes the scheduled rate; per-key ``lr_mult`` / ``wd_mult`` (from ``net``'s
           Parameters, else the optimizer's tables) scale each key's update; the step count starts at ``begin_num_update``.  An optimizer
@@ -260,7 +274,9 @@ class HipsCNNTrainStep:
         optimizer = optimizer or opt.Adam(learning_rate=0.01)
         spec = optimizer.spec()
         if spec is None:
-            raise ValueError("optimizer %s has no native spec; use Adam / SGD / DCASGD" % type(optimizer).__name__)
+            name = type(optimizer).__name__
+            why = _NOT_NATIVE.get(name + ("(centered=True)" if getattr(optimizer, "centered", False) else ""), "it has no native spec")
+            raise ValueError("optimizer %s cannot run in the update kernels: %s.  Supported: %s" % (name, why, _NATIVE_OPTIMIZERS))
         sched = optimizer.lr_scheduler
         if sched is not None:
             if not hasattr(sched, "device_spec"):
@@ -276,7 +292,7 @@ class HipsCNNTrainStep:
         self._lr = float(spec["lr"])
         self.layout = ArenaLayout.build(list(enumerate(CNN_PARAM_SHAPES)), mults=_key_mults(optimizer, net))
         self._local_spec = spec if self.update == "local" else None
-        self._local_sched = native.pack_schedule(spec["lr_schedule"]) if "lr_schedule" in spec else None   # packed once, for _local_opt
+        self._local_packed = (None, None)      # (spec, OptHyper): _local_opt packs self._local_spec again only when it was replaced
         self.fabric = HipsFabric(self.layout, self.topo, self.device, None if self.update == "local" else spec, use_multicast=use_multicast,
                                  loopback=loopback)
         # the script-level `grad / num_samples`, folded into the push kernel; with local updates the aggregate is also averaged over the workers
@@ -396,7 +412,7 @@ class HipsCNNTrainStep:
         f.load_master_from_param()
         if self.update == "local":
             self.Wl.copy_(f.param.tensor)
-            if self._local_spec["name"] == "dcasgd":
+            if native.OPT_KINDS[self._local_spec["name"]].s1_is_weight:
                 self.s1l.copy_(self.Wl)      # DCASGD's previous weight starts as the initial weight (reference create_state)
         if net is not None:  # re-home the Gluon parameters onto the live arena (zero-copy pull)
             for i, p in enumerate(net.collect_params().values()):
@@ -410,14 +426,14 @@ class HipsCNNTrainStep:
     # ------------------------------------------------------------------------------------------------------------
     def _local_opt(self, grad_tensor, zero=None):
         """update='local': the worker's arena optimizer (spec ``self._local_spec``) applied to ``grad_tensor``; ``zero`` is cleared."""
-        sp, f = self._local_spec, self.fabric
-        clip = sp.get("clip_gradient", -1.0)
-        # HFA applies the optimizer to the worker's own gradient arena, a sum over the batch: the reference's cnn_hfa.py steps the trainer
-        # with `trainer.step(num_samples)`, i.e. rescale_grad / B.  The pulled aggregate of the other local mode is already averaged.
-        rescale = sp["rescale_grad"] / self.B if self.hfa else sp["rescale_grad"]
-        native.arena_opt(sp["name"], self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, f.tile_mult, sp["lr"], sp["wd"], rescale,
-                         -1.0 if clip is None else clip, sp.get("momentum", 0.0), sp.get("beta1", 0.9), sp.get("beta2", 0.999),
-                         sp.get("epsilon", 1e-8), sp.get("lamda", 0.04), self.opt_state, zero, schedule=self._local_sched)
+        sp, h = self._local_packed
+        if sp is not self._local_spec:
+            sp = self._local_spec
+            # HFA applies the optimizer to the worker's own gradient arena, a sum over the batch: the reference's cnn_hfa.py steps the trainer
+            # with `trainer.step(num_samples)`, i.e. rescale_grad / B.  The pulled aggregate of the other local mode is already averaged.
+            h = native.pack_hyper(dict(sp, rescale_grad=sp["rescale_grad"] / self.B) if self.hfa else sp)
+            self._local_packed = (sp, h)
+        native.arena_opt_h(h, self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, self.fabric.tile_mult, self.opt_state, zero)
 
     def _steps(self):
         """The training step of ``self.path`` as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch

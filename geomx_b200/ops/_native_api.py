@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import ctypes
 import math
+from typing import NamedTuple
 
 import torch
 
@@ -413,8 +414,6 @@ def head_fwd_bwd(a, W, bias, label, loss, logits, dW, db, da, dbias_prev, relu_m
 
 
 # --------------------------------------------------------------------------------------------------------------- optimizers
-# optimizer kind codes of the kernels (OptKind in csrc/kernels/optim.cuh)
-OPT_KIND = {"sgd": 0, "adam": 1, "dcasgd": 2}
 
 # learning-rate schedule kinds of the kernels (SchedKind in csrc/kernels/optim.cuh); the dicts come from LRScheduler.device_spec()
 SCHED_KIND = {None: 0, "none": 0, "factor": 1, "multifactor": 2, "poly": 3, "cosine": 4}
@@ -448,6 +447,72 @@ def pack_schedule(sched):
     return s
 
 
+class OptHyper(ctypes.Structure):
+    """Mirror of ``OptHyper`` (csrc/kernels/optim.cuh): the field order is ABI.  :data:`OPT_HYPER_LAYOUT` holds the offsets that optim.cuh
+    pins with static_asserts."""
+    _fields_ = ([(n, ctypes.c_float) for n in ("lr", "wd", "rescale", "clip", "momentum", "beta1", "beta2", "eps", "lamda", "wd_lh",
+                                               "clip_weights", "gamma1", "rho", "beta", "lamda1")]
+                + [("kind", ctypes.c_int), ("sched", LrSchedule)])
+
+
+OPT_HYPER_LAYOUT = dict(wd_lh=36, lamda1=56, kind=60, sched=64, size=172, sched_size=108)
+assert all(getattr(OptHyper, k).offset == v for k, v in OPT_HYPER_LAYOUT.items() if k not in ("size", "sched_size"))
+assert ctypes.sizeof(OptHyper) == OPT_HYPER_LAYOUT["size"] and ctypes.sizeof(LrSchedule) == OPT_HYPER_LAYOUT["sched_size"]
+
+
+class OptKindInfo(NamedTuple):
+    code: int               # OptKind in csrc/kernels/optim.cuh
+    fields: tuple           # (OptHyper field, spec() key, default) of the kind's own hyper-parameters
+    clip_zero_off: bool     # clip_gradient 0 means "no clipping": the reference passes the clip to the operator only when it is truthy
+    s1_is_weight: bool      # the state slot s1 starts as the weight (DCASGD's previous weight); every other state starts at 0
+
+
+# The optimizers the update kernels run, by ``Optimizer.spec()['name']``.  The state slots of a kind, and how its class's create_state()
+# lays them out, are the same thing (state_slots): sgd / nag / signum: mom (None without momentum); adam: (m, v); dcasgd: (mom or None,
+# previous weight); rmsprop: (n,); adagrad: history; adadelta: (acc_g, acc_delta); ftrl: (z, n).
+_MOM = (("momentum", "momentum", 0.0),)
+OPT_KINDS = {
+    "sgd": OptKindInfo(0, _MOM, False, False),
+    "adam": OptKindInfo(1, (("beta1", "beta1", 0.9), ("beta2", "beta2", 0.999), ("eps", "epsilon", 1e-8)), False, False),
+    "dcasgd": OptKindInfo(2, _MOM + (("lamda", "lamda", 0.04),), False, True),
+    "nag": OptKindInfo(3, _MOM, False, False),
+    "signum": OptKindInfo(4, _MOM + (("wd_lh", "wd_lh", 0.0),), True, False),
+    "rmsprop": OptKindInfo(5, (("gamma1", "gamma1", 0.9), ("eps", "epsilon", 1e-8), ("clip_weights", "clip_weights", -1.0)), True, False),
+    "adagrad": OptKindInfo(6, (("eps", "epsilon", 1e-7),), False, False),
+    "adadelta": OptKindInfo(7, (("rho", "rho", 0.9), ("eps", "epsilon", 1e-5)), False, False),
+    "ftrl": OptKindInfo(8, (("beta", "beta", 1.0), ("lamda1", "lamda1", 0.01)), True, False),
+}
+OPT_KIND = {k: v.code for k, v in OPT_KINDS.items()}
+
+
+def pack_hyper(spec):
+    """``Optimizer.spec()`` dict -> :class:`OptHyper`, the kernels' view of it (its ``lr_schedule``, if any, included).  ``None``: no
+    optimizer (the fabric stores the aggregated gradient)."""
+    h = OptHyper()
+    if spec is None:
+        h.kind, h.lr, h.clip, h.rescale = -1, 0.0, -1.0, 1.0
+        return h
+    info = OPT_KINDS[spec["name"]]
+    clip = spec.get("clip_gradient", -1.0)
+    if clip is None or (info.clip_zero_off and not clip):
+        clip = -1.0
+    h.kind = info.code
+    h.lr, h.wd, h.rescale, h.clip = spec["lr"], spec["wd"], spec["rescale_grad"], clip
+    for field, key, default in info.fields:
+        setattr(h, field, spec.get(key, default))
+    h.sched = pack_schedule(spec.get("lr_schedule"))
+    return h
+
+
+def state_slots(state):
+    """The tensors ``(s0, s1)`` (None: no such slot) of an optimizer state as ``create_state`` of a native kind returns it."""
+    from ..ndarray import NDArray
+    if state is None or isinstance(state, NDArray):
+        state = (state,)
+    state = tuple(state) + (None,) * (2 - len(state))
+    return tuple(None if s is None else s._t for s in state)
+
+
 def arena_opt(kind, w, g, s0, s1, n, tile_mult, lr, wd, rescale, clip, momentum, b1, b2, eps, lamda, step_state, g_zero=None, schedule=None):
     """Fused arena optimizer; ``lr`` is the base lr of ``schedule`` (an ``LRScheduler.device_spec()`` dict, or an :class:`LrSchedule` that
     :func:`pack_schedule` made from one), which the kernel evaluates at the device step count ``step_state[0] + 1``; ``schedule=None``:
@@ -464,6 +529,17 @@ def single_opt(kind, w, g, s0, s1, lr_t, wd, rescale, clip, momentum=0.0, b1=0.9
         "single_opt")
 
 
+def arena_opt_h(hyper, w, g, s0, s1, n, tile_mult, step_state, g_zero=None):
+    """:func:`arena_opt` for any kind of :data:`OPT_KINDS`: ``hyper`` is the :class:`OptHyper` that :func:`pack_hyper` made from a spec."""
+    _ck(_lib().gx_arena_opt_h(ctypes.byref(hyper), _p(w), _p(g), _p(s0), _p(s1), n, _p(tile_mult), _p(step_state), _p(g_zero), _s()),
+        "arena_opt")
+
+
+def single_opt_h(hyper, w, g, s0, s1, lr_t):
+    """:func:`single_opt` for any kind; ``lr_t`` is the step's lr (Adam: bias-corrected)."""
+    _ck(_lib().gx_single_opt_h(ctypes.byref(hyper), _p(w), _p(g), _p(s0), _p(s1), w.numel(), lr_t, _s()), "single_opt")
+
+
 def adam_update(w, g, m, v, lr_t, b1, b2, eps, wd, rescale, clip):
     single_opt("adam", w, g.contiguous(), m, v, lr_t, wd, rescale, clip, 0.0, b1, b2, eps)
 
@@ -477,14 +553,10 @@ _mt_cache = {}
 
 
 def multi_tensor_update(optimizer, updater, idxs, ws, gs):
-    """One launch for the whole parameter list (Trainer fused path).  Returns False if this optimizer has no native spec."""
+    """One launch for the whole parameter list (Trainer fused path), for an optimizer whose ``spec()`` names a kind of :data:`OPT_KINDS`."""
     from ..ndarray import NDArray
     spec = optimizer.spec()
     kind = spec["name"]
-    if kind == "sgd" and spec.get("momentum", 0.0) == 0.0:
-        need = 0
-    else:
-        need = 1 if kind == "sgd" else 2
     for i, w in zip(idxs, ws):
         if i not in updater.states:
             updater.states[i] = optimizer.create_state_multi_precision(i, NDArray(w))
@@ -498,12 +570,7 @@ def multi_tensor_update(optimizer, updater, idxs, ws, gs):
     if ent is None:
         arr = (_TensorEntry * len(ws))()
         for j, (i, w, g) in enumerate(zip(idxs, ws, gs)):
-            st = updater.states[i]
-            s0 = s1 = None
-            if need == 1:
-                s0 = st._t
-            elif need == 2:
-                s0, s1 = st[0]._t, st[1]._t
+            s0, s1 = state_slots(updater.states[i])
             p = optimizer.param_dict.get(i)
             arr[j] = _TensorEntry(w.data_ptr(), g.data_ptr(), 0 if s0 is None else s0.data_ptr(), 0 if s1 is None else s1.data_ptr(),
                                   w.numel(), p.lr_mult if p is not None else 1.0, p.wd_mult if p is not None else 1.0)
@@ -514,10 +581,8 @@ def multi_tensor_update(optimizer, updater, idxs, ws, gs):
             _mt_cache.clear()
         _mt_cache[key] = ent
     dev, max_n, cnt = ent
-    clip = -1.0 if optimizer.clip_gradient is None else float(optimizer.clip_gradient)
-    _ck(_lib().gx_multi_tensor_opt(OPT_KIND[kind], _p(dev), cnt, max_n, lr_t, float(optimizer.wd), float(optimizer.rescale_grad), clip,
-                                   float(spec.get("momentum", 0.0)), float(spec.get("beta1", 0.9)), float(spec.get("beta2", 0.999)),
-                                   float(spec.get("epsilon", 1e-8)), float(spec.get("lamda", 0.04)), _s()), "multi_tensor_opt")
+    h = pack_hyper(dict(spec, lr=lr_t))
+    _ck(_lib().gx_multi_tensor_opt_h(ctypes.byref(h), _p(dev), cnt, max_n, lr_t, _s()), "multi_tensor_opt")
     return True
 
 

@@ -52,6 +52,9 @@ SIGS = {
     "gx_arena_opt": [I, P, P, P, P, L, P, F, F, F, F, F, F, F, F, F, P, P, P, P],
     "gx_multi_tensor_opt": [I, P, I, L, F, F, F, F, F, F, F, F, F, P],
     "gx_single_opt": [I, P, P, P, P, L, F, F, F, F, F, F, F, F, F, P],
+    "gx_arena_opt_h": [P, P, P, P, P, L, P, P, P, P],
+    "gx_multi_tensor_opt_h": [P, P, I, L, F, P],
+    "gx_single_opt_h": [P, P, P, P, P, L, F, P],
     "gx_nary_sum": [P, P, I, L, P],
     "gx_scale_cast": [P, I, P, I, F, L, P],
     # compress.cu

@@ -9,7 +9,8 @@ NAG, SGLD, Adam :1017, AdaGrad, RMSProp, AdaDelta, Ftrl, Adamax, Nadam, Test, an
 H100 design: every optimizer also exposes ``spec()`` — a *declarative* description
 (name + hyper-parameters) that the native fused kernels (``csrc/kernels/optim.cu``) and the
 native parameter-server (``csrc/hips/server_optim.h``) execute without Python; the dense
-update of SGD / SGD-momentum / Adam / DCASGD on CUDA tensors goes through those kernels.
+update of SGD / SGD-momentum / Adam / DCASGD on CUDA tensors goes through those kernels; NAG, Signum, RMSProp (not centered),
+AdaGrad, AdaDelta and Ftrl have a spec too, which the training engine, the fabric KVStore and the Trainer's fused update run.
 Arbitrary user optimizers still work everywhere through the Python ``update`` (on servers via
 the host-callback path, like the reference's ``Executor`` hand-off).
 """
@@ -26,6 +27,12 @@ from ..ndarray import NDArray
 __all__ = ["Optimizer", "SGD", "Signum", "FTML", "LBSGD", "DCASGD", "NAG", "SGLD", "ccSGD", "Adam", "AdaGrad",
            "RMSProp", "AdaDelta", "Ftrl", "Adamax", "Nadam", "Test", "Updater", "get_updater", "create",
            "register"]
+
+
+def _on_clip(c):
+    """The clip the reference's RMSProp / Ftrl / Signum apply: they pass ``clip_gradient`` / ``clip_weights`` to the operator only when it
+    is truthy, and the operator clips only when it is >= 0, so None, 0 and negative values all mean "off"."""
+    return c if c and c >= 0 else None
 
 
 def _t(x):
@@ -251,9 +258,18 @@ class LBSGD(SGD):
 
 @register
 class Signum(Optimizer):
+    """``optimizer.py:558-622``: with momentum, signum_update; without, signsgd_update ``w = (1 - lr*wd)*w - lr*sign(grad)`` (decoupled wd,
+    no clip, no wd_lh)."""
+    native_name = "signum"
+
     def __init__(self, learning_rate=0.01, momentum=0.9, wd_lh=0.0, **kwargs):
         super().__init__(learning_rate=learning_rate, **kwargs)
         self.momentum, self.wd_lh = momentum, wd_lh
+
+    def spec(self):
+        if self.momentum < 0:     # the reference runs signum_update with momentum 0 then: no native kind does that
+            return None
+        return self._base_spec(momentum=float(self.momentum), wd_lh=float(self.wd_lh))
 
     def create_state(self, index, weight):
         return NDArray(torch.zeros_like(_t(weight))) if self.momentum != 0.0 else None
@@ -261,12 +277,17 @@ class Signum(Optimizer):
     def update(self, index, weight, grad, state):
         self._update_count(index)
         lr, wd = self._get_lr(index), self._get_wd(index)
-        w = _t(weight); g = self._prep_grad(grad, weight, wd)
+        w = _t(weight)
         if state is not None:
-            m = _t(state); m.mul_(self.momentum).sub_(g, alpha=(1 - self.momentum))
+            # SignumKernel: mom = mu*mom - (1-mu)*wd*w - (1-mu)*clip(rescale*g); w = (1 - lr*wd_lh)*w + lr*sign(mom)
+            mu, clip = (self.momentum if self.momentum > 0 else 0.0), _on_clip(self.clip_gradient)
+            g = _t(grad).to(w.dtype) * self.rescale_grad
+            if clip is not None:
+                g = g.clamp(-clip, clip)
+            m = _t(state); m.mul_(mu).sub_(g + wd * w, alpha=(1 - mu))
             w.mul_(1 - lr * self.wd_lh).add_(torch.sign(m), alpha=lr)
         else:
-            w.mul_(1 - lr * self.wd_lh).sub_(torch.sign(g), alpha=lr)
+            w.mul_(1 - lr * wd).sub_(torch.sign(_t(grad)).to(w.dtype), alpha=lr)
 
 
 @register
@@ -327,8 +348,14 @@ class DCASGD(Optimizer):
 
 @register
 class NAG(Optimizer):
+    """``optimizer.py:928-978``: rescale, clip, ``+ wd*w``; ``mom = mu*mom + g``, ``w -= lr*(g + mu*mom)``."""
+    native_name = "nag"
+
     def __init__(self, momentum=0.0, **kwargs):
         super().__init__(**kwargs); self.momentum = momentum
+
+    def spec(self):
+        return self._base_spec(momentum=float(self.momentum))
 
     def create_state(self, index, weight):
         return NDArray(torch.zeros_like(_t(weight))) if self.momentum != 0.0 else None
@@ -389,8 +416,14 @@ class Adam(Optimizer):
 
 @register
 class AdaGrad(Optimizer):
+    """``optimizer.py:1099-1155`` (dense): rescale, clip; ``history += g^2``; ``w += (g / sqrt(history + eps) + wd*w) * -lr``."""
+    native_name = "adagrad"
+
     def __init__(self, eps=1e-7, **kwargs):
         super().__init__(**kwargs); self.float_stable_eps = eps
+
+    def spec(self):
+        return self._base_spec(epsilon=float(self.float_stable_eps))
 
     def create_state(self, index, weight):
         return NDArray(torch.zeros_like(_t(weight)))
@@ -405,10 +438,20 @@ class AdaGrad(Optimizer):
 
 @register
 class RMSProp(Optimizer):
+    """``optimizer.py:1158-1233``, rmsprop_update / rmspropalex_update: ``g = rescale*g + wd*w``, then clip; ``eps`` inside the square
+    root; ``clip_weights`` clamps the new weight.  Only the plain form (``centered=False``) has a native spec."""
+    native_name = "rmsprop"
+
     def __init__(self, learning_rate=0.001, gamma1=0.9, gamma2=0.9, epsilon=1e-8, centered=False,
                  clip_weights=None, **kwargs):
         super().__init__(learning_rate=learning_rate, **kwargs)
         self.gamma1, self.gamma2, self.centered, self.epsilon, self.clip_weights = gamma1, gamma2, centered, epsilon, clip_weights
+
+    def spec(self):
+        if self.centered:
+            return None
+        cw = _on_clip(self.clip_weights)
+        return self._base_spec(gamma1=float(self.gamma1), epsilon=float(self.epsilon), clip_weights=-1.0 if cw is None else float(cw))
 
     def create_state(self, index, weight):
         z = lambda: NDArray(torch.zeros_like(_t(weight)))
@@ -417,7 +460,11 @@ class RMSProp(Optimizer):
     def update(self, index, weight, grad, state):
         self._update_count(index)
         lr, wd = self._get_lr(index), self._get_wd(index)
-        w = _t(weight); g = self._prep_grad(grad, weight, wd)
+        w = _t(weight)
+        g = _t(grad).to(w.dtype) * self.rescale_grad + wd * w
+        clip = _on_clip(self.clip_gradient)
+        if clip is not None:
+            g = g.clamp(-clip, clip)
         if not self.centered:
             n = _t(state[0]); n.mul_(self.gamma1).addcmul_(g, g, value=1 - self.gamma1)
             w.sub_(lr * g / torch.sqrt(n + self.epsilon))
@@ -427,14 +474,21 @@ class RMSProp(Optimizer):
             gm.mul_(self.gamma1).add_(g, alpha=1 - self.gamma1)
             delta.mul_(self.gamma2).sub_(lr * g / torch.sqrt(n - gm * gm + self.epsilon))
             w.add_(delta)
-        if self.clip_weights:
-            w.clamp_(-self.clip_weights, self.clip_weights)
+        cw = _on_clip(self.clip_weights)
+        if cw is not None:
+            w.clamp_(-cw, cw)
 
 
 @register
 class AdaDelta(Optimizer):
+    """``optimizer.py:1236-1289``: no learning rate (nor its schedule or lr_mult); rescale, clip; wd outside: ``w -= delta + wd*w``."""
+    native_name = "adadelta"
+
     def __init__(self, rho=0.90, epsilon=1e-5, **kwargs):
         super().__init__(**kwargs); self.rho, self.epsilon = rho, epsilon
+
+    def spec(self):
+        return self._base_spec(rho=float(self.rho), epsilon=float(self.epsilon))
 
     def create_state(self, index, weight):
         z = lambda: NDArray(torch.zeros_like(_t(weight)))
@@ -453,8 +507,14 @@ class AdaDelta(Optimizer):
 
 @register
 class Ftrl(Optimizer):
+    """``optimizer.py:1294-1366``, ftrl_update: the weight is recomputed from ``z`` and ``n`` on every update."""
+    native_name = "ftrl"
+
     def __init__(self, lamda1=0.01, learning_rate=0.1, beta=1, **kwargs):
         super().__init__(learning_rate=learning_rate, **kwargs); self.lamda1, self.beta = lamda1, beta
+
+    def spec(self):
+        return self._base_spec(lamda1=float(self.lamda1), beta=float(self.beta))
 
     def create_state(self, index, weight):
         z = lambda: NDArray(torch.zeros_like(_t(weight)))
@@ -463,7 +523,11 @@ class Ftrl(Optimizer):
     def update(self, index, weight, grad, state):
         self._update_count(index)
         lr, wd = self._get_lr(index), self._get_wd(index)
-        w = _t(weight); g = self._prep_grad(grad)
+        w = _t(weight)
+        g = _t(grad).to(w.dtype) * self.rescale_grad
+        clip = _on_clip(self.clip_gradient)
+        if clip is not None:
+            g = g.clamp(-clip, clip)
         z, n = map(_t, state)
         z.add_(g - (torch.sqrt(n + g * g) - torch.sqrt(n)) * w / lr)
         n.addcmul_(g, g)

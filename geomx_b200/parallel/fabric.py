@@ -19,7 +19,7 @@ import torch
 
 from ..base import MXNetError, getenv_int
 from ..ops import native
-from ..ops._native_api import OPT_KIND, LrSchedule, pack_schedule
+from ..ops._native_api import OPT_KINDS, OptHyper, pack_hyper
 from .arena import ArenaLayout
 
 MAX_RANKS = 16
@@ -174,9 +174,7 @@ class SymmetricHeap:
 
 
 # ------------------------------------------------------------------------------------------------------------ kernel parameter block
-class _OptHyperF(ctypes.Structure):
-    _fields_ = ([(n, ctypes.c_float) for n in ("lr", "wd", "rescale", "clip", "momentum", "beta1", "beta2", "eps", "lamda")]
-                + [("kind", ctypes.c_int), ("sched", LrSchedule)])
+_OptHyperF = OptHyper      # the optimizer block inside _FabricParams (one definition, in ops/_native_api.py)
 
 
 class _FabricParams(ctypes.Structure):
@@ -202,7 +200,9 @@ class _FabricParams(ctypes.Structure):
     ]
 
 
-_KIND = {**OPT_KIND, None: -1, "none": -1}   # -1: no server optimizer, the kernels store the aggregated gradient
+# the block is passed by value as a kernel parameter, and CUDA limits those to 4 KB.  hips_ll.cuh static_asserts the same size and offset.
+FABRIC_PARAMS_BYTES, FABRIC_PARAMS_H_OFFSET = 1656, 728
+assert ctypes.sizeof(_FabricParams) == FABRIC_PARAMS_BYTES <= 4096 and _FabricParams.h.offset == FABRIC_PARAMS_H_OFFSET
 
 
 def dgt_num_important(sorted_contrib, k, adaptive=False, k_min=0.2):
@@ -403,22 +403,13 @@ class HipsFabric:
     def init_dcasgd_previous_weight(self):
         """DCASGD's previous weight (state slot ``s1``) starts as the current master weight, as the reference's ``create_state`` makes it
         (``(mom, weight.copy())``); a zero start would add ``lamda * g^2 * w`` to the first update."""
-        if self.opt_spec is not None and self.opt_spec.get("name") == "dcasgd":
+        if self.opt_spec is not None and OPT_KINDS[self.opt_spec["name"]].s1_is_weight:
             self.s1.copy_(self.w)
 
     # -- parameter block ------------------------------------------------------------------------------------------------
     def _hyper(self):
-        h = _OptHyperF()
-        s = self.opt_spec
-        if s is None:
-            h.kind = -1; h.lr = 0.0; h.clip = -1.0; h.rescale = 1.0
-            return h
-        h.kind = _KIND[s["name"]]
-        h.lr, h.wd, h.rescale, h.clip = s["lr"], s["wd"], s["rescale_grad"], s["clip_gradient"]
-        h.momentum = s.get("momentum", 0.0); h.beta1 = s.get("beta1", 0.9); h.beta2 = s.get("beta2", 0.999)
-        h.eps = s.get("epsilon", 1e-8); h.lamda = s.get("lamda", 0.04)
-        h.sched = pack_schedule(s.get("lr_schedule"))      # evaluated by the kernels at their step count; absent: constant lr
-        return h
+        # the schedule, if any, is evaluated by the kernels at their step count; without one the lr is constant
+        return pack_hyper(self.opt_spec)
 
     def _block(self, channel, masked=False, zero_grad=False):
         if channel in self.channels:

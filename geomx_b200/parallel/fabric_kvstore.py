@@ -11,7 +11,8 @@ Selected by ``kvstore.dist.create_dist`` when the process was started by ``torch
                key; keys that were not pushed this round are masked out (``tile_active``).  When the script passes priorities
                (``priority=-idx``, examples/cnn.py:121-125) — or sets ``ENABLE_P3=1`` — the kernel walks the tiles of high-priority keys first
                (``tile_order``), which is what P3 / the engine's priority queue achieve on the TCP path.
-* optimizers — Adam / SGD / DCASGD specs run natively on the global-PS shard inside the exchange kernel; any other ``mx.optimizer`` object
+* optimizers — the specs of SGD / Adam / DCASGD / NAG / Signum / RMSProp / AdaGrad / AdaDelta / Ftrl run natively on the global-PS shard
+               inside the exchange kernel; any other ``mx.optimizer`` object
                (or one with an lr_scheduler / per-parameter multipliers) is executed by the Python updater on the aggregated gradient, identically
                on every rank — the same arithmetic the reference's server-side pickled optimizer performs (kvstore.py:452-499).
 * TSEngine   — ``ENABLE_INTRA_TS`` / ``ENABLE_INTER_TS`` select an overlay for heterogeneous TCP links; NVSwitch is uniform, so they are
