@@ -619,6 +619,7 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
     const int t7 = j < 7 ? j : j < 14 ? 42 + (j - 7) : j < 19 ? (j - 13) * 7 : (j - 18) * 7 + 6;
     reinterpret_cast<float2*>(swt)[plane * 49 + t7] = make_float2(0.f, 0.f);
   }
+  stamp(25);
   for (int i = tid; i < CD_H * CD_H / 4; i += 288) cpa16(sx + 4 * i, x + (long long)b * CD_H * CD_H + 4 * i);
   for (int i = tid; i < 4 * 144 / 4; i += 288) cpa16(sa1 + 4 * i, a1 + ((long long)b * CD_C1 + 4 * cg) * 144 + 4 * i);
   for (int i = tid; i < 4 * 144; i += 288) {
@@ -626,6 +627,7 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
     const int win = i % 144, id = idx1[o];
     spos[i] = (2 * (win / CD_P1) + (id >> 1)) * CD_H + 2 * (win % CD_P1) + (id & 1);
   }
+  stamp(26);
   // where dz2 can be non-zero (a2 > 0, at the arg-max idx2) is known from the forward pass: one warp per pooling window lists its output
   // channels in ascending order, with the weight offset that places the arg-max pixel; only the values (da2) wait for the grid dependency
   {
@@ -645,6 +647,7 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
     list(wa, ava, ida);
     if (wb < 16) list(wb, avb, idb);
   }
+  stamp(27);
   cpa_wait_all();
   __syncthreads();
   stamp(9);
@@ -709,6 +712,7 @@ __device__ __forceinline__ void cnn_bwd_body(float* sm, const int b, const int c
     float acc = 0.f;
     for (int p = 0; p < 144; ++p) acc += sda1[cl * 144 + p];
     atomicAdd(db0 + 4 * cg + cl, acc);
+    if (dbg != nullptr && b == 0 && cg == 0 && cl == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[28] = t; }
   }
   stamp(13);
 }
@@ -950,7 +954,7 @@ __global__ void __launch_bounds__(288) cnn_bwd_exchange_kernel(const float* x, c
 
 using namespace gx;
 
-static unsigned long long* g_cnn_dbg = nullptr;      // optional %globaltimer stamps of CTA (0,0): fwd 0-6, bwd 8-13, wgrad1 16-18
+static unsigned long long* g_cnn_dbg = nullptr;      // optional %globaltimer stamps of CTA (0,0): fwd 0-6, bwd 8-13 and 25-28, wgrad1 16-18
 GX_API int gx_cnn_set_debug(unsigned long long* p) { g_cnn_dbg = p; return 0; }
 
 // x [B,1,28,28]; w0 [16,1,5,5]; w1 [32,16,5,5]; writes a1 [B,16,12,12] + idx1, a2 [B,32,4,4] + idx2

@@ -26,7 +26,8 @@
 // dense0 is row-separable (a3[b] needs only the pooled conv output of image b), so where the direct forward kernel runs (even batches <= 32)
 // it computes a3 on its 128 SMs (cnn_fwd_dense0_kernel, cnn_direct.cu) and the cluster kernel is dense_tail_kernel: the same chain from a3
 // on, through the same body (dense_chain_body), with no x tile, no dense0 phase and no a3 hand-off.  In the classic training step the
-// forward kernel also computes everything down to dz3 (all of it row-separable), and dense_tail_kernel runs from dz3: P5 (dx) only.
+// forward kernel also computes everything down to dz3 (all of it row-separable), and dense_tail_kernel runs from dz3: P5 (dx) only, over
+// one cluster per four batch rows (dense_dx_rows).
 //
 // Shapes are compile-time (D0 -> D1 -> D2 -> C<=16, batch <= 32): the demo CNN's 512 -> 256 -> 128 -> 10.  Other shapes use the wgmma GEMMs.
 #include <cooperative_groups.h>
@@ -41,6 +42,7 @@ constexpr int MC_THREADS = 512;   // 16 warps
 constexpr int MC_HALF = 256;      // warp-group 0: dense1, the logits and dz3
 constexpr int MC_B = 32;      // batch rows held (rows >= B are zero)
 constexpr int MC_CMAX = 16;   // classes (padded)
+constexpr int DX_THREADS = 128;   // dense_tail_kernel from dz3: threads per CTA
 
 struct MlpChainParams {
   const float* x;       // [B][D0]   input activations (flattened pooled conv output)
@@ -242,6 +244,9 @@ struct TailSmem {
   static constexpr int BAR = SCRATCH + SCRATCH_SZ;             // 2 mbarriers: a4, dz3 landed
   static constexpr int TOTAL = BAR + 2 * 2;
   static constexpr int BYTES = TOTAL * 4;
+  // from dz3 (dense_dx_rows): the W0 column slice [D1][KS0], DX_ROWS rows of dz3 and the partial sums of the K splits
+  static constexpr int DX_ROWS = 4, DX_KS = DX_THREADS / KS0;
+  static constexpr int DX_BYTES = (D1 * KS0 + DX_ROWS * D1 + DX_KS * DX_ROWS * KS0) * 4;
 };
 // the tail's CTAs stage their weights on the SMs beside the forward kernel's CTAs (one each: 256 x 64 + 512 x 96 = 65,536 registers), so
 // both kernels' shared memory, with the 1 KB the runtime reserves per CTA, has to fit into the SM's 228 KB
@@ -263,6 +268,61 @@ __device__ __forceinline__ void dense_dx(float* sm, const MlpChainParams& p, con
   for (int e = tid; e < MC_B * KS0 / 4; e += MC_THREADS) {
     const int b = e / (KS0 / 4), n4 = e % (KS0 / 4);
     if (b < p.B) *reinterpret_cast<float4*>(p.dx + (long long)b * D0 + cr * KS0 + 4 * n4) = sum_partials<KS0, KS>(scratch, b, n4);
+  }
+  stamp(9);
+}
+
+// dense_tail_kernel from dz3: dx = dz3 W0, one DX_ROWS x KS0 tile per CTA.  The kernel runs over ceil(B / DX_ROWS) clusters: cluster g takes
+// rows [g DX_ROWS, (g + 1) DX_ROWS), rank cr the columns of its W0 slice, so that da2 is computed on up to 128 SMs instead of one cluster's.
+// DX_THREADS threads (the tail's 512 would hold 49 K registers on every SM the grid lands on, where the convolution backward grid that
+// follows becomes resident).  The W0 slice is staged before the grid dependency, only the tile's dz3 rows after it.  Thread -> column
+// n = tid % KS0 and K split ks = tid / KS0, one fmaf chain per row over its K range; the splits are added in ascending order, so that
+// two launches give the same bits.
+template <class L, int D0, int D1, int CS, class Stamp>
+__device__ __forceinline__ void dense_dx_rows(float* sm, const MlpChainParams& p, const int cr, Stamp&& stamp) {
+  constexpr int R = L::DX_ROWS, KS0 = L::KS0, KS = L::DX_KS, KL = D1 / KS;
+  static_assert(DX_THREADS % KS0 == 0 && KL % 4 == 0, "dx tile splits");
+  float* sW = sm; float* sZ = sW + D1 * KS0; float* sP = sZ + R * D1;
+  const int tid = threadIdx.x, row0 = (blockIdx.x / CS) * R;
+  for (int c = tid; c < D1 * (KS0 / 4); c += DX_THREADS) {
+    const int r = c / (KS0 / 4), q = c - r * (KS0 / 4);
+    cp_async16(sW + r * KS0 + 4 * q, p.w0 + (long long)r * D0 + cr * KS0 + 4 * q);
+  }
+  cp_async_commit();
+  stamp(1);
+  pdl_wait();
+  pdl_launch();
+  stamp(2);
+  for (int c = tid; c < R * (D1 / 4); c += DX_THREADS) {
+    const int r = c / (D1 / 4), q = c - r * (D1 / 4);
+    if (row0 + r < p.B) cp_async16(sZ + r * D1 + 4 * q, p.dz3 + (long long)(row0 + r) * D1 + 4 * q);
+    else *reinterpret_cast<float4*>(sZ + r * D1 + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncthreads();
+  stamp(3);
+  const int n = tid % KS0, ks = tid / KS0;
+  float acc[R] = {};
+#pragma unroll 2
+  for (int k = ks * KL; k < (ks + 1) * KL; k += 4) {
+    const float w[4] = {sW[k * KS0 + n], sW[(k + 1) * KS0 + n], sW[(k + 2) * KS0 + n], sW[(k + 3) * KS0 + n]};
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const float4 z = *reinterpret_cast<const float4*>(sZ + r * D1 + k);
+      acc[r] = fmaf(z.x, w[0], acc[r]); acc[r] = fmaf(z.y, w[1], acc[r]); acc[r] = fmaf(z.z, w[2], acc[r]); acc[r] = fmaf(z.w, w[3], acc[r]);
+    }
+  }
+  stamp(14);
+#pragma unroll
+  for (int r = 0; r < R; ++r) sP[(ks * R + r) * KS0 + n] = acc[r];
+  __syncthreads();
+  for (int e = tid; e < R * KS0; e += DX_THREADS) {
+    const int r = e / KS0, c = e - r * KS0;
+    float s = sP[e];
+#pragma unroll
+    for (int k = 1; k < KS; ++k) s += sP[k * R * KS0 + e];
+    if (row0 + r < p.B) p.dx[(long long)(row0 + r) * D0 + cr * KS0 + c] = s;
   }
   stamp(9);
 }
@@ -524,28 +584,11 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dens
   const int tid = threadIdx.x;
   const int B = p.B, C = p.C;
   auto stamp = [&](int slot) {
-    if (p.dbg != nullptr && cr == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
+    if (p.dbg != nullptr && blockIdx.x == 0 && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); p.dbg[slot] = t; }
   };
   stamp(0);
-  if (p.from_dz3) {
-    // dx = dz3 W0 only: the W0 column slice before the grid dependency, then dz3 (rows >= B zero) into the buffer P5 reads.  Nothing is
-    // exchanged between the CTAs in this mode.
-    stage_plain_async(sW0, p.w0 + cr * L::KS0, D1, L::KS0, D0);
-    cp_async_commit();
-    stamp(1);
-    pdl_wait();
-    pdl_launch();
-    stamp(2);
-    for (int c = tid; c < MC_B * (D1 >> 2); c += MC_THREADS) {
-      const int r = c / (D1 >> 2), q = c - r * (D1 >> 2);
-      if (r < B) cp_async16(sA3 + sw_off(r, q << 2, D1), p.dz3 + (long long)r * D1 + (q << 2));
-      else *reinterpret_cast<float4*>(sA3 + sw_off(r, q << 2, D1)) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncthreads();
-    stamp(3);
-    dense_dx<L, D0, D1>(sm, p, cr, stamp);
+  if (p.from_dz3) {     // dx = dz3 W0 only, nothing exchanged between the CTAs
+    dense_dx_rows<L, D0, D1, CS>(sm, p, cr, stamp);
     return;
   }
   if (tid == 0) {
@@ -658,8 +701,13 @@ static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
   if (ready < 0) return -2;
   static int use_pdl = -1;
   if (use_pdl < 0) { const char* e = getenv("GEOMX_MLP_PDL"); use_pdl = (e && e[0] == '0') ? 0 : 1; }
-  if (use_pdl) launch_pdl(kern, dim3(CS), dim3(MC_THREADS), (size_t)BYTES, stream, p);
-  else kern<<<dim3(CS), dim3(MC_THREADS), (size_t)BYTES, stream>>>(p);
+  // dense_tail_kernel from dz3 (dense_dx_rows): one cluster per DX_ROWS rows, DX_THREADS threads, only the smem that mode uses
+  using T = TailSmem<512, 256, 128, CS>;
+  const bool dx_only = TAIL && p.from_dz3;
+  const dim3 grid(dx_only ? CS * ((p.B + T::DX_ROWS - 1) / T::DX_ROWS) : CS), block(dx_only ? DX_THREADS : MC_THREADS);
+  const size_t smem = dx_only ? (size_t)T::DX_BYTES : (size_t)BYTES;
+  if (use_pdl) launch_pdl(kern, grid, block, smem, stream, p);
+  else kern<<<grid, block, smem, stream>>>(p);
   return GX_CHECK_LAUNCH();
 }
 // cluster of 16 CTAs (one GPC) halves every slice; fall back to the portable size 8 when the device cannot co-schedule 16

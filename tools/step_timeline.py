@@ -21,9 +21,11 @@ from geomx_b200.parallel import Topology  # noqa: E402
 
 # in-kernel %globaltimer stamps of the direct-convolution kernels (gx_cnn_set_debug slots, written by the first CTA of each body).  The
 # forward kernel that also computes dense0 (even batches <= 32) stamps 5 a2 landed | 6 a3 stored before its end (4).
-CNN_PHASES = {"cnn_fwd": (0, 1, 2, 3, 4), "cnn_bwd": (8, 9, 10, 11, 12, 13), "cnn_wgrad1": (16, 17, 18)}
+# The data-gradient body splits its staging: 25 W1 issued | 26 x, a1, idx1 issued | 27 list ballots done | 9 staging landed; 28 is the end
+# of its db0 thread (shown relative to 13, the end of thread 0's conv0 weight gradient).
+CNN_PHASES = {"cnn_fwd": (0, 1, 2, 3, 4), "cnn_bwd": (8, 25, 26, 27, 9, 10, 11, 12, 13, 28), "cnn_wgrad1": (16, 17, 18)}
 CNN_PHASE_LABELS = {"cnn_fwd": ("staging", "conv0", "conv1", "epilogue"),
-                    "cnn_bwd": ("staging", "pdl-wait+dz2", "dgrad", "routing", "wgrad0"),
+                    "cnn_bwd": ("W1 issued", "x/a1/idx1", "ballots", "landed", "pdl-wait+dz2", "dgrad", "routing", "wgrad0", "db0 thread end"),
                     "cnn_wgrad1": ("staging+pdl-wait", "wgrad1")}
 FWD_DENSE0_PHASES, FWD_DENSE0_LABELS = (0, 1, 2, 3, 5, 6), ("staging", "conv0", "conv1", "a2 landed", "dense0 -> a3 stored")
 # with its training head (the classic step) it goes on: 7 a3 landed | 14 a4 landed | 15 dz3 stored
@@ -36,8 +38,9 @@ MLP_PHASES = (0, 3, 4, 5, 6, 7, 8, 9)
 MLP_PHASE_LABELS = ("staging+pdl-wait", "dense0 -> a3", "dense1 -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
 TAIL_PHASES = (0, 3, 5, 6, 7, 8, 9)
 TAIL_PHASE_LABELS = ("staging+pdl-wait", "a3 staged -> a4", "head -> dz4", "dz3 pushed", "dz3 landed", "da2")
-# ... and from dz3 (after the forward kernel's training head): 0 start | 3 dz3 staged | 9 end (da2 stored)
-TAIL_DZ3_PHASES, TAIL_DZ3_LABELS = (0, 3, 9), ("staging+pdl-wait+dz3 staged", "dz3 staged -> da2")
+# ... and from dz3 (after the forward kernel's training head): 0 start | 1 W0 issued | 2 grid dependency resolved | 3 dz3 staged | 14 product done |
+# 9 end (da2 stored)
+TAIL_DZ3_PHASES, TAIL_DZ3_LABELS = (0, 1, 2, 3, 14, 9), ("W0 issued", "pdl-wait", "dz3 staged", "da2 product", "da2 stored")
 
 
 def main():
