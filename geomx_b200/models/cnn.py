@@ -42,6 +42,7 @@ import copy
 import os
 from typing import NamedTuple
 
+import numpy as np
 import torch
 
 from .. import gluon, initializer
@@ -54,6 +55,12 @@ from ..parallel.fabric import HipsFabric, Topology
 __all__ = ["build_cnn", "CNN_PARAM_SHAPES", "HipsCNNTrainStep", "StepPath", "step_path", "STEP_SWITCHES"]
 
 CNN_PARAM_SHAPES = [(16, 1, 5, 5), (16,), (32, 16, 5, 5), (32,), (256, 512), (256,), (128, 256), (128,), (10, 128), (10,)]
+# the structural names that ``net.save_parameters`` gives the parameters of build_cnn() (the index of the layer in the Sequential)
+CNN_PARAM_NAMES = ["0.weight", "0.bias", "2.weight", "2.bias", "4.weight", "4.bias", "5.weight", "5.bias", "6.weight", "6.bias"]
+# version of the file that HipsCNNTrainStep.save_states writes
+CHECKPOINT_VERSION = 1
+# checkpoint meta fields that must equal the loading engine's: the optimizer kind, update mode, sync mode and the accelerator set
+_MUST_MATCH = ("meta:opt_kind", "meta:update", "meta:mode", "meta:hfa", "meta:wire_formats", "meta:bsc_threshold", "meta:dgt")
 
 # The environment variables that select the training step's kernel path; HipsCNNTrainStep reads them once, when it is constructed.
 STEP_SWITCHES = ("GEOMX_STEP_OVERLAP", "GEOMX_STEP_EXCHANGE", "GEOMX_FUSED_MLP", "GEOMX_DIRECT_CONV", "GEOMX_CNN_BWD_ONE_LAUNCH",
@@ -153,6 +160,21 @@ def build_cnn():
     return net
 
 
+def _pack(arrays):
+    """The bytes of ``arrays``, one after the other (one broadcast of a whole checkpoint)."""
+    return np.concatenate([np.ascontiguousarray(a).reshape(-1).view(np.uint8) for a in arrays])
+
+
+def _unpack(buf, layout):
+    """Inverse of :func:`_pack`: ``layout`` lists (name, shape, dtype) in packing order; returns name -> array."""
+    out, o = {}, 0
+    for name, shape, dt in layout:
+        n = int(np.prod(shape)) * np.dtype(dt).itemsize
+        out[name] = buf[o:o + n].view(dt).reshape(shape).copy()
+        o += n
+    return out
+
+
 class LossHandle:
     """Result of ``HipsCNNTrainStep.step_async``: the per-sample losses of one step in pinned host memory + the event that guards them."""
 
@@ -244,6 +266,9 @@ class HipsCNNTrainStep:
           whose schedule cannot run on the device (any other scheduler, or a subclass that changes a schedule's values) raises
           ``ValueError`` here.  ``set_learning_rate`` changes a constant rate between steps; ``learning_rate`` is the rate of the next update.
     topo : :class:`Topology` (default: from ``WORLD_SIZE`` / ``RANK`` / ``GEOMX_NUM_PARTIES`` / ``DMLC_NUM_GLOBAL_SERVER``).
+
+    ``save_states`` / ``load_states`` checkpoint and resume the whole training state (one ``mx.nd.save`` file, keyed by parameter, so a
+    run may resume with another batch size or number of ranks).
     """
 
     def __init__(self, net=None, batch_size=32, optimizer=None, topo=None, device=None, use_graph=True,
@@ -306,6 +331,7 @@ class HipsCNNTrainStep:
             fmts = {i: ("fp8" if wire_dtype == "fp8" else "fp16") for i, sl in enumerate(self.layout.slots) if sl.numel >= bound}
         if bsc_threshold and self.fabric.protocol == "ll":
             fmts.update({i: "bsc" for i, sl in enumerate(self.layout.slots) if sl.numel >= lower})
+        self._bsc_threshold = float(bsc_threshold or 0.01) if "bsc" in fmts.values() else 0.0
         if fmts:
             self.fabric.set_wire_formats(fmts, bsc_threshold=float(bsc_threshold or 0.01))
         self._dgt_every = 0
@@ -667,6 +693,289 @@ class HipsCNNTrainStep:
         self._primed = False
         self.steps_done += 1
         return float(self.loss.mean())
+
+    # checkpoints -----------------------------------------------------------------------------------------------------
+    def save_states(self, fname):
+        """Save the whole training state to ``fname``, as ``gluon.Trainer.save_states`` does for the generic path: waits for the steps
+        already enqueued and writes the state after the last completed update.  One ``mx.nd.save`` file (the ``.params`` format, no
+        pickle): the live weights under the names ``net.save_parameters`` writes for :func:`build_cnn` (so
+        ``build_cnn().load_parameters(fname, ignore_extra=True)`` loads them), and per parameter ``master:`` / ``s0:`` / ``s1:`` /
+        ``step:`` (the master weight, both optimizer state slots and the update count: one per key, one per tile with ``dist_async``; with
+        ``update='local'`` the worker's own), ``bsc_u:`` / ``bsc_v:`` (Bi-Sparse residuals of every rank), ``dgt_contrib:`` / ``dgt_fmt:``
+        and ``dgt:order`` (the DGT ranking), ``batch:x`` / ``batch:label`` (a look-ahead engine's primed batch, one row per rank), and a
+        ``meta:`` block.  The state is keyed by parameter, whichever rank holds it; what belongs to a worker (HFA's state, the primed
+        batches) has one row per rank.
+
+        Several ranks: collective, every rank calls it; rank 0 writes the file, and every rank raises if that fails."""
+        state = self._ckpt_state(with_batch=True)
+        err = None
+        if self.topo.rank == 0:
+            try:
+                from .. import ndarray as nd
+                nd.save(fname, {k: NDArray(torch.from_numpy(np.ascontiguousarray(v))) for k, v in state.items()})
+            except Exception as e:                          # the other ranks must learn of it instead of waiting
+                err = e
+        if self.topo.world > 1:
+            import torch.distributed as dist
+            status = torch.tensor([err is None], dtype=torch.int32, device=self.device)
+            dist.broadcast(status, src=0)
+            if err is None and not bool(status[0]):
+                raise RuntimeError("%s: rank 0 could not write the checkpoint" % fname)
+        if err is not None:
+            raise err
+
+    def load_states(self, fname):
+        """Resume from a :meth:`save_states` file.  Copies into the engine's buffers in place: the captured CUDA graphs stay valid (an engine
+        that has not captured yet runs its warm-up and capture first, so that the warm-up updates do not land on the loaded state).  When
+        the file's constant lr differs from the engine's, it is applied through :meth:`set_learning_rate`, which drops the graphs.  A
+        look-ahead engine with the saver's batch size, world size and parties primes each rank's own saved batch again; any other engine
+        does not train on the saved batches and warns (``flush()`` before saving avoids that).
+
+        The saving and the loading engine may differ in batch size, world size, parties, global servers and look-ahead; the optimizer kind,
+        ``update``, ``mode``, HFA and the accelerators (wire formats, Bi-Sparse, DGT) must match, and HFA and Bi-Sparse also need the same
+        world and party count.  A mismatch, or a missing, mis-shaped or mis-typed entry, raises ``ValueError`` naming it before anything
+        on the device is written.  Protocol state (packet epochs, counters, ready flags) is not restored.
+
+        Several ranks: collective, every rank calls it; only rank 0 reads the file and broadcasts its contents."""
+        torch.cuda.synchronize(self.device)
+        meta, layout = self._ckpt_meta(), self._ckpt_layout()
+        batch = [("batch:x", (self.topo.world, self.B, 1, 28, 28), np.dtype(np.float32)),
+                 ("batch:label", (self.topo.world, self.B), np.dtype(np.float32))]
+        data, err, use_batch = None, None, False
+        if self.topo.rank == 0:
+            try:
+                data = self._ckpt_read(fname, meta, layout)
+                use_batch = "batch:x" in data
+            except Exception as e:                          # other ranks must not wait for a payload that never comes
+                err = e
+        if self.topo.world > 1:
+            import torch.distributed as dist
+            status = torch.tensor([err is None, use_batch], dtype=torch.int32, device=self.device)
+            dist.broadcast(status, src=0)
+            if err is None and not bool(status[0]):
+                raise ValueError("%s: the checkpoint was refused on rank 0" % fname)
+            use_batch = bool(status[1])
+        if err is not None:
+            raise err
+        order = [(n, s, dt) for n, (s, dt) in layout.items()] + (batch if use_batch else [])
+        if self.topo.world > 1:
+            buf = _pack([data[n] for n, _, _ in order]) if self.topo.rank == 0 else \
+                np.empty(sum(int(np.prod(s)) * dt.itemsize for _, s, dt in order), dtype=np.uint8)
+            t = torch.from_numpy(buf).to(self.device)
+            dist.broadcast(t, src=0)
+            data = _unpack(t.cpu().numpy(), order)
+        lr = float(data["meta:lr"][0])
+        if self._sched is None and lr != self._lr:
+            self.set_learning_rate(lr)
+        if self.use_graph and not self._warmed:
+            self.xin.zero_()
+            self.capture()
+        self._ckpt_apply(data)
+        self._primed = False
+        if use_batch:
+            self.x.copy_(torch.from_numpy(data["batch:x"][self.topo.rank]))
+            self.label.copy_(torch.from_numpy(data["batch:label"][self.topo.rank]))
+            self._prime()
+        torch.cuda.synchronize(self.device)
+
+    def _ckpt_meta(self):
+        f, t = self.fabric, self.topo
+        spec = self._local_spec if self.update == "local" else f.opt_spec
+        base = f._dgt_base_fmt if f.dgt_contrib is not None else f.tile_fmt
+        i32 = lambda *v: np.array(v, dtype=np.int32)
+        return {
+            "meta:version": i32(CHECKPOINT_VERSION),
+            "meta:opt_kind": i32(native.OPT_KINDS[spec["name"]].code),
+            "meta:update": i32(self.update == "local"),
+            "meta:mode": i32(self.mode == "dist_async"),
+            "meta:hfa": i32(*(self.hfa or (0, 0))),
+            "meta:wire_formats": base.cpu().numpy() if base is not None else np.zeros(f.tiles, dtype=np.uint8),
+            "meta:bsc_threshold": np.array([self._bsc_threshold], dtype=np.float64),
+            "meta:dgt": i32(f.dgt_contrib is not None),
+            "meta:topology": i32(t.world, t.num_parties, 0 if t.tile_sharded else t.num_gs),
+            "meta:steps_done": np.array([self.steps_done], dtype=np.int64),
+            "meta:lr": np.array([self._lr], dtype=np.float64),
+        }
+
+    def _ckpt_layout(self):
+        """name -> (shape, dtype) of every entry this engine reads from a checkpoint, meta block first (the primed batch aside)."""
+        f32, i32 = np.dtype(np.float32), np.dtype(np.int32)
+        out = {n: (v.shape, v.dtype) for n, v in self._ckpt_meta().items()}
+        f, world = self.fabric, self.topo.world
+        row = (world,) if self.hfa else ()
+        for i, n in enumerate(CNN_PARAM_NAMES):
+            out[n] = (CNN_PARAM_SHAPES[i], f32)
+        for i, n in enumerate(CNN_PARAM_NAMES):
+            sl = self.layout.slots[i]
+            for p in ("master:", "s0:", "s1:"):
+                out[p + n] = (row + CNN_PARAM_SHAPES[i], f32)
+            if self.update == "local":
+                out["step:" + n] = ((world if self.hfa else 1,), i32)
+            else:
+                out["step:" + n] = ((sl.tiles if self.mode == "dist_async" else 1,), i32)
+            if f.bsc_u is not None:
+                out["bsc_u:" + n] = out["bsc_v:" + n] = ((world, sl.tiles * 1024), f32)
+            if f.dgt_contrib is not None:
+                out["dgt_contrib:" + n] = ((sl.tiles,), f32)
+                out["dgt_fmt:" + n] = ((sl.tiles,), np.dtype(np.uint8))
+        if f.dgt_contrib is not None:
+            out["dgt:order"] = ((f.tiles,), i32)
+        return out
+
+    def _ckpt_state(self, with_batch):
+        """Collective: this engine's state as checkpoint entries (name -> host array), the values of rank 0 where ranks differ."""
+        torch.cuda.synchronize(self.device)
+        f, L, T = self.fabric, self.layout, self.fabric.tiles
+        out = self._ckpt_meta()
+        for i, n in enumerate(CNN_PARAM_NAMES):
+            out[n] = self.P[i].detach().cpu().numpy()
+        per_tile = self.update == "server" and self.mode == "dist_async"
+        fs = f.export_state(async_counts=per_tile)
+        if self.update == "local":
+            # the worker's own optimizer: identical on every rank, except with HFA, where each worker trains on its own gradient
+            ranks = (lambda x: np.stack(f.gather_ranks(x))) if self.hfa else (lambda x: x.cpu().numpy())
+            fs["w"], fs["s0"], fs["s1"] = ranks(self.Wl), ranks(self.s0l), ranks(self.s1l)
+            count = ranks(self.opt_state[:1])
+        for i, n in enumerate(CNN_PARAM_NAMES):
+            sl = L.slots[i]
+            a, t0 = sl.offset, sl.offset // 1024
+            shape = CNN_PARAM_SHAPES[i]
+            for k, name in (("w", "master:"), ("s0", "s0:"), ("s1", "s1:")):
+                v = fs[k][..., a:a + sl.numel]
+                out[name + n] = v.reshape(v.shape[:-1] + shape)
+            if self.update == "local":
+                out["step:" + n] = count.reshape(-1)
+            else:
+                out["step:" + n] = fs["step"][t0:t0 + (sl.tiles if per_tile else 1)]
+            if "bsc_u" in fs:
+                out["bsc_u:" + n] = fs["bsc_u"][:, a:a + sl.tiles * 1024]
+                out["bsc_v:" + n] = fs["bsc_v"][:, a:a + sl.tiles * 1024]
+            if "dgt_contrib" in fs:
+                out["dgt_contrib:" + n] = fs["dgt_contrib"][t0:t0 + sl.tiles]
+                out["dgt_fmt:" + n] = fs["tile_fmt"][t0:t0 + sl.tiles]
+        if "tile_order" in fs:
+            out["dgt:order"] = fs["tile_order"]
+        # a look-ahead engine is primed on every rank or on none (the ranks make the same calls); each rank primed its own batch
+        if with_batch and self.lookahead and self._primed:
+            out["batch:x"] = np.stack(f.gather_ranks(self.x_cur))
+            out["batch:label"] = np.stack(f.gather_ranks(self.label_cur))
+        return out
+
+    def _ckpt_read(self, fname, meta, layout):
+        """Read and check a checkpoint against this engine's meta block ``meta`` and its entry layout ``layout`` (name -> (shape, dtype)):
+        name -> host array, ``ValueError`` for anything malformed or mismatched.  The file is untrusted input."""
+        from .. import ndarray as nd
+        try:
+            raw = nd.load(fname)
+        except OSError:
+            raise
+        except Exception as e:          # the parser's errors on a damaged or foreign file (MXNetError, struct / decoding errors)
+            raise ValueError("%s is not a readable NDArray file: %s" % (fname, e)) from e
+        if not isinstance(raw, dict):
+            raise ValueError("%s holds unnamed arrays, not a training-engine checkpoint" % fname)
+        got = {}
+        for k, v in raw.items():
+            try:
+                got[k] = v.asnumpy()
+            except Exception as e:
+                raise ValueError("checkpoint entry %r cannot be read: %s" % (k, e)) from e
+
+        def entry(name):
+            shape, dtype = layout[name]
+            if name not in got:
+                raise ValueError("checkpoint entry %r is missing" % name)
+            have = got[name]
+            if have.dtype != dtype or have.shape != tuple(shape):
+                raise ValueError("checkpoint entry %r is %s %s; this engine needs %s %s" % (name, have.dtype, have.shape, dtype, tuple(shape)))
+            return have
+
+        v = entry("meta:version")
+        if int(v[0]) != CHECKPOINT_VERSION:
+            raise ValueError("meta:version: unknown checkpoint format version %d (this engine reads %d)" % (int(v[0]), CHECKPOINT_VERSION))
+        for n in meta:
+            entry(n)
+        for n in _MUST_MATCH:
+            if not np.array_equal(got[n], meta[n]):
+                raise ValueError("%s: the checkpoint has %s, this engine %s" % (n, got[n].tolist(), meta[n].tolist()))
+        same_ranks = np.array_equal(got["meta:topology"][:2], meta["meta:topology"][:2])
+        if (self.hfa or self._bsc_threshold) and not same_ranks:
+            # HFA state belongs to each worker, Bi-Sparse residuals to each party owner: the same ranks must take them up again
+            raise ValueError("meta:topology: HFA / Bi-Sparse state was saved by %d ranks in %d parties, this engine has %d in %d"
+                             % tuple(got["meta:topology"][:2].tolist() + meta["meta:topology"][:2].tolist()))
+        if int(got["meta:steps_done"][0]) < 0:
+            raise ValueError("meta:steps_done: negative step count %d" % int(got["meta:steps_done"][0]))
+        lr = float(got["meta:lr"][0])
+        if self._sched is not None and lr != self._lr:
+            raise ValueError("meta:lr: the checkpoint's lr %g differs from the base lr %g of this engine's lr_scheduler" % (lr, self._lr))
+        if not np.isfinite(lr):
+            raise ValueError("meta:lr: %g is not a learning rate" % lr)
+        out = {n: entry(n) for n in layout}
+        if self.update == "server" and self.mode != "dist_async":
+            # the keys exchanged together share one optimizer step word: they must carry one count
+            words = self.fabric.tile_step_words()
+            first = {}
+            for i, n in enumerate(CNN_PARAM_NAMES):
+                w = words[self.layout.slots[i].offset // 1024]
+                m, c = first.setdefault(w, (n, int(out["step:" + n][0])))
+                if int(out["step:" + n][0]) != c:
+                    raise ValueError("step:%s: %d updates, but step:%s, exchanged with it, has %d" % (n, int(out["step:" + n][0]), m, c))
+        if "dgt:order" in layout:
+            if not np.array_equal(np.sort(out["dgt:order"]), np.arange(self.fabric.tiles)):
+                raise ValueError("dgt:order: not a permutation of the %d tiles" % self.fabric.tiles)
+            base = meta["meta:wire_formats"]
+            for i, n in enumerate(CNN_PARAM_NAMES):
+                t0 = self.layout.slots[i].offset // 1024
+                fmt, b = out["dgt_fmt:" + n], base[t0:t0 + len(out["dgt_fmt:" + n])]
+                if not np.where(b == self.fabric.FMT_BSC, fmt == b, (fmt == b) | (fmt == self.fabric.FMT_F8)).all():
+                    raise ValueError("dgt_fmt:%s: formats other than the base format or its fp8 demotion" % n)
+        if "batch:x" in got or "batch:label" in got:
+            x, y = got.get("batch:x"), got.get("batch:label")
+            if x is None or y is None or x.dtype != np.float32 or y.dtype != np.float32 or x.ndim != 5 or x.shape[2:] != (1, 28, 28) \
+                    or y.shape != x.shape[:2] or x.shape[0] != int(got["meta:topology"][0]):
+                raise ValueError("batch:x / batch:label: not one batch of (B, 1, 28, 28) fp32 images and B fp32 labels per saving rank")
+            if self.lookahead and same_ranks and x.shape[1] == self.B:
+                out["batch:x"], out["batch:label"] = x, y
+            else:
+                import warnings
+                warnings.warn("%s holds the primed batches of %d ranks of batch size %d, which this engine does not train on (it restores "
+                              "them only with lookahead=True and the same batch size, world size and parties)" % (fname, x.shape[0], x.shape[1]))
+        return out
+
+    def _ckpt_apply(self, data):
+        """Write the checked entries ``data`` into this engine's buffers, in place."""
+        f, L, me = self.fabric, self.layout, self.topo.rank
+        fs = {k: np.zeros(f.n, dtype=np.float32) for k in ("w", "s0", "s1")}
+        per_tile = self.update == "server" and self.mode == "dist_async"
+        step = np.zeros(f.tiles, dtype=np.int32)
+        if "dgt:order" in data:
+            fs["dgt_contrib"], fs["tile_fmt"] = np.zeros(f.tiles, dtype=np.float32), np.zeros(f.tiles, dtype=np.uint8)
+            fs["tile_order"] = data["dgt:order"]
+        if f.bsc_u is not None:
+            fs["bsc_u"], fs["bsc_v"] = (np.zeros((self.topo.world, f.n), dtype=np.float32) for _ in range(2))
+        row = (lambda v: v[me]) if self.hfa else (lambda v: v)
+        for i, n in enumerate(CNN_PARAM_NAMES):
+            sl = L.slots[i]
+            a, t0 = sl.offset, sl.offset // 1024
+            for k, name in (("w", "master:"), ("s0", "s0:"), ("s1", "s1:")):
+                fs[k][a:a + sl.numel] = row(data[name + n]).reshape(-1)
+            step[t0:t0 + sl.tiles] = row(data["step:" + n])
+            if "bsc_u" in fs:
+                fs["bsc_u"][:, a:a + sl.tiles * 1024] = data["bsc_u:" + n]
+                fs["bsc_v"][:, a:a + sl.tiles * 1024] = data["bsc_v:" + n]
+            if "dgt_contrib" in fs:
+                fs["dgt_contrib"][t0:t0 + sl.tiles] = data["dgt_contrib:" + n]
+                fs["tile_fmt"][t0:t0 + sl.tiles] = data["dgt_fmt:" + n]
+        if self.update == "local":
+            wl = {k: torch.from_numpy(fs.pop(k)).to(self.device) for k in ("w", "s0", "s1")}
+            f.import_state(fs)
+            self.Wl.copy_(wl["w"]); self.s0l.copy_(wl["s0"]); self.s1l.copy_(wl["s1"])
+            self.opt_state[0] = int(step[0])
+        else:
+            fs["step"] = step
+            f.import_state(fs, async_counts=per_tile)
+            for i, n in enumerate(CNN_PARAM_NAMES):
+                self.P[i].copy_(torch.from_numpy(data[n]))
+        self.steps_done = int(data["meta:steps_done"][0])
 
     def _bind_input(self, k):
         """Point the step at input buffer ``k`` (0 = ``self.xin``; 1 = the second staging buffer of the host pipeline).  Only matters while

@@ -89,6 +89,38 @@ def global_tile_owners(topo, layout, protocol, bigarray_bound=1000000):
     return np.array([topo.gs_ranks[i] for i in owner_idx], dtype=np.int32)
 
 
+def held_tiles(owners, replicated, rank):
+    """Tiles whose server state ``rank`` holds: those it owns, and every tile in ``replicated`` (each rank updates its own replica of those:
+    a single rank, or a one-hop replicated channel).  ``replicated``: bool per tile or None."""
+    held = np.asarray(owners) == rank
+    return held if replicated is None else held | np.asarray(replicated, dtype=bool)
+
+
+def gather_tile_state(per_rank, owners, replicated=None):
+    """One piece of server state as a full array, from every rank's copy of it: tile ``t`` from its owner ``owners[t]``, a replicated tile
+    from rank 0's replica.  ``per_rank[r]``: rank r's array, tile-major with the same number of values per tile (1024 for an arena, 1 for a
+    per-tile word).  Host-only, so that any topology can be simulated."""
+    owners = np.asarray(owners)
+    src = owners if replicated is None else np.where(np.asarray(replicated, dtype=bool), 0, owners)
+    T = len(src)
+    out = np.array(per_rank[0], copy=True).reshape(T, -1)
+    for r in np.unique(src):
+        sel = src == r
+        out[sel] = np.asarray(per_rank[int(r)]).reshape(T, -1)[sel]
+    return out.reshape(np.shape(per_rank[0]))
+
+
+def scatter_tile_state(full, per_rank, owners, replicated=None):
+    """Inverse of :func:`gather_tile_state`: write ``full`` into the arrays of ``per_rank`` (a dict rank -> array, updated in place) on the
+    tiles that rank holds (:func:`held_tiles`); the other tiles keep their values.  Returns ``per_rank``."""
+    T = len(owners)
+    src = np.asarray(full).reshape(T, -1)
+    for r, arr in per_rank.items():
+        sel = held_tiles(owners, replicated, r)
+        arr.reshape(T, -1)[sel] = src[sel]
+    return per_rank
+
+
 # ------------------------------------------------------------------------------------------------------------ symmetric heap
 class SymmetricBuffer:
     """A tensor allocated at the same size on every rank of ``group`` with peer-mapped pointers (+ multicast address if NVLS)."""
@@ -554,6 +586,101 @@ class HipsFabric:
     def set_opt_step(self, t):
         for n in ["fsa"] + list(self.channels):
             self.state[n][2] = int(t)
+
+    # -- checkpoints ----------------------------------------------------------------------------------------------------
+    def replicated_tiles(self):
+        """bool per tile: every rank keeps its own replica of the tile's server state (a single rank, or a one-hop replicated channel)."""
+        if self.topo.world == 1:
+            return np.ones(self.tiles, dtype=bool)
+        rep = np.zeros(self.tiles, dtype=bool)
+        for ch in self.channels.values():
+            if ch["replicate"]:
+                rep |= self._key_tile_mask(ch["keys"])
+        return rep
+
+    def _key_tile_mask(self, keys):
+        mask = np.zeros(self.tiles, dtype=bool)
+        for i in keys:
+            sl = self.layout.slots[i]
+            mask[sl.offset // 1024: sl.offset // 1024 + sl.tiles] = True
+        return mask
+
+    def tile_step_words(self):
+        """Per tile, the state whose optimizer step word counts the tile's dist_sync updates: its channel's, else the one exchange's."""
+        words = np.array(["fsa"] * self.tiles, dtype=object)
+        for name, ch in self.channels.items():
+            words[self._key_tile_mask(ch["keys"])] = name
+        return words
+
+    def gather_ranks(self, t):
+        """Host (numpy) copies of the local tensor ``t`` of every rank, in rank order (collective over the world)."""
+        t = t.contiguous()
+        if self.topo.world == 1:
+            return [t.cpu().numpy()]
+        import torch.distributed as dist
+        out = [torch.empty_like(t) for _ in range(self.topo.world)]
+        dist.all_gather(out, t)
+        return [o.cpu().numpy() for o in out]
+
+    def export_state(self, async_counts=False):
+        """Collective over the world: the server state as full host arrays in arena order, whoever holds each tile (the owner of a sharded
+        tile, rank 0's replica of a replicated one).  ``w`` / ``s0`` / ``s1``: float32 [n]; ``step``: int32 [tiles], the update count of
+        each tile — the step word of its exchange (dist_sync), or with ``async_counts`` the one-sided update's per-tile count.  With DGT
+        ``dgt_contrib`` (from the owners, as ``dgt_rerank`` reads it), ``tile_order`` and ``tile_fmt``; with Bi-Sparse the party owners'
+        residuals ``bsc_u`` / ``bsc_v`` of every rank, float32 [world, n].  Protocol state (epochs, counters, flags) is not part of it."""
+        owners, rep = self.tile_owner_np, self.replicated_tiles()
+        out = {k: gather_tile_state(self.gather_ranks(getattr(self, k)), owners, rep) for k in ("w", "s0", "s1")}
+        if async_counts:
+            a = self.off["async_step"]
+            out["step"] = gather_tile_state(self.gather_ranks(self.flags.tensor[a:a + self.tiles]), owners)
+        else:
+            words = self.tile_step_words()
+            out["step"] = np.array([int(self.state[n][2].item()) for n in words], dtype=np.int32)
+        if self.dgt_contrib is not None:
+            out["dgt_contrib"] = gather_tile_state(self.gather_ranks(self.dgt_contrib), owners)
+            out["tile_order"] = self.tile_order.cpu().numpy()
+            out["tile_fmt"] = self.tile_fmt.cpu().numpy()
+        if self.bsc_u is not None:
+            out["bsc_u"] = np.stack(self.gather_ranks(self.bsc_u))
+            out["bsc_v"] = np.stack(self.gather_ranks(self.bsc_v))
+        return out
+
+    def import_state(self, state, async_counts=False):
+        """Inverse of :meth:`export_state`, on every rank with the same ``state``: each rank copies the tiles it holds into its buffers in
+        place (captured graphs stay valid); the optimizer step words are set, the protocol state is left as it is.  A tile's step word is
+        shared by its channel, so every tile of a channel must carry the same count (``ValueError`` otherwise, before anything is written)."""
+        owners, rep, me, T = self.tile_owner_np, self.replicated_tiles(), self.topo.rank, self.tiles
+        step = np.asarray(state.get("step", np.zeros(T, dtype=np.int32)))
+        words = None
+        if not async_counts:
+            words = {}
+            for n, w in zip(self.tile_step_words(), step.tolist()):
+                if words.setdefault(n, w) != w:
+                    raise ValueError("step: the keys exchanged together (%s) were saved with different update counts" % n)
+
+        def put(dev, full, replicated):
+            local = dev.cpu().numpy()
+            scatter_tile_state(np.asarray(full), {me: local}, owners, replicated)
+            dev.copy_(torch.from_numpy(local))
+
+        for k in ("w", "s0", "s1"):
+            if k in state:
+                put(getattr(self, k), state[k], rep)
+        if async_counts:
+            a = self.off["async_step"]
+            put(self.flags.tensor[a:a + T], step, None)
+        elif "step" in state:
+            for n, w in words.items():
+                self.state[n][2] = w
+            if "fsa" not in words:
+                self.state["fsa"][2] = int(step.max())
+        if self.dgt_contrib is not None:
+            put(self.dgt_contrib, state["dgt_contrib"], None)
+            self.tile_order.copy_(torch.from_numpy(np.asarray(state["tile_order"])))
+            self.tile_fmt.copy_(torch.from_numpy(np.asarray(state["tile_fmt"])))
+        if self.bsc_u is not None:
+            self.bsc_u.copy_(torch.from_numpy(np.asarray(state["bsc_u"])[me]))
+            self.bsc_v.copy_(torch.from_numpy(np.asarray(state["bsc_v"])[me]))
 
     def _peer_table(self, name, ptrs):
         if name not in self._peer_tables:
