@@ -414,7 +414,11 @@ static_assert(sizeof(CnnFwdHeadSmem) == CNN_FWD_DENSE0_SMEM_BYTES, "CNN_FWD_DENS
 // sums over W1 rows 16 w .. 16 w + 15 (lane = column, so a warp reads 128 contiguous bytes of a row from L2), the 8 partials are added in
 // warp order.  Stores this CTA's a4, dz4 and dz3 columns; ranks 0 and 1 store the loss, logits and dlogits of image bpair + rank.  Every
 // output has one writer and a fixed summation order: two launches give the same bits.
-__device__ __forceinline__ void fwd_train_head(CnnFwdHeadSmem& s, const FwdHeadArgs& hd, int cr, int bpair, unsigned long long* dbg) {
+// WEIGHTED: the dlogits of image b are scaled by coef[b] (the per-row gradient coefficient of a short or sample-weighted batch) where they
+// are produced, so that dz4, dz3 and every weight gradient carry it; the loss stays unweighted.
+template <bool WEIGHTED>
+__device__ __forceinline__ void fwd_train_head(CnnFwdHeadSmem& s, const FwdHeadArgs& hd, int cr, int bpair, unsigned long long* dbg,
+                                               const float* __restrict__ coef) {
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, j = tid & 15, c = tid >> 4;
@@ -439,6 +443,11 @@ __device__ __forceinline__ void fwd_train_head(CnnFwdHeadSmem& s, const FwdHeadA
 #pragma unroll
     for (int k = 0; k < 4; ++k) lg[k] = c0 + k < CD_NC ? s.h.logit[16 * i + c0 + k] : 0.f;
     const float loss = softmax_ce_quad(lg, CD_NC, (int)__ldg(hd.label + b), dl);
+    if (WEIGHTED) {
+      const float cb = __ldg(coef + b);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) dl[k] = __fmul_rn(dl[k], cb);
+    }
     if (lane < 8) {
       *reinterpret_cast<float4*>(s.dl + 16 * i + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
       if (cr == i) {
@@ -488,12 +497,16 @@ __device__ __forceinline__ void fwd_train_head(CnnFwdHeadSmem& s, const FwdHeadA
 
 // grid (B, 4), B even, 256 threads, clusters of (2, 4, 1).  Without the head's outputs (hd.a4 == nullptr) it ends with a3 (stamps 5 a2 landed,
 // 6 a3 stored); with them it also runs fwd_train_head (stamps 7 a3 landed, 14 a4 landed, 15 dz3 stored).  Slot 4 is the end of the kernel.
-__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
-    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
-                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
-                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
-                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
-                          unsigned long long* dbg, const FwdHeadArgs hd) {
+// Instantiated twice: cnn_fwd_dense0_kernel (WEIGHTED = false) compiles to the code it had before the weighted head existed;
+// cnn_fwd_dense0_weighted_kernel scales the dlogits by coef.
+template <bool WEIGHTED>
+__device__ __forceinline__ void cnn_fwd_dense0_body(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0,
+                                                    const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ wd,
+                                                    const float* __restrict__ bd, float* __restrict__ a1, unsigned char* __restrict__ idx1,
+                                                    float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
+                                                    const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n,
+                                                    float* __restrict__ x_keep, unsigned long long* dbg, const FwdHeadArgs& hd,
+                                                    const float* __restrict__ coef) {
   __shared__ CnnFwdHeadSmem s;
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0;
   auto stamp = [&](int slot) { if (dbg_on) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); dbg[slot] = t; } };
@@ -512,8 +525,28 @@ __global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 r
     s.h.a3own[j * 32 + (tid >> 3)] = y;
   });
   stamp(6);
-  if (head) fwd_train_head(s, hd, cr, bpair, dbg);
+  if (head) fwd_train_head<WEIGHTED>(s, hd, cr, bpair, dbg, coef);
   stamp(4);      // (slot 4 stays the end of the forward kernel)
+}
+
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers: fits beside a dense_tail_kernel CTA
+    cnn_fwd_dense0_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0, const float* __restrict__ w1,
+                          const float* __restrict__ b1, const float* __restrict__ wd, const float* __restrict__ bd, float* __restrict__ a1,
+                          unsigned char* __restrict__ idx1, float* __restrict__ a2, unsigned char* __restrict__ idx2, float* __restrict__ a3,
+                          const float* __restrict__ carry_src, float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep,
+                          unsigned long long* dbg, const FwdHeadArgs hd) {
+  cnn_fwd_dense0_body<false>(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n, x_keep, dbg, hd, nullptr);
+}
+
+// coef [B]: the gradient coefficient of each row (see fwd_train_head); always launched with the head
+__global__ void __cluster_dims__(2, 4, 1) __launch_bounds__(256, 4)   // <= 64 registers, as its unweighted twin
+    cnn_fwd_dense0_weighted_kernel(const float* __restrict__ x, const float* __restrict__ w0, const float* __restrict__ b0,
+                                   const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ wd,
+                                   const float* __restrict__ bd, float* __restrict__ a1, unsigned char* __restrict__ idx1, float* __restrict__ a2,
+                                   unsigned char* __restrict__ idx2, float* __restrict__ a3, const float* __restrict__ carry_src,
+                                   float* __restrict__ carry_dst, int carry_n, float* __restrict__ x_keep, unsigned long long* dbg,
+                                   const FwdHeadArgs hd, const float* __restrict__ coef) {
+  cnn_fwd_dense0_body<true>(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n, x_keep, dbg, hd, coef);
 }
 
 // ------------------------------------------------------------------------------------------------------------------ inference
@@ -966,15 +999,21 @@ GX_API int gx_cnn_fwd(const float* x, const float* w0, const float* b0, const fl
 }
 // the same, plus the first dense layer: a3 [B,256] = relu(a2 [B,512] · wd [256,512]^T + bd).  With a4 non-null also the training head
 // (fwd_train_head): wd1 [128,256], bd1, wd2 [10,128], bd2, label [B] in; loss [B], logits [B,10] (unless null), a4 [B,128], dz4 [B,128],
-// dz3 [B,256] and dl [B,16] out.  Only for even B <= 32 (clusters of two images); returns -1 without launching otherwise.
+// dz3 [B,256] and dl [B,16] out.  coef [B] (with the head only; may be null): the dlogits of row b are scaled by coef[b] before anything is
+// derived from them (cnn_fwd_dense0_weighted_kernel); the loss is not.  Only for even B <= 32 (clusters of two images); returns -1 without
+// launching otherwise, or for coef without the head.
 GX_API int gx_cnn_fwd_dense0(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* wd, const float* bd,
                              float* a1, unsigned char* idx1, float* a2, unsigned char* idx2, float* a3, const float* carry_src, float* carry_dst,
                              int carry_n, float* x_keep, const float* wd1, const float* bd1, const float* wd2, const float* bd2, const float* label,
-                             float* loss, float* logits, float* a4, float* dz4, float* dz3, float* dl, int B, cudaStream_t s) {
-  if (B < 2 || (B & 1) || B > 32) return -1;
+                             float* loss, float* logits, float* a4, float* dz4, float* dz3, float* dl, const float* coef, int B, cudaStream_t s) {
+  if (B < 2 || (B & 1) || B > 32 || (coef != nullptr && a4 == nullptr)) return -1;
   const FwdHeadArgs hd = {wd1, bd1, wd2, bd2, label, loss, logits, a4, dz4, dz3, dl};
-  launch_pdl(cnn_fwd_dense0_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n,
-             x_keep, g_cnn_dbg, hd);
+  if (coef != nullptr)
+    launch_pdl(cnn_fwd_dense0_weighted_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst,
+               carry_n, x_keep, g_cnn_dbg, hd, coef);
+  else
+    launch_pdl(cnn_fwd_dense0_kernel, dim3(B, 4), dim3(256), 0, s, x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry_src, carry_dst, carry_n,
+               x_keep, g_cnn_dbg, hd);
   return GX_CHECK_LAUNCH();
 }
 // inference of the whole demo CNN (cnn_eval_kernel): x [N,1,28,28], the ten parameters in CNN_PARAM_SHAPES order; writes logits [N,10] (unless

@@ -55,10 +55,15 @@ __global__ void __launch_bounds__(256) softmax_ce_bwd_kernel(const float* __rest
 //   phase 1 : warp per sample: logits, loss, dlogits -> smem
 //   phase 2 : dW[c][k] = sum_b dl[b][c]*a[b][k] ; db[c] = sum_b dl[b][c]
 //             da[b][k] = (a[b][k] > 0 ? sum_c dl[b][c]*W[c][k] : 0)  over all B*K outputs in parallel;  dbias_prev[k] = sum_b da[b][k]
-__global__ void __launch_bounds__(1024) head_fwd_bwd_kernel(const float* __restrict__ a, const float* __restrict__ W, const float* __restrict__ bias,
-                                                             const float* __restrict__ label, float* __restrict__ loss, float* __restrict__ logits_out,
-                                                             float* __restrict__ dW, float* __restrict__ db, float* __restrict__ da,
-                                                             float* __restrict__ dbias_prev, int B, int K, int C, int relu_mask) {
+// WEIGHTED: the dlogits of sample b are scaled by coef[b] in phase 1 (the per-row gradient coefficient of a short or sample-weighted batch),
+// so every gradient carries it; the loss stays unweighted.  Instantiated twice: head_fwd_bwd_kernel (WEIGHTED = false) compiles to the code
+// it had before the weighted head existed; head_fwd_bwd_weighted_kernel.
+template <bool WEIGHTED>
+__device__ __forceinline__ void head_fwd_bwd_body(const float* __restrict__ a, const float* __restrict__ W, const float* __restrict__ bias,
+                                                  const float* __restrict__ label, float* __restrict__ loss, float* __restrict__ logits_out,
+                                                  float* __restrict__ dW, float* __restrict__ db, float* __restrict__ da,
+                                                  float* __restrict__ dbias_prev, int B, int K, int C, int relu_mask,
+                                                  const float* __restrict__ coef) {
   gx::pdl_wait();
   gx::pdl_launch();
   extern __shared__ float sm[];
@@ -90,7 +95,8 @@ __global__ void __launch_bounds__(1024) head_fwd_bwd_kernel(const float* __restr
     const float s = warp_sum(e);
     const int l = (int)slab[b];
     if (lane < C) {
-      dl[b * C + lane] = e / s - (lane == l ? 1.f : 0.f);
+      const float d = e / s - (lane == l ? 1.f : 0.f);
+      dl[b * C + lane] = WEIGHTED ? __fmul_rn(d, coef[b]) : d;
       if (logits_out) logits_out[(long long)b * C + lane] = mylogit;
     }
     const float picked = __shfl_sync(0xffffffffu, mylogit, l & 31);
@@ -125,6 +131,19 @@ __global__ void __launch_bounds__(1024) head_fwd_bwd_kernel(const float* __restr
     }
   }
 }
+__global__ void __launch_bounds__(1024) head_fwd_bwd_kernel(const float* __restrict__ a, const float* __restrict__ W, const float* __restrict__ bias,
+                                                             const float* __restrict__ label, float* __restrict__ loss, float* __restrict__ logits_out,
+                                                             float* __restrict__ dW, float* __restrict__ db, float* __restrict__ da,
+                                                             float* __restrict__ dbias_prev, int B, int K, int C, int relu_mask) {
+  head_fwd_bwd_body<false>(a, W, bias, label, loss, logits_out, dW, db, da, dbias_prev, B, K, C, relu_mask, nullptr);
+}
+__global__ void __launch_bounds__(1024) head_fwd_bwd_weighted_kernel(const float* __restrict__ a, const float* __restrict__ W,
+                                                                      const float* __restrict__ bias, const float* __restrict__ label,
+                                                                      float* __restrict__ loss, float* __restrict__ logits_out, float* __restrict__ dW,
+                                                                      float* __restrict__ db, float* __restrict__ da, float* __restrict__ dbias_prev,
+                                                                      int B, int K, int C, int relu_mask, const float* __restrict__ coef) {
+  head_fwd_bwd_body<true>(a, W, bias, label, loss, logits_out, dW, db, da, dbias_prev, B, K, C, relu_mask, coef);
+}
 
 }  // namespace gx
 
@@ -138,10 +157,18 @@ GX_API int gx_softmax_ce_bwd(const float* x, const float* label, const float* dl
   launch_pdl(softmax_ce_bwd_kernel, dim3((R + 7) / 8), dim3(256), 0, s, x, label, dloss, dx, R, C);
   return GX_CHECK_LAUNCH();
 }
+// coef [B] (may be null): the dlogits of sample b are scaled by coef[b] (head_fwd_bwd_weighted_kernel); the loss is not
 GX_API int gx_head_fwd_bwd(const float* a, const float* W, const float* bias, const float* label, float* loss, float* logits, float* dW,
-                           float* db, float* da, float* dbias_prev, int B, int K, int C, int relu_mask, cudaStream_t s) {
+                           float* db, float* da, float* dbias_prev, const float* coef, int B, int K, int C, int relu_mask, cudaStream_t s) {
   const size_t smem = ((size_t)2 * B * K + (size_t)C * K + (size_t)B * C + 32 + (size_t)B) * sizeof(float);
   if (C > 32 || (long long)B * C > 8192 || smem > 200 * 1024 || (K & 3)) return -1;
+  if (coef != nullptr) {
+    static bool set_w = false;
+    if (!set_w) { cudaFuncSetAttribute(head_fwd_bwd_weighted_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); set_w = true; }
+    launch_pdl(head_fwd_bwd_weighted_kernel, dim3(1), dim3(1024), smem, s, a, W, bias, label, loss, logits, dW, db, da, dbias_prev, B, K, C,
+               relu_mask, coef);
+    return GX_CHECK_LAUNCH();
+  }
   static bool set = false;
   if (!set) { cudaFuncSetAttribute(head_fwd_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); set = true; }
   launch_pdl(head_fwd_bwd_kernel, dim3(1), dim3(1024), smem, s, a, W, bias, label, loss, logits, dW, db, da, dbias_prev, B, K, C, relu_mask);

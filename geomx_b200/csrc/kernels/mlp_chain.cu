@@ -59,6 +59,7 @@ struct MlpChainParams {
   int B, C;
   int from_dz3;              // dense_tail_kernel: dz3 is the input (cnn_fwd_dense0_kernel's training head computed it) and dx the only output
   unsigned long long* dbg;   // optional %globaltimer stamps of cluster CTA 0 (tools/kernel_times.py)
+  const float* coef;         // [B] per-row gradient coefficient: read by the weighted instances only (dense_chain_body's W)
 };
 
 // 16-byte chunk swizzle of a K-major [rows][K] tile: chunk (k>>2) is XORed with (row>>2)&7, so the 8 row-groups a warp touches in one
@@ -330,8 +331,10 @@ __device__ __forceinline__ void dense_dx_rows(float* sm, const MlpChainParams& p
 // P2 .. P5 of the chain, the part both cluster kernels share: a4 = relu(a3 W1^T + b1) with the a4 hand-off, the classifier, softmax-CE and
 // the whole dz4, dz3 with its hand-off, and dx.  On entry the weights are staged (W0 as the column slice for dx still in flight, W1 as the
 // row slice), a3 is in the A3 buffer (FROM_X: as it lands from the peers) and in A3OWN (this CTA's columns), the labels and biases are
-// staged and the cluster has met once.  FROM_X (mlp_chain_kernel) also waits for a3 and stores this CTA's a3 columns.
-template <class L, int D0, int D1, int D2, int CS, bool FROM_X, class Stamp>
+// staged and the cluster has met once.  FROM_X (mlp_chain_kernel) also waits for a3 and stores this CTA's a3 columns.  W (the weighted
+// instances): the dlogits of row b are scaled by p.coef[b] where they are produced, so that dz4, dz3, dx and every weight gradient carry it;
+// the loss stays unweighted.
+template <class L, int D0, int D1, int D2, int CS, bool FROM_X, bool W, class Stamp>
 __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams& p, const int cr, uint64_t* bar_a3, uint64_t* bar_a4,
                                                  uint64_t* bar_dz3, Stamp&& stamp) {
   constexpr int NS1 = L::NS1, NS2 = L::NS2, KS0 = L::KS0;
@@ -396,6 +399,11 @@ __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams
       float dl[4];
       const float loss = softmax_ce_quad(lg, C, (int)sLab[b], dl);
       if (b >= B) dl[0] = dl[1] = dl[2] = dl[3] = 0.f;
+      if (W && b < B) {
+        const float cb = __ldg(p.coef + b);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dl[j] = __fmul_rn(dl[j], cb);
+      }
       *reinterpret_cast<float4*>(sDL + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
       if (cr == 0 && b < B) {
         *reinterpret_cast<float4*>(p.dl + b * MC_CMAX + c0) = make_float4(dl[0], dl[1], dl[2], dl[3]);
@@ -472,9 +480,10 @@ __device__ __forceinline__ void dense_chain_body(float* sm, const MlpChainParams
   dense_dx<L, D0, D1>(sm, p, cr, stamp);
 }
 
-// CS = CTAs per cluster: 8 (portable) or 16 (non-portable size, one GPC): every layer is cut into CS column slices
-template <int D0, int D1, int D2, int CS>
-__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_kernel(const MlpChainParams p) {
+// CS = CTAs per cluster: 8 (portable) or 16 (non-portable size, one GPC): every layer is cut into CS column slices.  Instantiated twice:
+// mlp_chain_kernel (W = false) compiles to the code it had before the weighted chain existed; mlp_chain_weighted_kernel scales the dlogits.
+template <int D0, int D1, int D2, int CS, bool W>
+__device__ __forceinline__ void mlp_chain_body(const MlpChainParams& p) {
   using L = MlpSmem<D0, D1, D2, CS>;
   constexpr int NS1 = L::NS1, NS2 = L::NS2;
   static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
@@ -561,14 +570,23 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_
     }
     stamp(13);
   }
-  dense_chain_body<L, D0, D1, D2, CS, true>(sm, p, cr, bar_a3, bar_a4, bar_dz3, stamp);
+  dense_chain_body<L, D0, D1, D2, CS, true, W>(sm, p, cr, bar_a3, bar_a4, bar_dz3, stamp);
+}
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_kernel(const MlpChainParams p) {
+  mlp_chain_body<D0, D1, D2, CS, false>(p);
+}
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) mlp_chain_weighted_kernel(const MlpChainParams p) {
+  mlp_chain_body<D0, D1, D2, CS, true>(p);
 }
 
 // The chain from a3 on, for a step whose forward kernel (cnn_fwd_dense0_kernel) has already computed a3 = relu(x W0^T + b0): P2 .. P5 of
 // mlp_chain_kernel, unchanged, on the same cluster.  Everything but a3 and the labels (the W1 row slice, W2, the biases and the W0 column
 // slice of dx) is staged before griddepcontrol.wait, i.e. while the forward kernel still runs; then a3 (32 KB) is the only input left.
-template <int D0, int D1, int D2, int CS>
-__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dense_tail_kernel(const MlpChainParams p) {
+// Instantiated twice, as mlp_chain_kernel: dense_tail_kernel (W = false) and dense_tail_weighted_kernel.
+template <int D0, int D1, int D2, int CS, bool W>
+__device__ __forceinline__ void dense_tail_body(const MlpChainParams& p) {
   using L = TailSmem<D0, D1, D2, CS>;
   constexpr int NS1 = L::NS1, NS2 = L::NS2;
   static_assert((CS & (CS - 1)) == 0, "cluster size must be a power of two");
@@ -624,7 +642,15 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dens
   __syncthreads();
   cluster.barrier_wait();
   stamp(3);
-  dense_chain_body<L, D0, D1, D2, CS, false>(sm, p, cr, nullptr, bar_a4, bar_dz3, stamp);
+  dense_chain_body<L, D0, D1, D2, CS, false, W>(sm, p, cr, nullptr, bar_a4, bar_dz3, stamp);
+}
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dense_tail_kernel(const MlpChainParams p) {
+  dense_tail_body<D0, D1, D2, CS, false>(p);
+}
+template <int D0, int D1, int D2, int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(MC_THREADS, 1) dense_tail_weighted_kernel(const MlpChainParams p) {
+  dense_tail_body<D0, D1, D2, CS, true>(p);
 }
 
 // ---- the dense weight gradients, from what mlp_chain_kernel stored: dW0 = dz3^T x, dW1 = dz4^T a3, dW2 = dl^T a4, and the bias gradients
@@ -677,12 +703,13 @@ __global__ void __launch_bounds__(WG_THREADS) dense_wgrad_kernel(const DenseWgra
 
 using namespace gx;
 
-// 512 -> 256 -> 128 -> C (C <= 16), B <= 32.  TAIL: dense_tail_kernel, else mlp_chain_kernel.  Returns -2 when this cluster size cannot be
-// scheduled on this device.
-template <bool TAIL, int CS>
+// 512 -> 256 -> 128 -> C (C <= 16), B <= 32.  TAIL: dense_tail_kernel, else mlp_chain_kernel; W: their weighted instances.  Returns -2 when
+// this cluster size cannot be scheduled on this device.
+template <bool TAIL, bool W, int CS>
 static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
   constexpr int BYTES = TAIL ? TailSmem<512, 256, 128, CS>::BYTES : MlpSmem<512, 256, 128, CS>::BYTES;
-  auto kern = TAIL ? dense_tail_kernel<512, 256, 128, CS> : mlp_chain_kernel<512, 256, 128, CS>;
+  auto kern = TAIL ? (W ? dense_tail_weighted_kernel<512, 256, 128, CS> : dense_tail_kernel<512, 256, 128, CS>)
+                   : (W ? mlp_chain_weighted_kernel<512, 256, 128, CS> : mlp_chain_kernel<512, 256, 128, CS>);
   static int ready = 0;      // 0 = not configured, 1 = ok, -1 = this cluster size cannot be scheduled on this device
   if (ready == 0) {
     ready = -1;
@@ -711,45 +738,48 @@ static int mlp_launch(const MlpChainParams& p, cudaStream_t stream) {
   return GX_CHECK_LAUNCH();
 }
 // cluster of 16 CTAs (one GPC) halves every slice; fall back to the portable size 8 when the device cannot co-schedule 16
-template <bool TAIL>
+template <bool TAIL, bool W>
 static int mlp_launch_any(const MlpChainParams& p, cudaStream_t stream) {
   static int want = -1;
   if (want < 0) { const char* e = getenv("GEOMX_MLP_CLUSTER"); want = e ? atoi(e) : 16; }
   if (want >= 16) {
-    const int rc = mlp_launch<TAIL, 16>(p, stream);
+    const int rc = mlp_launch<TAIL, W, 16>(p, stream);
     if (rc != -2) return rc;
     want = 8;
   }
-  return mlp_launch<TAIL, 8>(p, stream);
+  return mlp_launch<TAIL, W, 8>(p, stream);
 }
 
 static unsigned long long* g_mlp_dbg = nullptr;
 GX_API int gx_mlp_chain_set_debug(unsigned long long* p) { g_mlp_dbg = p; return 0; }
 
-// the data path: loss, logits, dx; stores a3, a4, dz4, dz3 and the dlogits (rows b < B) for gx_dense_wgrad.  Returns -1 for unsupported
-// shapes (caller uses the per-layer kernels).
+// the data path: loss, logits, dx; stores a3, a4, dz4, dz3 and the dlogits (rows b < B) for gx_dense_wgrad.  coef [B] (may be null): the
+// dlogits of row b are scaled by coef[b] before anything is derived from them (mlp_chain_weighted_kernel); the loss is not.  Returns -1 for
+// unsupported shapes (caller uses the per-layer kernels).
 GX_API int gx_mlp_chain(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
                         const float* label, float* loss, float* logits, float* dx, float* a3, float* a4, float* dz4, float* dz3, float* dl,
-                        int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
+                        const float* coef, int B, int D0, int D1, int D2, int C, cudaStream_t stream) {
   if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
   MlpChainParams p;
   p.x = x; p.w0 = w0; p.b0 = b0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
-  p.a3 = a3; p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
-  return mlp_launch_any<false>(p, stream);
+  p.a3 = a3; p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg; p.coef = coef;
+  return coef != nullptr ? mlp_launch_any<false, true>(p, stream) : mlp_launch_any<false, false>(p, stream);
 }
 
 // the same data path from a3 [B][D1] (computed by gx_cnn_fwd_dense0): loss, logits, dx; stores a4, dz4, dz3 and the dlogits for
 // gx_dense_wgrad.  w0 is read only as the column slices of dx.  from_dz3 != 0: dx = dz3 [B][D1] · w0 only (dz3 computed by gx_cnn_fwd_dense0's
-// training head); nothing else is read or written.  Returns -1 for unsupported shapes.
+// training head); nothing else is read or written.  coef [B] (may be null, and must be without from_dz3, whose dz3 already carries it): the
+// dlogits of row b are scaled by coef[b] (dense_tail_weighted_kernel), as in gx_mlp_chain.  Returns -1 for unsupported shapes.
 GX_API int gx_dense_tail(const float* a3, const float* w0, const float* w1, const float* b1, const float* w2, const float* b2, const float* label,
-                         float* loss, float* logits, float* dx, float* a4, float* dz4, float* dz3, float* dl, int B, int D0, int D1, int D2, int C,
-                         int from_dz3, cudaStream_t stream) {
-  if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B) return -1;
+                         float* loss, float* logits, float* dx, float* a4, float* dz4, float* dz3, float* dl, const float* coef, int B, int D0, int D1,
+                         int D2, int C, int from_dz3, cudaStream_t stream) {
+  if (D0 != 512 || D1 != 256 || D2 != 128 || C < 1 || C > MC_CMAX || B < 1 || B > MC_B || (coef != nullptr && from_dz3)) return -1;
   MlpChainParams p = {};
   p.w0 = w0; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.label = label; p.loss = loss; p.logits = logits; p.dx = dx;
   p.a3 = const_cast<float*>(a3); p.a4 = a4; p.dz4 = dz4; p.dz3 = dz3; p.dl = dl; p.B = B; p.C = C; p.dbg = g_mlp_dbg;
   p.from_dz3 = from_dz3 != 0;
-  return mlp_launch_any<true>(p, stream);
+  p.coef = coef;
+  return coef != nullptr ? mlp_launch_any<true, true>(p, stream) : mlp_launch_any<true, false>(p, stream);
 }
 
 // dW0 / db0, dW1 / db1, dW2 / db2 (overwritten) from what gx_mlp_chain stored; x has exactly B rows, dl rows hold 16 floats

@@ -29,7 +29,9 @@ engine's arguments and the step switches (``STEP_SWITCHES``, read from the envir
 ``_steps()`` binds the launches of that record.  Changing a switch afterwards does not change the engine; construct a new one.
 
 The reference runs the same step as ~200 engine ops (per-image im2col+SGEMM) + 20 ZMQ round trips (SURVEY §3.3-3.4).
-The public API a user calls is ``step(X_host, y_host) -> loss`` (H2D of the batch from pinned memory, graph replay, D2H of the loss).
+The public API a user calls is ``step(X_host, y_host, sample_weight=None) -> loss`` (H2D of the batch from pinned memory, graph replay, D2H of
+the loss), for any 1 <= n <= B rows: a short or sample-weighted batch runs the weighted instance of the kernel that produces the dlogits,
+which scales row i by its coefficient w_i * B / n (0 for the padding rows), in graphs of its own.
 
 The engine also scores its live weights: ``evaluate(X, y) -> (mean_loss, accuracy)`` (``evaluate_async`` returns a handle) and
 ``predict(X) -> logits`` run the whole forward pass of any number of images, the per-sample softmax-CE and the arg-max as ONE launch
@@ -176,23 +178,32 @@ def _unpack(buf, layout):
 
 
 class LossHandle:
-    """Result of ``HipsCNNTrainStep.step_async``: the per-sample losses of one step in pinned host memory + the event that guards them."""
+    """Result of ``HipsCNNTrainStep.step_async``: the per-sample losses of one step in pinned host memory + the event that guards them.
+    For a batch of ``n`` rows with sample weights ``w`` (``None``: unweighted), ``wait()`` returns the ``n`` values ``w_i * loss_i`` and
+    ``item()`` their mean over ``n``, as Gluon's losses weight them."""
 
-    __slots__ = ("_host", "_event")
+    __slots__ = ("_host", "_event", "_n", "_w")
 
-    def __init__(self, host, event):
-        self._host, self._event = host, event
+    def __init__(self, host, event, n=None, w=None):
+        self._host, self._event, self._n, self._w = host, event, n, w
+
+    def _values(self):
+        if self._n is None or (self._w is None and self._n == self._host.numel()):
+            return self._host
+        v = self._host[:self._n]
+        return v if self._w is None else v * self._w
 
     def wait(self):
         if self._event is not None:
             self._event.synchronize()
-        return self._host
+        return None if self._host is None else self._values()
 
     def item(self):
         if self._host is None:          # look-ahead engine, first call: no step has finished yet
             return float("nan")
         self._event.synchronize()
-        return float(self._host.sum()) / self._host.numel()
+        v = self._values()
+        return float(v.sum()) / v.numel()
 
     asscalar = item
 
@@ -378,9 +389,11 @@ class HipsCNNTrainStep:
         self._init_params(net)
         dev, f32 = self.device, torch.float32
         e = lambda *s, dt=f32: torch.empty(*s, dtype=dt, device=dev)
-        # the batch lives in ONE device buffer [x | label] so that the per-step staging -> compute hand-over is a single D2D copy
-        self.xin = e(B * 28 * 28 + B)
-        self.x, self.label = self.xin[:B * 784].view(B, 1, 28, 28), self.xin[B * 784:]
+        # the batch lives in ONE device buffer [x | label | coef] so that the per-step staging -> compute hand-over is a single D2D copy.
+        # coef [B] is the per-row gradient coefficient of a short or sample-weighted batch (see step_async); only weighted steps read it
+        self.xin = e(B * 28 * 28 + 2 * B)
+        self.x, self.lc = self.xin[:B * 784].view(B, 1, 28, 28), self.xin[B * 784:]
+        self.label, self.coef = self.lc[:B], self.lc[B:]
         self.a1, self.idx1 = e(B, 16, 12, 12), e(B, 16, 12, 12, dt=torch.uint8)
         self.col1 = e(B * 64, 400)
         self.z2 = e(B, 32, 8, 8)
@@ -391,13 +404,17 @@ class HipsCNNTrainStep:
         self.dl = e(B, 16)          # dlogits, classes padded to 16 (cluster kernel -> dense weight-gradient kernel)
         self.dz2rows, self.dcol1, self.da1 = e(B * 64, 32), e(B * 64, 400), e(B, 16, 12, 12)
         self.loss_host = torch.empty(B, dtype=f32).pin_memory()
-        # look-ahead: the head of the launch belongs to the PREVIOUS batch, whose labels must outlive the arrival of the next batch in `xin`
-        self.label_cur = torch.empty_like(self.label) if path.lookahead else self.label
+        # look-ahead: the head of the launch belongs to the PREVIOUS batch, whose labels and coefficients must outlive the arrival of the next
+        # batch in `xin`
+        self.lc_cur = torch.empty_like(self.lc) if path.lookahead else self.lc
+        self.label_cur, self.coef_cur = self.lc_cur[:B], self.lc_cur[B:]
         self.x_cur = torch.empty_like(self.x) if path.lookahead else self.x        # ... and so must its images (conv0's weight gradient reads them)
+        self._primed_batch = (False, B, None)   # look-ahead: (weighted, n, host weights) of the primed batch, whose loss the next launch reports
         self._primed = False
         self._warmed = False        # capture() has run its two eager warm-up steps
         self.graph = None
         self._graph_alt = None
+        self._graph_w = {}          # weighted steps: input buffer -> graph, captured on first use
         self._xbufs = [self.xin, None]
         self._side = torch.cuda.Stream(device=self.device)
         # the exchange branch gets a high-priority stream: its (few) CTAs must become resident at once on every rank — they poll each other —
@@ -461,21 +478,24 @@ class HipsCNNTrainStep:
             self._local_packed = (sp, h)
         native.arena_opt_h(h, self.Wl, grad_tensor, self.s0l, self.s1l, self.layout.total, self.fabric.tile_mult, self.opt_state, zero)
 
-    def _steps(self):
+    def _steps(self, weighted=False):
         """The training step of ``self.path`` as an ordered list of (name, stream, launch); `stream` is 'main', 'side' (parallel graph branch
         for weight gradients), 'comm' (a key group's exchange on the high-priority stream), 'join' (main, after the side branch) or 'join_comm'
-        (main, after the side branch and the comm stream).  The launches look their kernels, buffers and parameter blocks up when they run."""
+        (main, after the side branch and the comm stream).  The launches look their kernels, buffers and parameter blocks up when they run.
+        ``weighted``: the kernel that produces the dlogits scales row b by ``coef_cur[b]`` (its weighted instance); the launches are the same."""
         n, path = native, self.path
         B, P, G, f = self.B, self.P, self.G, self.fabric
         a2f = self.a2.view(B, 512)
         Wc1, Gc1 = P[2].view(32, 400), G[2].view(32, 400)
-        carry = (self.label, self.label_cur) if path.lookahead else None
+        # look-ahead: the forward launch carries the labels and coefficients of its batch to where the next launch's head reads them
+        carry = (self.lc, self.lc_cur) if path.lookahead else None
+        w = self.coef_cur if weighted else None
 
         # forward convolutions (the part a look-ahead launch runs for the NEXT batch)
         if path.dense in ("a3", "dz3"):
             def conv_fwd():
                 head = dict(wd1=P[6], bd1=P[7], wd2=P[8], bd2=P[9], label=self.label_cur, loss=self.loss, logits=self.logits, a4=self.a4,
-                            dz4=self.dz4, dz3=self.dz3, dl=self.dl) if path.dense == "dz3" else {}
+                            dz4=self.dz4, dz3=self.dz3, dl=self.dl, weight=w) if path.dense == "dz3" else {}
                 if not n.cnn_fwd_dense0(self.x, P[0], P[1], P[2], P[3], P[4], P[5], self.a1, self.idx1, self.a2, self.idx2, self.a3, carry=carry,
                                         x_keep=self.x_cur if path.lookahead else None, **head):
                     raise RuntimeError("cnn_fwd_dense0 does not cover batch %d" % B)
@@ -491,7 +511,7 @@ class HipsCNNTrainStep:
                     n.gemm(self.col1, Wc1, self.z2, bias=P[3], relu=True, store_nchw_hw=64)
                     n.maxpool2x2_fwd(self.z2, self.a2, self.idx2)
                 if path.lookahead:
-                    self.label_cur.copy_(self.label); self.x_cur.copy_(self.x)
+                    self.lc_cur.copy_(self.lc); self.x_cur.copy_(self.x)
             fwd = [(GEMM_FWD[0], "main", lambda: n.conv_relu_pool_im2col_fwd(self.x, P[0], P[1], self.a1, self.idx1, self.col1, 5, 5)),
                    (GEMM_FWD[1], "main", conv1_fwd)]
 
@@ -502,7 +522,7 @@ class HipsCNNTrainStep:
                 ("dense0 gemm", "main", lambda: n.gemm(a2f, P[4], self.a3, bias=P[5], relu=True)),
                 ("dense1 gemm", "main", lambda: n.gemm(self.a3, P[6], self.a4, bias=P[7], relu=True)),
                 ("head fwd+bwd", "main", lambda: n.head_fwd_bwd(self.a4, P[8], P[9], self.label_cur, self.loss, self.logits, G[8], G[9], self.dz4, G[7],
-                                                                True)),
+                                                                True, weight=w)),
                 ("dW1 gemm", "side", lambda: n.gemm(self.dz4, self.a3, G[6], a_mn=True, b_mn=True)),
                 ("dz3 gemm (mask,colsum)", "main", lambda: n.gemm(self.dz4, P[6], self.dz3, b_mn=True, mask=self.a3, colsum=G[5])),
                 ("dW0 gemm", "side", lambda: n.gemm(self.dz3, a2f, G[4], a_mn=True, b_mn=True)),
@@ -512,10 +532,11 @@ class HipsCNNTrainStep:
             # dense0 -> dense1 -> classifier -> softmax-CE forward and backward: one cluster launch for the data path (what the convolution
             # backward pass waits for) and one weight-gradient launch on a parallel branch, instead of the seven above
             dense = [(MLP, "main", lambda: n.mlp_chain_data(a2f, P[4], P[5], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits,
-                                                            self.da2, self.a3, self.a4, self.dz4, self.dz3, self.dl))]
+                                                            self.da2, self.a3, self.a4, self.dz4, self.dz3, self.dl, weight=w))]
         else:
             dense = [(MLP, "main", lambda: n.dense_tail(self.a3, P[4], P[6], P[7], P[8], P[9], self.label_cur, self.loss, self.logits, self.da2,
-                                                        self.a4, self.dz4, self.dz3, self.dl, from_dz3=path.dense == "dz3"))]
+                                                        self.a4, self.dz4, self.dz3, self.dl, from_dz3=path.dense == "dz3",
+                                                        weight=w if path.dense == "a3" else None))]
         if path.wgrad == "side":
             dense.append((DENSE_WGRAD, "side", wgrad))
 
@@ -570,9 +591,9 @@ class HipsCNNTrainStep:
         tail = [(LOCAL, "main", lambda: self._local_opt(f.param.tensor))] if path.local_tail else []
         return fwd + dense + comm + bwd + exchange + tail
 
-    def _body(self, stop_after=None, part="all"):
+    def _body(self, stop_after=None, part="all", weighted=False):
         """Issue the step (``part='all'``), only its forward convolutions (``'fwd'``), everything after them (``'rest'``), or the look-ahead
-        rotation ``rest(batch k) + fwd(batch k+1)`` (``'rotated'``)."""
+        rotation ``rest(batch k) + fwd(batch k+1)`` (``'rotated'``); ``weighted`` as in :meth:`_steps`."""
         before = native.launch_count
         f = self.fabric
         # the gradient arena is cleared by the previous step's HiPS kernel (fused zero_grad) unless gradients must stay readable
@@ -580,7 +601,7 @@ class HipsCNNTrainStep:
             f.grad.tensor.zero_()
         main, side, comm = torch.cuda.current_stream(), self._side, self._comm
         forked = comm_forked = False
-        steps = self._steps()
+        steps = self._steps(weighted)
         nf, join = self.path.n_fwd, self.path.lookahead_join
         rotated = steps[nf:] + [(name, join if where == "main" else where, fn) for name, where, fn in steps[:nf]]
         steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": rotated}[part]
@@ -612,9 +633,10 @@ class HipsCNNTrainStep:
         if part in ("all", "rotated"):
             self.kernels_per_step = native.launch_count - before
 
-    def capture(self):
+    def capture(self, weighted=False):
         """Warm up (2 eager steps on a side stream) and capture the step into a CUDA graph.  After ``set_learning_rate`` dropped the graphs,
-        only the capture runs: the warm-up steps are real updates and happen once per engine."""
+        only the capture runs: the warm-up steps are real updates and happen once per engine (``weighted``: on the batch in the input buffer
+        with its coefficients, see :meth:`_steps`)."""
         if self.graph is not None or not self.use_graph:
             return
         if not self._warmed:
@@ -622,7 +644,7 @@ class HipsCNNTrainStep:
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
                 for _ in range(2):
-                    self._body()
+                    self._body(weighted=weighted)
                     self.steps_done += 1
             torch.cuda.current_stream().wait_stream(s)
             torch.cuda.synchronize()
@@ -639,6 +661,7 @@ class HipsCNNTrainStep:
             self._body(part="rotated" if self.lookahead else "all")
         self.graph = g
         self._graph_alt = None
+        self._graph_w = {}
 
     # learning rate ---------------------------------------------------------------------------------------------------
     @property
@@ -678,6 +701,7 @@ class HipsCNNTrainStep:
             self.fabric.set_optimizer(dict(self.fabric.opt_spec, lr=self._lr))
         self.graph = None
         self._graph_alt = None
+        self._graph_w = {}
 
     def _prime(self):
         """Look-ahead: run the forward convolutions of the batch in ``self.x`` so that the next launch can start at the classifier head."""
@@ -689,10 +713,15 @@ class HipsCNNTrainStep:
         """Look-ahead: train on the batch whose convolutions are already done (the last one enqueued) and return its mean loss."""
         if not (self.lookahead and self._primed):
             return None
-        self._body(part="rest")
+        weighted, n, w = self._primed_batch
+        self._body(part="rest", weighted=weighted)
         self._primed = False
+        self._primed_batch = (False, self.B, None)
         self.steps_done += 1
-        return float(self.loss.mean())
+        if not weighted:
+            return float(self.loss.mean())
+        loss = self.loss[:n].cpu()
+        return float((loss if w is None else loss * w).sum()) / n
 
     # checkpoints -----------------------------------------------------------------------------------------------------
     def save_states(self, fname):
@@ -702,8 +731,9 @@ class HipsCNNTrainStep:
         ``build_cnn().load_parameters(fname, ignore_extra=True)`` loads them), and per parameter ``master:`` / ``s0:`` / ``s1:`` /
         ``step:`` (the master weight, both optimizer state slots and the update count: one per key, one per tile with ``dist_async``; with
         ``update='local'`` the worker's own), ``bsc_u:`` / ``bsc_v:`` (Bi-Sparse residuals of every rank), ``dgt_contrib:`` / ``dgt_fmt:``
-        and ``dgt:order`` (the DGT ranking), ``batch:x`` / ``batch:label`` (a look-ahead engine's primed batch, one row per rank), and a
-        ``meta:`` block.  The state is keyed by parameter, whichever rank holds it; what belongs to a worker (HFA's state, the primed
+        and ``dgt:order`` (the DGT ranking), ``batch:x`` / ``batch:label`` (a look-ahead engine's primed batch, one row per rank) and
+        ``batch:weight`` (its gradient coefficients ``w_i * B / n``, 0 for padding rows; written only when a rank's primed batch was short or
+        weighted, an absent entry meaning all ones), and a ``meta:`` block.  The state is keyed by parameter, whichever rank holds it; what belongs to a worker (HFA's state, the primed
         batches) has one row per rank.
 
         Several ranks: collective, every rank calls it; rank 0 writes the file, and every rank raises if that fails."""
@@ -729,7 +759,9 @@ class HipsCNNTrainStep:
         that has not captured yet runs its warm-up and capture first, so that the warm-up updates do not land on the loaded state).  When
         the file's constant lr differs from the engine's, it is applied through :meth:`set_learning_rate`, which drops the graphs.  A
         look-ahead engine with the saver's batch size, world size and parties primes each rank's own saved batch again; any other engine
-        does not train on the saved batches and warns (``flush()`` before saving avoids that).
+        does not train on the saved batches and warns (``flush()`` before saving avoids that).  A restored short or weighted batch trains with
+        its saved coefficients; the loss the next step reports for it is the mean over ``B`` of ``coef_i * loss_i``, which equals the mean over
+        its ``n`` rows of ``w_i * loss_i``.
 
         The saving and the loading engine may differ in batch size, world size, parties, global servers and look-ahead; the optimizer kind,
         ``update``, ``mode``, HFA and the accelerators (wire formats, Bi-Sparse, DGT) must match, and HFA and Bi-Sparse also need the same
@@ -741,22 +773,24 @@ class HipsCNNTrainStep:
         meta, layout = self._ckpt_meta(), self._ckpt_layout()
         batch = [("batch:x", (self.topo.world, self.B, 1, 28, 28), np.dtype(np.float32)),
                  ("batch:label", (self.topo.world, self.B), np.dtype(np.float32))]
-        data, err, use_batch = None, None, False
+        data, err, use_batch, use_weight = None, None, False, False
         if self.topo.rank == 0:
             try:
                 data = self._ckpt_read(fname, meta, layout)
-                use_batch = "batch:x" in data
+                use_batch, use_weight = "batch:x" in data, "batch:weight" in data
             except Exception as e:                          # other ranks must not wait for a payload that never comes
                 err = e
         if self.topo.world > 1:
             import torch.distributed as dist
-            status = torch.tensor([err is None, use_batch], dtype=torch.int32, device=self.device)
+            status = torch.tensor([err is None, use_batch, use_weight], dtype=torch.int32, device=self.device)
             dist.broadcast(status, src=0)
             if err is None and not bool(status[0]):
                 raise ValueError("%s: the checkpoint was refused on rank 0" % fname)
-            use_batch = bool(status[1])
+            use_batch, use_weight = bool(status[1]), bool(status[2])
         if err is not None:
             raise err
+        if use_weight:
+            batch.append(("batch:weight", (self.topo.world, self.B), np.dtype(np.float32)))
         order = [(n, s, dt) for n, (s, dt) in layout.items()] + (batch if use_batch else [])
         if self.topo.world > 1:
             buf = _pack([data[n] for n, _, _ in order]) if self.topo.rank == 0 else \
@@ -772,10 +806,16 @@ class HipsCNNTrainStep:
             self.capture()
         self._ckpt_apply(data)
         self._primed = False
+        self._primed_batch = (False, self.B, None)
         if use_batch:
             self.x.copy_(torch.from_numpy(data["batch:x"][self.topo.rank]))
             self.label.copy_(torch.from_numpy(data["batch:label"][self.topo.rank]))
+            c = data["batch:weight"][self.topo.rank] if use_weight else None
+            weighted = c is not None and not bool((c == 1).all())
+            if weighted:
+                self.coef.copy_(torch.from_numpy(c))
             self._prime()
+            self._primed_batch = (weighted, self.B, torch.from_numpy(c.copy()) if weighted else None)
         torch.cuda.synchronize(self.device)
 
     def _ckpt_meta(self):
@@ -859,6 +899,10 @@ class HipsCNNTrainStep:
         if with_batch and self.lookahead and self._primed:
             out["batch:x"] = np.stack(f.gather_ranks(self.x_cur))
             out["batch:label"] = np.stack(f.gather_ranks(self.label_cur))
+            coef = self.coef_cur if self._primed_batch[0] else torch.ones_like(self.coef_cur)
+            coef = np.stack(f.gather_ranks(coef))
+            if not (coef == 1).all():
+                out["batch:weight"] = coef
         return out
 
     def _ckpt_read(self, fname, meta, layout):
@@ -928,13 +972,20 @@ class HipsCNNTrainStep:
                 fmt, b = out["dgt_fmt:" + n], base[t0:t0 + len(out["dgt_fmt:" + n])]
                 if not np.where(b == self.fabric.FMT_BSC, fmt == b, (fmt == b) | (fmt == self.fabric.FMT_F8)).all():
                     raise ValueError("dgt_fmt:%s: formats other than the base format or its fp8 demotion" % n)
+        if "batch:weight" in got and "batch:x" not in got:
+            raise ValueError("batch:weight without the primed batch batch:x / batch:label it belongs to")
         if "batch:x" in got or "batch:label" in got:
             x, y = got.get("batch:x"), got.get("batch:label")
             if x is None or y is None or x.dtype != np.float32 or y.dtype != np.float32 or x.ndim != 5 or x.shape[2:] != (1, 28, 28) \
                     or y.shape != x.shape[:2] or x.shape[0] != int(got["meta:topology"][0]):
                 raise ValueError("batch:x / batch:label: not one batch of (B, 1, 28, 28) fp32 images and B fp32 labels per saving rank")
+            wt = got.get("batch:weight")
+            if wt is not None and (wt.dtype != np.float32 or wt.shape != y.shape):
+                raise ValueError("batch:weight: not one fp32 gradient coefficient per row of batch:label")
             if self.lookahead and same_ranks and x.shape[1] == self.B:
                 out["batch:x"], out["batch:label"] = x, y
+                if wt is not None:
+                    out["batch:weight"] = wt
             else:
                 import warnings
                 warnings.warn("%s holds the primed batches of %d ranks of batch size %d, which this engine does not train on (it restores "
@@ -982,9 +1033,10 @@ class HipsCNNTrainStep:
         launches are being issued or captured: a captured graph keeps the buffer it was captured with."""
         buf = self._xbufs[k]
         B = self.B
-        self.xin, self.x, self.label = buf, buf[:B * 784].view(B, 1, 28, 28), buf[B * 784:]
+        self.xin, self.x, self.lc = buf, buf[:B * 784].view(B, 1, 28, 28), buf[B * 784:]
+        self.label, self.coef = self.lc[:B], self.lc[B:]
         if not self.lookahead:
-            self.x_cur, self.label_cur = self.x, self.label
+            self.x_cur, self.lc_cur, self.label_cur, self.coef_cur = self.x, self.lc, self.label, self.coef
 
     def _alt_graph(self):
         """The same step captured on input buffer 1: the host pipeline alternates between the two graphs, so a batch is consumed where the
@@ -1004,9 +1056,30 @@ class HipsCNNTrainStep:
             self._graph_alt = g
         return self._graph_alt
 
-    def run_device(self, buf=0):
+    def _weighted_graph(self, k):
+        """The step with the weighted instances of its dlogits kernel (see :meth:`_steps`), captured on input buffer ``k`` on first use, as
+        :meth:`_alt_graph` does: no warm-up steps, nothing collective.  The unweighted graphs stay as they are.  The capture is relaxed: it
+        may be the first launch of a weighted kernel, whose one-time set-up (shared-memory size, cluster occupancy) runs then."""
+        g = self._graph_w.get(k)
+        if g is None:
+            self._bind_input(k)
+            try:
+                s = torch.cuda.Stream()
+                s.wait_stream(torch.cuda.current_stream())
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.stream(s):
+                    with torch.cuda.graph(g, stream=s, capture_error_mode="relaxed"):
+                        self._body(part="rotated" if self.lookahead else "all", weighted=True)
+                torch.cuda.current_stream().wait_stream(s)
+            finally:
+                self._bind_input(0)
+            self._graph_w[k] = g
+        return g
+
+    def run_device(self, buf=0, weighted=False):
         """One step on whatever is currently in input buffer ``buf`` (0: ``self.x`` / ``self.label``; device-only, used by the kernel-time
-        bench and by the host pipeline)."""
+        bench and by the host pipeline).  ``weighted``: the step scales the gradient of row b by ``coef[b]`` of its input buffer (with
+        look-ahead, of the primed batch, carried to ``coef_cur``)."""
         # DGT: re-rank before every step whose count of steps already taken (graph warm-up steps included) is a positive multiple of
         # dgt_rerank_every, eager or graphed; capture() also ranks once after its warm-up.  Outside any captured graph: the order and the
         # formats are updated in place
@@ -1014,21 +1087,24 @@ class HipsCNNTrainStep:
             self.fabric.dgt_rerank()
         if self.use_graph:
             if self.graph is None:
-                self.capture()
+                self.capture(weighted)
             if self.lookahead:
                 self._prime()
-            (self._alt_graph() if buf == 1 else self.graph).replay()
+            if weighted:
+                self._weighted_graph(buf).replay()
+            else:
+                (self._alt_graph() if buf == 1 else self.graph).replay()
         elif buf == 1:
             self._bind_input(1)
             try:
-                self._body()
+                self._body(weighted=weighted)
             finally:
                 self._bind_input(0)
         elif self.lookahead:
             self._prime()
-            self._body(part="rotated")
+            self._body(part="rotated", weighted=weighted)
         else:
-            self._body()
+            self._body(weighted=weighted)
         self.steps_done += 1
         if self.hfa and self.steps_done % self.hfa[0] == 0:
             self._hfa_sync(global_round=(self.steps_done // self.hfa[0]) % self.hfa[1] == 0)
@@ -1063,53 +1139,126 @@ class HipsCNNTrainStep:
                 stage = [torch.empty_like(self.xin) for _ in range(2)]
             self._pl = {
                 "h2d": torch.cuda.Stream(device=dev), "d2h": torch.cuda.Stream(device=dev), "stage": stage,
-                "sx": [s[:B * 784].view(B, 1, 28, 28) for s in stage], "sy": [s[B * 784:] for s in stage],
+                "sx": [s[:B * 784].view(B, 1, 28, 28) for s in stage], "sy": [s[B * 784:B * 785] for s in stage],
+                "sc": [s[B * 785:] for s in stage],
+                # what the staging -> compute copy of an unweighted step covers: the images and labels, not the coefficients
+                "xl": self.xin[:B * 785], "stage_xl": [s[:B * 785] for s in stage],
                 "ready": [torch.cuda.Event() for _ in range(2)], "done": [torch.cuda.Event() for _ in range(2)],
                 "ring": [(torch.empty_like(self.loss, device="cpu").pin_memory(), torch.cuda.Event()) for _ in range(4)], "n": 0, "last_loss": None,
             }
         return self._pl
 
-    def step_async(self, X, y):
+    def _coefficients(self, dst, w, n):
+        """Write the gradient coefficients of a batch of ``n`` rows into ``dst`` [B] on the current stream: ``w_i * B / n`` for the real rows
+        (``w_i = 1`` when ``w`` is None), 0 for the padding rows.  With the push scale 1 / B the step then contributes
+        ``(1/n) * sum_i w_i * grad_i``, the reference loop's ``grad / num_samples`` of a weighted loss."""
+        B = self.B
+        if w is not None and w.is_cuda:
+            dst[n:].zero_()
+            dst[:n].copy_(w.reshape(n), non_blocking=True)
+            dst[:n].mul_(B / n)
+            return
+        c = torch.zeros(B, dtype=torch.float32)
+        if w is None:
+            c[:n] = B / n
+        else:
+            c[:n] = w.reshape(n).float() * (B / n)
+        dst.copy_(c.pin_memory(), non_blocking=True)
+
+    def step_async(self, X, y, sample_weight=None):
         """Public API: enqueue one training step and return a :class:`LossHandle` without waiting for the GPU (the MXNet engine's contract:
-        an op returns at once, ``asscalar()`` synchronises).  ``X`` (B,1,28,28) and ``y`` (B,) are host tensors / NDArrays (pinned → async
-        H2D) or device tensors.
+        an op returns at once, ``asscalar()`` synchronises).  ``X`` (n,1,28,28) or (n,784) and ``y`` (n,), ``1 <= n <= B``, are host tensors /
+        NDArrays (pinned → async H2D) or device tensors; so is ``sample_weight`` (n,) when given.
+
+        A batch of ``n`` rows with weights ``w`` (``w_i = 1`` without ``sample_weight``) contributes the gradient ``(1/n) * sum_i w_i grad_i``
+        in every update mode, as the reference loop's ``loss_fn(net(X), y, sample_weight).backward(); kv.push(idx, grad / n)`` does; the
+        last, short batch of an epoch (``DataLoader(..., last_batch='keep')``) trains on its own rows.  The step pads the batch to ``B`` rows
+        with zero images of label 0 and gives each row the coefficient ``w_i * B / n`` (0 for the padding rows), which the kernel producing
+        the dlogits applies.  The handle reports ``w_i * loss_i`` of the ``n`` rows.  A full batch without weights runs exactly the step it
+        ran before weights existed.  Ranks may pass different ``n`` and weights in the same step.  ``n`` outside ``[1, B]`` or ``y`` /
+        ``sample_weight`` of another length raise ``ValueError`` before anything is enqueued; weights are not checked for finiteness.
 
         Three streams: the batch is copied host→device on a copy stream into one of the step's TWO input buffers (overlapping the previous
         step's compute); the compute stream replays the graph that was captured on that buffer (two graphs of the same step, alternating —
         no staging→compute copy; ``GEOMX_E2E_DIRECT_INPUT=0`` and look-ahead steps use one graph plus a device-to-device copy), and the
         per-sample loss goes device→host on a third stream into a pinned ring slot; ``handle.item()`` waits for exactly that copy.  A
-        training loop therefore launches step i+1 before it reads the loss of step i."""
+        training loop therefore launches step i+1 before it reads the loss of step i.  Weighted and short steps replay graphs of their own,
+        captured on first use."""
         X = X._t if isinstance(X, NDArray) else X
         y = y._t if isinstance(y, NDArray) else y
+        w = sample_weight._t if isinstance(sample_weight, NDArray) else sample_weight
+        B = self.B
+        n = int(X.shape[0]) if X.dim() > 0 else 0
+        if not 1 <= n <= B or X.numel() != n * 784:
+            raise ValueError("X must be (n, 1, 28, 28) or (n, 784) with 1 <= n <= %d (the batch size), got %s" % (B, tuple(X.shape)))
+        if y.numel() != n:
+            raise ValueError("y must hold one label per image: %d labels for %d images" % (y.numel(), n))
+        if w is not None and w.numel() != n:
+            raise ValueError("sample_weight must hold one weight per image: %d weights for %d images" % (w.numel(), n))
+        weighted = w is not None or n < B
         pl = self._pipeline()
         i = pl["n"]; b = i % 2
         pl["n"] = i + 1
         main = torch.cuda.current_stream()
+        # a short batch fills the first n rows of the input buffer and clears the rest; a full one is copied as it always was
         if X.is_cuda:
-            self.x.copy_(X.reshape(self.x.shape), non_blocking=True)
-            self.label.copy_(y.reshape(self.label.shape), non_blocking=True)
+            if n < B:
+                self.x[:n].copy_(X.reshape(n, 1, 28, 28), non_blocking=True)
+                self.label[:n].copy_(y.reshape(n), non_blocking=True)
+                self.x[n:].zero_(); self.label[n:].zero_()
+            else:
+                self.x.copy_(X.reshape(self.x.shape), non_blocking=True)
+                self.label.copy_(y.reshape(self.label.shape), non_blocking=True)
+            if weighted:
+                self._coefficients(self.coef, w, n)
         else:
             h2d = pl["h2d"]
             if i >= 2:
                 h2d.wait_event(pl["done"][b])              # staging buffer b was handed over by step i-2
+            if w is not None and w.is_cuda:
+                h2d.wait_stream(main)                      # the weights come from work on the compute stream
             with torch.cuda.stream(h2d):
-                pl["sx"][b].copy_(X.reshape(self.x.shape), non_blocking=True)
-                pl["sy"][b].copy_(y.reshape(self.label.shape), non_blocking=True)
+                if n < B:
+                    pl["sx"][b][:n].copy_(X.reshape(n, 1, 28, 28), non_blocking=True)
+                    pl["sy"][b][:n].copy_(y.reshape(n), non_blocking=True)
+                    pl["sx"][b][n:].zero_(); pl["sy"][b][n:].zero_()
+                else:
+                    pl["sx"][b].copy_(X.reshape(self.x.shape), non_blocking=True)
+                    pl["sy"][b].copy_(y.reshape(self.label.shape), non_blocking=True)
+                if weighted:
+                    self._coefficients(pl["sc"][b], w, n)
                 pl["ready"][b].record(h2d)
             main.wait_event(pl["ready"][b])
             if not self.path.direct_input:
-                self.xin.copy_(pl["stage"][b], non_blocking=True)
+                if weighted:
+                    self.xin.copy_(pl["stage"][b], non_blocking=True)
+                else:
+                    pl["xl"].copy_(pl["stage_xl"][b], non_blocking=True)
+        w_host = None
+        if w is not None:
+            # the weights the loss is reported with (a host copy, taken in stream order when they live on the device)
+            if w.is_cuda:
+                w_host = torch.empty(n, dtype=torch.float32).pin_memory()
+                w_host.copy_(w.reshape(n), non_blocking=True)
+            else:
+                w_host = w.reshape(n).float().clone()
         if pl["last_loss"] is not None:
             main.wait_event(pl["last_loss"])                # the loss buffer of the previous step has been read out
         if self.lookahead and not self._primed:
             # first batch of a look-ahead run: only its convolutions can run yet (after the graph warm-up, which also uses this batch);
             # there is no finished step to report
             if self.use_graph and self.graph is None:
-                self.capture()
+                self.capture(weighted)
             self._prime()
+            self._primed_batch = (weighted, n, w_host)
             pl["done"][b].record(main)
             return LossHandle(None, None)
-        self.run_device(buf=b if (not X.is_cuda and self.path.direct_input) else 0)
+        if self.lookahead:
+            # the launch trains the primed batch (its head runs now) and primes this one
+            (run_weighted, ln, lw), self._primed_batch = self._primed_batch, (weighted, n, w_host)
+        else:
+            run_weighted, ln, lw = weighted, n, w_host
+        self.run_device(buf=b if (not X.is_cuda and self.path.direct_input) else 0, weighted=run_weighted)
         pl["done"][b].record(main)
         host, ev = pl["ring"][i % 4]
         d2h = pl["d2h"]
@@ -1118,11 +1267,12 @@ class HipsCNNTrainStep:
             host.copy_(self.loss, non_blocking=True)
             ev.record(d2h)
         pl["last_loss"] = ev
-        return LossHandle(host, ev)
+        return LossHandle(host, ev, ln, lw)
 
-    def step(self, X, y):
-        """Public API: one training step; returns the mean loss as a Python float (forces the D2H read of the per-sample loss)."""
-        return self.step_async(X, y).item()
+    def step(self, X, y, sample_weight=None):
+        """Public API: one training step; returns the mean (weighted) loss as a Python float (forces the D2H read of the per-sample loss).
+        Arguments as in :meth:`step_async`."""
+        return self.step_async(X, y, sample_weight).item()
 
     # evaluation -----------------------------------------------------------------------------------------------------
     def _eval_launch(self, X, y, want_logits=False):

@@ -104,31 +104,39 @@ def mlp_chain(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dw0, db0, dw1, db1
     return True
 
 
-def mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, dz4, dz3, dl):
+def _weight(weight, B):
+    assert weight is None or (weight.shape == (B,) and weight.is_cuda and weight.dtype == torch.float32 and weight.is_contiguous())
+    return _p(weight)
+
+
+def mlp_chain_data(x, w0, b0, w1, b1, w2, b2, label, loss, logits, dx, a3, a4, dz4, dz3, dl, weight=None):
     """The data path of the dense chain in ONE cluster launch: per-sample loss, logits and dx; it also stores what :func:`dense_wgrad` reads:
-    a3 [B,D1], a4 [B,D2], dz4 [B,D2], dz3 [B,D1] and the dlogits dl [B,16].  Returns False for shapes other than 512 -> 256 -> 128 -> C<=16,
-    batch <= 32."""
+    a3 [B,D1], a4 [B,D2], dz4 [B,D2], dz3 [B,D1] and the dlogits dl [B,16].  ``weight`` [B] (fp32): the dlogits of row b are scaled by
+    ``weight[b]`` before anything is derived from them (the weighted instance of the kernel); the loss is not.  Returns False for shapes
+    other than 512 -> 256 -> 128 -> C<=16, batch <= 32."""
     B, D0 = x.shape
     D1, D2, C = w0.shape[0], w1.shape[0], w2.shape[0]
     rc = _lib().gx_mlp_chain(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dx),
-                             _p(a3), _p(a4), _p(dz4), _p(dz3), _p(dl), B, D0, D1, D2, C, _s())
+                             _p(a3), _p(a4), _p(dz4), _p(dz3), _p(dl), _weight(weight, B), B, D0, D1, D2, C, _s())
     if rc == -1:
         return False
     _ck(rc, "mlp_chain")
     return True
 
 
-def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl, from_dz3=False):
+def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl, from_dz3=False, weight=None):
     """The data path of the dense chain from a3 [B,D1] on (what :func:`cnn_fwd_dense0` computed), in ONE cluster launch: per-sample loss,
     logits and dx [B,D0]; it also stores a4, dz4, dz3 and the dlogits dl [B,16] for :func:`dense_wgrad` (a3 is already in memory).  ``w0``
     [D1,D0] is read for dx only.  ``from_dz3=True``: dz3 [B,D1] is the input (what :func:`cnn_fwd_dense0`'s training head computed) and the
-    launch computes dx = dz3 · w0 only; the other buffers are neither read nor written.  Returns False for shapes other than
-    512 -> 256 -> 128 -> C<=16, batch <= 32."""
+    launch computes dx = dz3 · w0 only; the other buffers are neither read nor written.  ``weight`` [B] (not with ``from_dz3``, whose dz3
+    already carries it) scales the dlogits as in :func:`mlp_chain_data`.  Returns False for shapes other than 512 -> 256 -> 128 -> C<=16,
+    batch <= 32."""
     B, D1 = dz3.shape
     D0, D2, C = w0.shape[1], w1.shape[0], w2.shape[0]
     assert w0.shape[0] == D1 and dx.shape == (B, D0) and dl.shape == (B, 16) and dz3.is_contiguous()
+    assert weight is None or not from_dz3, "from_dz3: the weights are applied where dz3 is computed"
     rc = _lib().gx_dense_tail(_p(a3), _p(w0), _p(w1), _p(b1), _p(w2), _p(b2), _p(label), _p(loss), _p(logits), _p(dx), _p(a4), _p(dz4), _p(dz3),
-                              _p(dl), B, D0, D1, D2, C, int(bool(from_dz3)), _s())
+                              _p(dl), _weight(weight, B), B, D0, D1, D2, C, int(bool(from_dz3)), _s())
     if rc == -1:
         return False
     _ck(rc, "dense_tail")
@@ -157,7 +165,7 @@ def cnn_fwd(x, w0, b0, w1, b1, a1, idx1, a2, idx2, carry=None, x_keep=None):
 
 
 def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None, x_keep=None, *, wd1=None, bd1=None, wd2=None, bd2=None,
-                   label=None, loss=None, logits=None, a4=None, dz4=None, dz3=None, dl=None):
+                   label=None, loss=None, logits=None, a4=None, dz4=None, dz3=None, dl=None, weight=None):
     """:func:`cnn_fwd` followed by the first dense layer in the same launch: also a3 [B,256] = relu(a2.view(B,512) · wdᵀ + bd), with
     wd [256,512].  ``carry`` / ``x_keep`` as in :func:`cnn_fwd`.  Runs clusters of two images: returns False without launching for odd B or
     B > 32.
@@ -165,8 +173,11 @@ def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None
     With ``a4`` given, the same launch also runs the rest of the dense chain's row-separable part (the training head): dense1 (``wd1``
     [128,256], ``bd1``), the classifier (``wd2`` [10,128], ``bd2``) and softmax-CE against ``label`` [B] (float class ids), and the data
     gradients down to dz3.  It writes loss [B], logits [B,10] (skipped when None), a4 [B,128], dz4 [B,128], dz3 [B,256] and the dlogits
-    dl [B,16] (classes >= 10 zero): what :func:`dense_tail` with ``from_dz3=True`` and :func:`dense_wgrad` read."""
+    dl [B,16] (classes >= 10 zero): what :func:`dense_tail` with ``from_dz3=True`` and :func:`dense_wgrad` read.  ``weight`` [B] (with the
+    head only) scales the dlogits of row b by ``weight[b]`` before dz4 and dz3 are derived from them (the weighted instance of the kernel);
+    the loss is not."""
     B = x.shape[0]
+    assert weight is None or a4 is not None, "weight scales the training head's dlogits"
     assert wd.shape == (256, 512) and a3.shape == (B, 256) and a3.is_contiguous()
     head = (wd1, bd1, wd2, bd2, label, loss, logits, a4, dz4, dz3, dl)
     if a4 is not None:
@@ -177,7 +188,7 @@ def cnn_fwd_dense0(x, w0, b0, w1, b1, wd, bd, a1, idx1, a2, idx2, a3, carry=None
     src, dst = carry if carry is not None else (None, None)
     rc = _lib().gx_cnn_fwd_dense0(_p(x), _p(w0), _p(b0), _p(w1), _p(b1), _p(wd), _p(bd), _p(a1), _p(idx1), _p(a2), _p(idx2), _p(a3), _p(src),
                                   _p(dst), 0 if src is None else src.numel(), _p(x_keep),
-                                  *(_p(t) if a4 is not None else None for t in head), B, _s())
+                                  *(_p(t) if a4 is not None else None for t in head), _weight(weight, B), B, _s())
     if rc == -1:
         return False
     _ck(rc, "cnn_fwd_dense0")
@@ -406,11 +417,13 @@ def softmax_ce_bwd(logits, label, dloss, out=None):
     return out
 
 
-def head_fwd_bwd(a, W, bias, label, loss, logits, dW, db, da, dbias_prev, relu_mask=True):
+def head_fwd_bwd(a, W, bias, label, loss, logits, dW, db, da, dbias_prev, relu_mask=True, weight=None):
+    """Classifier head forward and backward in one launch (csrc/kernels/loss_head.cu).  ``weight`` [B] (fp32): the dlogits of sample b are
+    scaled by ``weight[b]`` before dW, db, da and dbias_prev are derived from them (the weighted instance of the kernel); the loss is not."""
     B, K = a.shape
     Cc = W.shape[0]
     _ck(_lib().gx_head_fwd_bwd(_p(a), _p(W), _p(bias), _p(label), _p(loss), _p(logits), _p(dW), _p(db), _p(da), _p(dbias_prev),
-                               B, K, Cc, int(relu_mask), _s()), "head_fwd_bwd")
+                               _weight(weight, B), B, K, Cc, int(relu_mask), _s()), "head_fwd_bwd")
 
 
 # --------------------------------------------------------------------------------------------------------------- optimizers

@@ -7,11 +7,11 @@ SIGS = {
     # gemm_wgmma.cu
     "gx_gemm_tf32": [P, L, I, P, L, I, I, I, I, P, L, P, P, L, P, I, I, I, I, F, I, P],
     "gx_gemm_tf32_pool": [P, L, I, P, L, I, I, I, I, P, P, I, I, I, P, F, P],
-    "gx_mlp_chain": [P] * 16 + [I] * 5 + [P],
+    "gx_mlp_chain": [P] * 17 + [I] * 5 + [P],
     "gx_dense_wgrad": [P] * 12 + [I] * 5 + [P],
-    "gx_dense_tail": [P] * 14 + [I] * 6 + [P],
+    "gx_dense_tail": [P] * 15 + [I] * 6 + [P],
     "gx_cnn_fwd": [P] * 11 + [I, P, I, P],
-    "gx_cnn_fwd_dense0": [P] * 14 + [I] + [P] * 12 + [I, P],
+    "gx_cnn_fwd_dense0": [P] * 14 + [I] + [P] * 13 + [I, P],
     "gx_cnn_bwd": [P] * 9 + [I, P],
     "gx_cnn_wgrad1": [P] * 6 + [I, P],
     "gx_cnn_bwd_all": [P] * 11 + [I, P],
@@ -47,7 +47,7 @@ SIGS = {
     # loss_head.cu
     "gx_softmax_ce_fwd": [P, P, P, I, I, P],
     "gx_softmax_ce_bwd": [P, P, P, P, I, I, P],
-    "gx_head_fwd_bwd": [P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
+    "gx_head_fwd_bwd": [P] * 11 + [I, I, I, I, P],
     # optim.cu
     "gx_arena_opt": [I, P, P, P, P, L, P, F, F, F, F, F, F, F, F, F, P, P, P, P],
     "gx_multi_tensor_opt": [I, P, I, L, F, F, F, F, F, F, F, F, F, P],
