@@ -3,8 +3,9 @@
 // running = momentum*running + (1-momentum)*batch  (:262-266, population variance :355-362).
 //
 // Two forms.  Feature maps (N*HW >= 4096, HW >= 16) are bandwidth problems and use the SPLIT form: a statistics kernel on a (channel, slice)
-// grid that fills the machine (one pass over x: sum and sum of squares per thread in fp32, combined across CTAs with fp64 atomics; the CTA that
-// draws the last ticket of a channel finalises mean / inv-std / running statistics and re-arms the accumulators), then an apply kernel that
+// grid that fills the machine (one pass over x: sum and sum of squares of x minus a per-channel pivot per thread in fp32, combined across
+// CTAs with fp64 atomics; the CTA that draws the last ticket of a channel finalises mean / inv-std / running statistics and re-arms the
+// accumulators), then an apply kernel that
 // streams every (image, channel) plane with 128-bit accesses.  x is read twice and y written once — 3 passes at HBM rate instead of the 4
 // strided passes of a one-CTA-per-channel kernel.
 // Small problems (Dense + BN, tiny maps) keep the one-CTA-per-channel kernels: they are latency-bound and one launch beats two.
@@ -67,7 +68,8 @@ __global__ void __launch_bounds__(512) bn_fwd_kernel(const float* __restrict__ x
 
 __global__ void __launch_bounds__(512) bn_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ gamma,
                                                       const float* __restrict__ save_mean, const float* __restrict__ save_invstd,
-                                                      float* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta, int N, int C, int HW) {
+                                                      float* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta, int N, int C, int HW,
+                                                      int fixed_stats) {
   gx::pdl_wait();
   gx::pdl_launch();
   __shared__ float red[16];
@@ -91,6 +93,7 @@ __global__ void __launch_bounds__(512) bn_bwd_kernel(const float* __restrict__ x
   const float k = g * invstd, inv_cnt = 1.f / (float)cnt;
   for (long long i = threadIdx.x; i < cnt; i += blockDim.x) {
     const long long o = ((i / HW) * C + c) * HW + i % HW;
+    if (fixed_stats) { dx[o] = k * dy[o]; continue; }
     const float xh = (x[o] - mean) * invstd;
     dx[o] = k * (dy[o] - (sdy + xh * sdyx) * inv_cnt);
   }
@@ -111,6 +114,8 @@ __device__ __forceinline__ void bn_block_sum2(float& u, float& v, float* red) {
 }
 
 // grid (C, S), 256 threads: CTA (c, s) covers images s, s+S, ...
+// Every CTA of a channel accumulates x - p for the same pivot p = x[0, c, 0], so the fp32 partial sums stay of the size of the spread of x,
+// not of its mean: E[x^2] - mean^2 of raw values loses the variance to cancellation once |mean| / std is in the hundreds.
 __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__ x, float* __restrict__ running_mean, float* __restrict__ running_var,
                                                         float* __restrict__ save_mean, float* __restrict__ save_invstd, BnAcc* __restrict__ acc,
                                                         int* __restrict__ tickets, int N, int C, int HW, float momentum, float eps) {
@@ -118,13 +123,18 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
   gx::pdl_launch();
   __shared__ float red[32];
   const int c = blockIdx.x, S = gridDim.y;
+  const float p = __ldg(x + (long long)c * HW);
   float s = 0.f, q = 0.f;
   if ((HW & 3) == 0) {
     // flattened (image, 128-bit chunk) index: all 256 threads stay busy whatever HW is, four independent loads in flight per thread
     const int hw4 = HW >> 2, imgs = (N - (int)blockIdx.y + S - 1) / S, total = imgs * hw4;
     const long long img_stride = (long long)S * C * HW;
     const float* base = x + ((long long)blockIdx.y * C + c) * HW;
-    auto at = [&](int j) { const int k = j / hw4; return __ldg(reinterpret_cast<const float4*>(base + k * img_stride) + (j - k * hw4)); };
+    auto at = [&](int j) {
+      const int k = j / hw4;
+      const float4 v = __ldg(reinterpret_cast<const float4*>(base + k * img_stride) + (j - k * hw4));
+      return make_float4(v.x - p, v.y - p, v.z - p, v.w - p);
+    };
     int j = threadIdx.x;
     for (; j + 768 < total; j += 1024) {
       const float4 v0 = at(j), v1 = at(j + 256), v2 = at(j + 512), v3 = at(j + 768);
@@ -141,8 +151,8 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
     }
   } else {
     for (int n = blockIdx.y; n < N; n += S) {
-      const float* p = x + ((long long)n * C + c) * HW;
-      for (int i = threadIdx.x; i < HW; i += 256) { const float v = __ldg(p + i); s += v; q = fmaf(v, v, q); }
+      const float* px = x + ((long long)n * C + c) * HW;
+      for (int i = threadIdx.x; i < HW; i += 256) { const float v = __ldg(px + i) - p; s += v; q = fmaf(v, v, q); }
     }
   }
   bn_block_sum2(s, q, red);
@@ -154,8 +164,8 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
       __threadfence();
       const double cnt = (double)N * HW;
       const double sum = *reinterpret_cast<volatile double*>(&acc[c].a), sq = *reinterpret_cast<volatile double*>(&acc[c].b);
-      const double mean = sum / cnt;
-      double var = sq / cnt - mean * mean;
+      const double dm = sum / cnt, mean = (double)p + dm;   // sums are of x - p
+      double var = sq / cnt - dm * dm;
       if (var < 0.0) var = 0.0;
       save_mean[c] = (float)mean;
       save_invstd[c] = rsqrtf((float)var + eps);
@@ -260,7 +270,8 @@ __global__ void __launch_bounds__(256) bn_bwd_stats_kernel(const float* __restri
 
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ gamma,
                                                             const float* __restrict__ save_mean, const float* __restrict__ save_invstd,
-                                                            const float* __restrict__ sums, float* __restrict__ dx, long long planes, int C, int HW, float inv_cnt) {
+                                                            const float* __restrict__ sums, float* __restrict__ dx, long long planes, int C, int HW, float inv_cnt,
+                                                            int fixed_stats) {
   gx::pdl_wait();
   gx::pdl_launch();
   if ((HW & 3) == 0) {
@@ -271,7 +282,9 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float* __restri
       const float mean = __ldg(save_mean + c), invstd = __ldg(save_invstd + c);
       const float k = (gamma ? __ldg(gamma + c) : 1.f) * invstd;
       const float m_dy = __ldg(sums + 2 * c) * inv_cnt, m_dyx = __ldg(sums + 2 * c + 1) * inv_cnt * invstd;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i), g = __ldg(reinterpret_cast<const float4*>(dy) + i);
+      const float4 g = __ldg(reinterpret_cast<const float4*>(dy) + i);
+      if (fixed_stats) { reinterpret_cast<float4*>(dx)[i] = make_float4(k * g.x, k * g.y, k * g.z, k * g.w); continue; }
+      const float4 v = __ldg(reinterpret_cast<const float4*>(x) + i);
       float4 o;
       o.x = k * (g.x - m_dy - (v.x - mean) * m_dyx); o.y = k * (g.y - m_dy - (v.y - mean) * m_dyx);
       o.z = k * (g.z - m_dy - (v.z - mean) * m_dyx); o.w = k * (g.w - m_dy - (v.w - mean) * m_dyx);
@@ -285,6 +298,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float* __restri
     const float k = (gamma ? gamma[c] : 1.f) * invstd;
     const float m_dy = sums[2 * c] * inv_cnt, m_dyx = sums[2 * c + 1] * inv_cnt * invstd;   // dx = k * (dy - mean(dy) - xhat * mean(dy*xhat))
     const float* px = x + pl * HW; const float* pg = dy + pl * HW; float* pd = dx + pl * HW;
+    if (fixed_stats) { for (int i = threadIdx.x; i < HW; i += 256) pd[i] = k * __ldg(pg + i); continue; }
     for (int i = threadIdx.x; i < HW; i += 256) pd[i] = k * (__ldg(pg + i) - m_dy - (__ldg(px + i) - mean) * m_dyx);
   }
 }
@@ -297,14 +311,26 @@ using namespace gx;
 // never share them (self-cleaning: the finalising CTA zeroes what it consumed)
 constexpr int BN_MAX_C = 16384;
 struct BnWorkspace { int dev = -1; cudaStream_t stream = nullptr; BnAcc* acc = nullptr; int* tickets = nullptr; float* sums = nullptr; };
-static BnWorkspace* bn_workspace(cudaStream_t s) {
-  static BnWorkspace ws[64];
-  static int used = 0;
-  static std::mutex mu;
+static BnWorkspace g_bn_ws[64];
+static int g_bn_ws_used = 0;
+static std::mutex g_bn_ws_mu;
+static BnWorkspace* bn_workspace_find(int dev, cudaStream_t s) {
+  for (int i = 0; i < g_bn_ws_used; ++i) if (g_bn_ws[i].dev == dev && g_bn_ws[i].stream == s) return &g_bn_ws[i];
+  return nullptr;
+}
+static BnWorkspace* bn_workspace_lookup(cudaStream_t s) {
   int dev = 0;
   cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lk(mu);
-  for (int i = 0; i < used; ++i) if (ws[i].dev == dev && ws[i].stream == s) return &ws[i];
+  std::lock_guard<std::mutex> lk(g_bn_ws_mu);
+  return bn_workspace_find(dev, s);
+}
+static BnWorkspace* bn_workspace(cudaStream_t s) {
+  BnWorkspace* ws = g_bn_ws;
+  int& used = g_bn_ws_used;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lk(g_bn_ws_mu);
+  if (BnWorkspace* w = bn_workspace_find(dev, s)) return w;
   // first use on this stream: allocation is not allowed while the stream is being captured into a graph (the caller then uses the
   // single-kernel form for this launch; warm-up steps normally run before a capture and allocate here)
   cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
@@ -318,6 +344,11 @@ static BnWorkspace* bn_workspace(cudaStream_t s) {
   cudaDeviceSynchronize();
   ws[used] = w;
   return &ws[used++];
+}
+// 1 when the split form's accumulators already exist for the calling device and stream `s` (introspection for tests: the first BatchNorm
+// on a stream that is being captured into a graph cannot allocate them and runs the one-CTA form)
+GX_API int gx_bn_workspace_ready(cudaStream_t s) {
+  return bn_workspace_lookup(s) != nullptr ? 1 : 0;
 }
 static bool bn_split_form(int N, int C, int HW) { return (long long)N * HW >= 4096 && HW >= 16 && C <= BN_MAX_C; }
 static int bn_slices(int N, int C) {
@@ -350,8 +381,10 @@ GX_API int gx_bn_fwd(const float* x, const float* gamma, const float* beta, floa
   launch_pdl(bn_fwd_kernel, dim3(C), dim3(512), 0, s, x, gamma, beta, rm, rv, y, save_mean, save_invstd, N, C, HW, training, momentum, eps);
   return GX_CHECK_LAUNCH();
 }
+// fixed_stats: save_mean / save_invstd are the running statistics the forward pass normalised with (inference mode, use_global_stats), which
+// do not depend on x, so dx = dy * gamma * invstd (reference batch_norm.cu, is_train_and_not_global_stats); dgamma / dbeta are the same sums.
 GX_API int gx_bn_bwd(const float* x, const float* dy, const float* gamma, const float* save_mean, const float* save_invstd, float* dx, float* dgamma,
-                     float* dbeta, int N, int C, int HW, cudaStream_t s) {
+                     float* dbeta, int N, int C, int HW, int fixed_stats, cudaStream_t s) {
   BnWorkspace* w = bn_split_form(N, C, HW) ? bn_workspace(s) : nullptr;
   if (w != nullptr) {
     int sms = 148, dev = 0;
@@ -362,9 +395,9 @@ GX_API int gx_bn_bwd(const float* x, const float* dy, const float* gamma, const 
     launch_pdl(bn_bwd_stats_kernel, dim3(C, bn_slices(N, C)), dim3(256), 0, s, x, dy, save_mean, save_invstd, dgamma, dbeta, w->sums, w->acc, w->tickets, N, C, HW);
     if (int rc = GX_CHECK_LAUNCH()) return rc;
     launch_pdl(bn_bwd_apply_kernel, dim3(grid), dim3(256), 0, s, x, dy, gamma, save_mean, save_invstd, (const float*)w->sums, dx, planes, C, HW,
-               1.f / ((float)N * (float)HW));
+               1.f / ((float)N * (float)HW), fixed_stats);
     return GX_CHECK_LAUNCH();
   }
-  launch_pdl(bn_bwd_kernel, dim3(C), dim3(512), 0, s, x, dy, gamma, save_mean, save_invstd, dx, dgamma, dbeta, N, C, HW);
+  launch_pdl(bn_bwd_kernel, dim3(C), dim3(512), 0, s, x, dy, gamma, save_mean, save_invstd, dx, dgamma, dbeta, N, C, HW, fixed_stats);
   return GX_CHECK_LAUNCH();
 }

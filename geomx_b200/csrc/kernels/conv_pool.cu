@@ -171,29 +171,34 @@ __global__ void __launch_bounds__(256) chansum_nchw_kernel(const float* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ ReLU
+// Each thread owns 4 consecutive elements: one 128-bit access per tensor when every pointer is 16-byte aligned (uniform over the grid),
+// scalar accesses otherwise (a contiguous view such as x[1:] or a slice handed over by cat / split backward starts anywhere).
+// fmaxf maps NaN to 0, like the reference's mshadow_op::relu (torch.relu would propagate it).
 __global__ void __launch_bounds__(256) relu_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, long long n) {
   gx::pdl_wait();
   gx::pdl_launch();
   const long long i4 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) * 4;
-  if (i4 + 3 < n) {
+  const bool vec = ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+  if (vec && i4 + 3 < n) {
     float4 v = *reinterpret_cast<const float4*>(x + i4);
     v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
     *reinterpret_cast<float4*>(y + i4) = v;
   } else {
-    for (long long i = i4; i < n; ++i) y[i] = fmaxf(x[i], 0.f);
+    for (long long i = i4; i < n && i < i4 + 4; ++i) y[i] = fmaxf(x[i], 0.f);
   }
 }
 __global__ void __launch_bounds__(256) relu_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, float* __restrict__ dx, long long n) {
   gx::pdl_wait();
   gx::pdl_launch();
   const long long i4 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) * 4;
-  if (i4 + 3 < n) {
+  const bool vec = ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
+  if (vec && i4 + 3 < n) {
     const float4 a = *reinterpret_cast<const float4*>(y + i4);
     float4 g = *reinterpret_cast<const float4*>(dy + i4);
     g.x = a.x > 0.f ? g.x : 0.f; g.y = a.y > 0.f ? g.y : 0.f; g.z = a.z > 0.f ? g.z : 0.f; g.w = a.w > 0.f ? g.w : 0.f;
     *reinterpret_cast<float4*>(dx + i4) = g;
   } else {
-    for (long long i = i4; i < n; ++i) dx[i] = y[i] > 0.f ? dy[i] : 0.f;
+    for (long long i = i4; i < n && i < i4 + 4; ++i) dx[i] = y[i] > 0.f ? dy[i] : 0.f;
   }
 }
 
@@ -534,10 +539,12 @@ GX_API int gx_chansum_nchw(const float* x, float* out, int N, int C, int HW, cud
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_relu_fwd(const float* x, float* y, long long n, cudaStream_t s) {
+  if (n <= 0) return 0;
   launch_pdl(relu_fwd_kernel, dim3((unsigned)((n + 1023) / 1024)), dim3(256), 0, s, x, y, n);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_relu_bwd(const float* y, const float* dy, float* dx, long long n, cudaStream_t s) {
+  if (n <= 0) return 0;
   launch_pdl(relu_bwd_kernel, dim3((unsigned)((n + 1023) / 1024)), dim3(256), 0, s, y, dy, dx, n);
   return GX_CHECK_LAUNCH();
 }

@@ -455,7 +455,8 @@ GX_API int gx_gemm_get_precision() { return gemm_precision(); }
 GX_API int gx_gemm_set_debug(unsigned long long* p) { g_gemm_dbg = p; return 0; }
 
 // A: K-major -> [M][K] with row stride lda; MN-major -> [K][M] with row stride lda.  Same for B with N.
-// returns 0 on success, -1 if the operands do not satisfy TMA alignment (caller falls back to gx_gemm_simt), -2 for a ReLU epilogue with
+// returns 0 on success, -1 if the operands do not satisfy TMA alignment or K <= 0 (caller falls back to gx_gemm_simt, which writes
+// D = epi(0) for an empty K, the same contract), -2 for a ReLU epilogue with
 // split_k > 1: every split applies the epilogue to its partial sum before the atomic add, which is right for the bias (split 0 only), the
 // mask and the column sum (linear), but would give sum(relu(partial)) instead of relu(sum).
 static int gemm_tf32_impl(const float* A, long long lda, int a_mn, const float* B, long long ldb, int b_mn, int M, int N, int K, float* D,
@@ -464,7 +465,8 @@ static int gemm_tf32_impl(const float* A, long long lda, int a_mn, const float* 
                           int pool_w, unsigned char* pool_idx, cudaStream_t stream) {
   using namespace gx;
   if (relu && split_k > 1) return -2;
-  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if (M <= 0 || N <= 0) return 0;
+  if (K <= 0) return -1;
   if (store_mode == 2) {   // fused pooling: whole windows must live inside one warp's 32 rows, no split-K / accumulate
     if (pool_w < 2 || (pool_w & 1) || (32 % (2 * pool_w)) != 0 || hw % 32 != 0 || (hw % pool_w) != 0 || ((hw / pool_w) & 1) || M % 32 != 0 ||
         split_k > 1 || accumulate || pool_idx == nullptr) return -1;

@@ -36,6 +36,12 @@ def _f32c(t):
     return t
 
 
+def _aligned(t, nbytes):
+    """``t`` itself when its data starts on an ``nbytes`` boundary, else an aligned copy (for kernels with vector accesses and no scalar
+    path; a contiguous view such as ``x[1:]`` can start anywhere)."""
+    return t if t.data_ptr() % nbytes == 0 else t.clone()
+
+
 # --------------------------------------------------------------------------------------------------------------- GEMM
 def set_gemm_precision(mode):
     """Process-wide multiply precision of the wgmma GEMM: ``"3xtf32"`` (default; fp32-accurate: hi/lo split of both operands, three MMAs per
@@ -264,6 +270,27 @@ def cnn_wgrad1(a1, a2, idx2, da2, dw1, db1):
 
 
 # --------------------------------------------------------------------------------------------------------------- depthwise convolution
+DW_SMEM_LIMIT = 200 * 1024       # ensure_smem in depthwise_conv.cu
+
+
+def depthwise_smem(H, W, KH, KW, stride, padding):
+    """Dynamic shared memory (bytes) of the forward, input-gradient and filter-gradient kernels, or None when the output is empty."""
+    OH, OW = conv_out_hw(H, W, KH, KW, stride[0], stride[1], padding[0], padding[1])
+    if OH < 1 or OW < 1:
+        return None
+    return dict(fwd=(H * W + KH * KW) * 4, dgrad=(OH * OW + KH * KW) * 4, wgrad=(H * W + OH * OW) * 4)
+
+
+def depthwise_supported(x_shape, w_shape, stride, padding):
+    """Whether a depthwise layer runs on the kernels: the input plane is at most ~95 KB (forward: plane + filter in shared memory) and the
+    input- and filter-gradient kernels, whose footprints grow with the OUTPUT plane (padding), fit as well, so that backward never refuses
+    a shape the forward accepted."""
+    H, W = x_shape[2], x_shape[3]
+    KH, KW = w_shape[2], w_shape[3]
+    sm = depthwise_smem(H, W, KH, KW, stride, padding)
+    return sm is not None and (H * W + KH * KW) * 8 <= 190 * 1024 and max(sm.values()) <= DW_SMEM_LIMIT
+
+
 def depthwise_fwd(x, w, bias, y, stride, padding, relu=False):
     N, C, H, W = x.shape
     rc = _lib().gx_depthwise_fwd(_p(x), _p(w), _p(bias), _p(y), N, C, H, W, w.shape[2], w.shape[3], stride[0], stride[1], padding[0], padding[1],
@@ -358,7 +385,7 @@ def maxpool2x2_fwd(x, out=None, idx=None):
         out = torch.empty(N, C, H // 2, W // 2, dtype=torch.float32, device=x.device)
     if idx is None:
         idx = torch.empty(N, C, H // 2, W // 2, dtype=torch.uint8, device=x.device)
-    _ck(_lib().gx_maxpool2x2_fwd(_p(_f32c(x)), _p(out), _p(idx), N * C, H, W, _s()), "maxpool_fwd")
+    _ck(_lib().gx_maxpool2x2_fwd(_p(_aligned(_f32c(x), 8)), _p(out), _p(idx), N * C, H, W, _s()), "maxpool_fwd")
     return out, idx
 
 
@@ -366,6 +393,7 @@ def maxpool2x2_bwd(dy, idx, x_shape, out=None):
     N, C, H, W = x_shape
     if out is None:
         out = torch.empty(x_shape, dtype=torch.float32, device=dy.device)
+    assert out.data_ptr() % 8 == 0, "maxpool2x2_bwd writes float2 pairs"
     _ck(_lib().gx_maxpool2x2_bwd(_p(_f32c(dy)), _p(idx), _p(out), N * C, H, W, _s()), "maxpool_bwd")
     return out
 
@@ -702,6 +730,7 @@ def scatter_rows(dst, ids, rows, add=False):
 def bn_fwd(x, gamma, beta, rm, rv, training, momentum, eps):
     N, C = x.shape[0], x.shape[1]
     HW = x.numel() // (N * C)
+    x = _aligned(_f32c(x), 16)            # the feature-map kernels stream x with 128-bit loads
     y = torch.empty_like(x)
     sm = torch.empty(C, dtype=torch.float32, device=x.device)
     si = torch.empty(C, dtype=torch.float32, device=x.device)
@@ -710,11 +739,21 @@ def bn_fwd(x, gamma, beta, rm, rv, training, momentum, eps):
     return y, sm, si
 
 
-def bn_bwd(x, dy, gamma, sm, si):
+def bn_workspace_ready(stream=None):
+    """Whether the split form's accumulators exist for ``stream`` (default: the current stream) on the current device."""
+    s = torch.cuda.current_stream() if stream is None else stream
+    return bool(_lib().gx_bn_workspace_ready(ctypes.c_void_p(s.cuda_stream)))
+
+
+def bn_bwd(x, dy, gamma, sm, si, fixed_stats=False):
+    """Input, scale and shift gradients of :func:`bn_fwd`.  ``sm`` / ``si``: the mean and inverse standard deviation the forward pass
+    normalised with.  ``fixed_stats``: they were the running statistics (inference mode, ``use_global_stats``), constants with respect to x,
+    so dx = dy * gamma * si; otherwise they were the batch's own and dx carries the terms of their dependence on x."""
     N, C = x.shape[0], x.shape[1]
     HW = x.numel() // (N * C)
+    x, dy = _aligned(_f32c(x), 16), _aligned(_f32c(dy), 16)
     dx = torch.empty_like(x)
     dg = torch.empty(C, dtype=torch.float32, device=x.device)
     dbt = torch.empty(C, dtype=torch.float32, device=x.device)
-    _ck(_lib().gx_bn_bwd(_p(x), _p(_f32c(dy)), _p(gamma), _p(sm), _p(si), _p(dx), _p(dg), _p(dbt), N, C, HW, _s()), "bn_bwd")
+    _ck(_lib().gx_bn_bwd(_p(x), _p(dy), _p(gamma), _p(sm), _p(si), _p(dx), _p(dg), _p(dbt), N, C, HW, int(bool(fixed_stats)), _s()), "bn_bwd")
     return dx, dg, dbt

@@ -69,7 +69,8 @@ SIGS = {
     "gx_bsc_seg_size": [],
     # batchnorm.cu
     "gx_bn_fwd": [P, P, P, P, P, P, P, P, I, I, I, I, F, F, P],
-    "gx_bn_bwd": [P, P, P, P, P, P, P, P, I, I, I, P],
+    "gx_bn_bwd": [P, P, P, P, P, P, P, P, I, I, I, I, P],
+    "gx_bn_workspace_ready": [P],
     # hips_fabric.cu
     "gx_fabric_params_size": [],
     "gx_hips_fsa_step": [P, I, P],

@@ -165,10 +165,11 @@ class BatchNormFn(torch.autograd.Function):
         if not training:
             sm = rm.clone(); si = torch.rsqrt(rv + eps)
         ctx.save_for_backward(x, gamma, sm, si)
+        ctx.fixed_stats = not training
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, gamma, sm, si = ctx.saved_tensors
-        dx, dg, db = native.bn_bwd(x, dy.contiguous(), gamma, sm, si)
+        dx, dg, db = native.bn_bwd(x, dy.contiguous(), gamma, sm, si, fixed_stats=ctx.fixed_stats)
         return dx, dg, db, None, None, None, None, None

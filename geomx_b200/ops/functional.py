@@ -71,7 +71,7 @@ def conv2d(x, w, b=None, stride=(1, 1), padding=(0, 0), dilation=(1, 1), groups=
         from .autograd_fns import Conv2dFn
         return Conv2dFn.apply(x, w, b, tuple(stride), tuple(padding), act == "relu")
     if (_nat(x) and x.dtype == torch.float32 and x.dim() == 4 and groups == x.shape[1] == w.shape[0] and w.shape[1] == 1 and tuple(dilation) == (1, 1)
-            and act in (None, "relu") and (x.shape[2] * x.shape[3] + w.shape[2] * w.shape[3]) * 8 <= 190 * 1024):
+            and act in (None, "relu") and native.depthwise_supported(x.shape, w.shape, stride, padding)):
         from .autograd_fns import DepthwiseConv2dFn            # depthwise: one CTA per (image, channel) plane, filter + plane in shared memory
         return DepthwiseConv2dFn.apply(x, w, b, tuple(stride), tuple(padding), act == "relu")
     return _act(F.conv2d(x, w, b, stride, padding, dilation, groups), act)
