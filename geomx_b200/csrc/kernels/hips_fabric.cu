@@ -54,6 +54,75 @@ __device__ __forceinline__ void global_apply_tile(const FabricParams& p, int t, 
   }
 }
 
+// Single rank: both server tiers collapse into the fused arena optimizer.  No peer ever spins on this launch, so the grid need not be
+// co-resident: one tile per CTA, grid-stride beyond the grid.  A channel passes its active tiles as `tile_list` and launches one CTA per
+// entry (CTA i serves tile_list[i]); otherwise CTA i serves tile i, skipping those `tile_active` excludes.  A kernel of its own, apart from
+// the multi-rank one, so that its register count is its own: its CTAs are meant to become resident beside the grid that produces the
+// gradients (the convolution backward wave, the dense weight gradients) and to have staged their tile when that grid ends.
+template <bool SCHED, bool EXT>
+__global__ void __launch_bounds__(FAB_THREADS, 4) hips_fsa_step_single_kernel(const FabricParams p) {
+  const volatile int* state = p.state;
+  const bool dbg = state[3] != 0 && blockIdx.x == 0 && threadIdx.x == 0;
+  unsigned long long* stamps = reinterpret_cast<unsigned long long*>(p.state + 8);
+  auto stamp = [&](int i) { if (dbg) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); stamps[i] = t; } };
+  const bool listed = p.tile_list != nullptr;
+  const int count = listed ? p.list_tiles : p.tiles;
+  auto tile_of = [&](int i) { return listed ? __ldg(p.tile_list + i) : i; };
+  auto prefetch_l2 = [](const float* q) { asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q), "r"(TILE * 4) : "memory"); };
+
+  // Before the grid dependency resolves, i.e. while the grid that writes the gradients still runs, this CTA stages its first tile:
+  //   - into registers: the tile index and its (lr_mult, wd_mult), which only the host writes (when the channel is declared and the arena
+  //     laid out), and the step size of the optimizer step that the state words announce;
+  //   - into L2 (bulk prefetch): the tile's master weights and optimizer state, and the state words.
+  // No kernel of a training step writes these except the previous launch on the same state block.  That launch may still be running here
+  // when it is the grid this one depends on (one channel launched twice back to back), so the weights, optimizer state and state words are
+  // loaded into registers only after the wait, from L2, and the early step size is kept only if the step word has not moved.  After the
+  // wait only L2 is read: those, and the gradient that the grid just waited for wrote.
+  const int i0 = blockIdx.x;
+  const int t0 = i0 < count ? tile_of(i0) : 0;
+  const float2 mult0 = (p.tile_mult != nullptr && i0 < count) ? __ldg(p.tile_mult + t0) : make_float2(1.f, 1.f);
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(p.state) : "memory");
+    if (i0 < count) {
+      const long long base = (long long)t0 * TILE;
+      prefetch_l2(p.w + base);
+      if (p.s0) prefetch_l2(p.s0 + base);
+      if (p.s1) prefetch_l2(p.s1 + base);
+    }
+  }
+  const int opt_early = state[2] + 1;
+  const float lr_early = step_lr<SCHED>(p.h, opt_early);
+  gx::pdl_wait();
+  gx::pdl_launch();
+  stamp(0);
+  const int round = state[0];
+  const int opt_t = state[2] + 1;
+  const float lr_t = opt_t == opt_early ? lr_early : step_lr<SCHED>(p.h, opt_t);
+  for (int i = i0; i < count; i += gridDim.x) {
+    const int t = i == i0 ? t0 : tile_of(i);
+    if (!listed && p.tile_active != nullptr && !p.tile_active[t]) continue;
+    const float2 mm = i == i0 ? mult0 : (p.tile_mult != nullptr ? __ldg(p.tile_mult + t) : make_float2(1.f, 1.f));
+    const long long off = (long long)t * TILE + threadIdx.x * 4;
+    float* g = p.grad[0] + off;
+    const float4 G = __ldcg(reinterpret_cast<const float4*>(g));
+    TileState s;
+    s.lr = lr_t * mm.x; s.wd = p.h.wd * mm.y;
+    s.W = *reinterpret_cast<const float4*>(p.w + off);
+    s.A = p.s0 ? *reinterpret_cast<const float4*>(p.s0 + off) : make_float4(0, 0, 0, 0);
+    s.B = p.s1 ? *reinterpret_cast<const float4*>(p.s1 + off) : make_float4(0, 0, 0, 0);
+    const float4 W = tile_state_apply<EXT>(p, off, s, f4_scale(G, p.push_scale));
+    if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
+    *reinterpret_cast<float4*>(p.param[0] + off) = W;
+  }
+  // bookkeeping: the state words are read by the next launch on this block after its own grid dependency, so a relaxed counter is enough
+  if (threadIdx.x == 0) {
+    const int done = atomicAdd(p.state + 1, 1);
+    if (done == (int)gridDim.x - 1) { p.state[1] = 0; p.state[2] = opt_t; p.state[0] = round + 1; }
+  }
+  stamp(5);
+}
+
+// Multi-rank flag ("bulk") protocol; a single rank runs hips_fsa_step_single_kernel (gx_hips_fsa_step picks it).
 template <bool SCHED, bool EXT>
 __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const FabricParams p) {
   gx::pdl_wait();
@@ -71,27 +140,6 @@ __global__ void __launch_bounds__(FAB_THREADS, 1) hips_fsa_step_kernel(const Fab
   const int S = p.party_size, P = p.num_parties;
   const int party_base = p.party * S;
   uint32_t* my_flags = p.flags[p.rank];
-
-  if (p.world == 1) {
-    // ---------------- single rank: both tiers collapse into the fused arena optimizer.  No peer ever spins on this launch, so the grid
-    // may exceed what is co-resident (one tile per CTA); all four operand loads are issued before the first use => ONE memory round trip.
-    for (int t = blockIdx.x; t < p.tiles; t += gridDim.x) {
-      if (p.tile_active != nullptr && !p.tile_active[t]) continue;
-      const long long off = (long long)t * TILE + threadIdx.x * 4;
-      float* g = p.grad[0] + off;
-      const float4 G = *reinterpret_cast<const float4*>(g);
-      TileState s = tile_state_load(p, t, off, lr_t);
-      const float4 W = tile_state_apply<EXT>(p, off, s, f4_scale(G, p.push_scale));
-      if (p.zero_grad) *reinterpret_cast<float4*>(g) = make_float4(0.f, 0.f, 0.f, 0.f);
-      *reinterpret_cast<float4*>(p.param[0] + off) = W;
-    }
-    if (threadIdx.x == 0) {
-      const int done = atomicAdd(p.state + 1, 1);
-      if (done == (int)gridDim.x - 1) { p.state[1] = 0; p.state[2] = opt_t; p.state[0] = (int)epoch; }
-    }
-    stamp(5);
-    return;
-  }
 
   // ---------------- phase A: publish gradient-ready to the party
   if (p.world > 1 && blockIdx.x == 0 && threadIdx.x < S) {
@@ -710,7 +758,8 @@ GX_API int gx_fabric_params_size() { return (int)sizeof(FabricParams); }
 GX_API int gx_hips_fsa_step(const void* params, int grid, cudaStream_t s) {
   FabricParams p = *reinterpret_cast<const FabricParams*>(params);
   if (grid < 1) grid = 1;
-  launch_pdl(GX_FAB_INSTANCE(hips_fsa_step_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  if (p.world == 1) launch_pdl(GX_FAB_INSTANCE(hips_fsa_step_single_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
+  else launch_pdl(GX_FAB_INSTANCE(hips_fsa_step_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
 // Largest co-resident grid of the fused kernels (they spin on each other: every CTA of a launch must be resident).

@@ -66,6 +66,8 @@ struct FabricParams {
   int direct_replicate;        // 1: EVERY rank reduces and applies every active tile on its own replica of the server state (one hop);
                                // 0: the tile's global owner does and pushes the result back (two hops)
   int channel_id;              // 0..7, folded into the packet epoch so that channels can never mistake each other's packets
+  int list_tiles;              // entries of tile_list
+  const int* tile_list;        // [list_tiles] the active tiles of a channel, ascending, or nullptr (single rank: CTA i serves tile_list[i])
 };
 // The instance of a fabric kernel (template <bool SCHED, bool EXT>) for a parameter block: the scheduled-lr instance when the block has a
 // schedule (step_lr<SCHED>), and the one with the later optimizer kinds compiled in only for those kinds (opt_apply4<EXT>).
@@ -73,7 +75,7 @@ struct FabricParams {
   ((p).h.sched.kind != SCHED_NONE ? ((p).h.kind > OPT_DCASGD ? kern<true, true> : kern<true, false>)                  \
                                   : ((p).h.kind > OPT_DCASGD ? kern<false, true> : kern<false, false>))
 // parallel/fabric.py's _FabricParams mirrors this block and asserts the same size (FABRIC_PARAMS_BYTES); kernel parameters are limited to 4 KB
-static_assert(sizeof(FabricParams) == 1656 && offsetof(FabricParams, h) == 728, "FabricParams layout (parallel/fabric.py)");
+static_assert(sizeof(FabricParams) == 1672 && offsetof(FabricParams, h) == 728, "FabricParams layout (parallel/fabric.py)");
 
 __device__ __forceinline__ void wait_flag_ge(const uint32_t* p, uint32_t v) {
   while (ld_acquire_sys(p) < v) { __nanosleep(20); }

@@ -228,12 +228,12 @@ class _FabricParams(ctypes.Structure):
         ("tile_order", ctypes.c_void_p), ("dgt_contrib", ctypes.c_void_p), ("dgt_alpha", ctypes.c_float),
         ("ll_party_mode", ctypes.c_int),
         ("ll_d", ctypes.c_void_p * MAX_RANKS), ("ll_d_mc", ctypes.c_void_p), ("ll_e", ctypes.c_void_p * MAX_RANKS), ("ll_e_mc", ctypes.c_void_p),
-        ("direct_replicate", ctypes.c_int), ("channel_id", ctypes.c_int),
+        ("direct_replicate", ctypes.c_int), ("channel_id", ctypes.c_int), ("list_tiles", ctypes.c_int), ("tile_list", ctypes.c_void_p),
     ]
 
 
 # the block is passed by value as a kernel parameter, and CUDA limits those to 4 KB.  hips_ll.cuh static_asserts the same size and offset.
-FABRIC_PARAMS_BYTES, FABRIC_PARAMS_H_OFFSET = 1656, 728
+FABRIC_PARAMS_BYTES, FABRIC_PARAMS_H_OFFSET = 1672, 728
 assert ctypes.sizeof(_FabricParams) == FABRIC_PARAMS_BYTES <= 4096 and _FabricParams.h.offset == FABRIC_PARAMS_H_OFFSET
 
 
@@ -518,6 +518,7 @@ class HipsFabric:
         self.state[name][2] = int(self.state["fsa"][2].item())        # optimizer step t continues
         self.channels[name] = {"id": len(self.channels) + 1, "mask": torch.from_numpy(mask).to(self.device), "replicate": bool(replicate),
                                "keys": list(key_indices), "tiles": active,
+                               "list": torch.from_numpy(np.flatnonzero(mask).astype(np.int32)).to(self.device),
                                "grid": int(grid) if grid else max(1, min(active, int(native.require().gx_hips_max_grid()) // 2))}
         self._params_cache.clear()
         return self.channels[name]
@@ -537,6 +538,7 @@ class HipsFabric:
         base = self._block("fsa", False, zero_grad)
         p = _FabricParams.from_buffer_copy(base)
         p.tile_active = ch["mask"].data_ptr()
+        p.tile_list, p.list_tiles = ch["list"].data_ptr(), ch["tiles"]
         p.state = self.state[name].data_ptr()
         p.direct_replicate = int(ch["replicate"])
         if ch["replicate"] and os.environ.get("GEOMX_REPL_MULTICAST", "1") != "1":
@@ -551,7 +553,7 @@ class HipsFabric:
         p = self._channel_block(name, zero_grad)
         lib = native.require()
         if self.topo.world == 1 and not self.loopback:
-            rc = lib.gx_hips_fsa_step(ctypes.byref(p), self.grid, self._stream())         # single rank: the fused arena optimizer on the masked tiles
+            rc = lib.gx_hips_fsa_step(ctypes.byref(p), ch["tiles"], self._stream())       # single rank: the fused arena optimizer, a CTA per tile
         elif self.ll_d is not None and self._channel_formats_direct_ok(ch):
             rc = lib.gx_hips_fsa_direct_step(ctypes.byref(p), ch["grid"], self._stream())
         elif self.protocol == "ll":
@@ -573,8 +575,6 @@ class HipsFabric:
             return None
         if not single and (self.ll_d is None or not self._channel_formats_direct_ok(ch)):
             return None
-        if "list" not in ch:
-            ch["list"] = torch.nonzero(ch["mask"]).flatten().to(torch.int32)
         return self._channel_block(name, zero_grad), ch["list"], ch["tiles"]
 
     @property
