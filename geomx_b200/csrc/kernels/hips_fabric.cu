@@ -762,6 +762,38 @@ GX_API int gx_hips_fsa_step(const void* params, int grid, cudaStream_t s) {
   else launch_pdl(GX_FAB_INSTANCE(hips_fsa_step_kernel, p), dim3(grid), dim3(FAB_THREADS), 0, s, p);
   return GX_CHECK_LAUNCH();
 }
+// During stream capture: the node just captured on `s` keeps a programmatic edge only from its first dependency (the launch before it on
+// its own stream); its edges from the streams it joined become full dependencies.  Measured on an H100: with a programmatic edge from the
+// dense-chain tail, the dense keys' channel resolved its grid dependency about 1 us after the convolution backward grid that follows the
+// tail on the main stream ended (21.5 us into the step), 2.4 us after its own predecessors had; with a full edge, 0.5 us after
+// dense_wgrad ended (19.7 us).  Returns the number of edges changed (0 outside a capture), -1 on an error.
+GX_API int gx_capture_demote_joined_edges(cudaStream_t s) {
+  cudaStreamCaptureStatus st;
+  cudaGraph_t g = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t n = 0;
+  if (cudaStreamGetCaptureInfo(s, &st, nullptr, &g, &deps, &n) != cudaSuccess || st != cudaStreamCaptureStatusActive || n != 1) {
+    cudaGetLastError();
+    return 0;
+  }
+  cudaGraphNode_t node = deps[0];
+  size_t m = 0;
+  if (cudaGraphNodeGetDependencies_v2(node, nullptr, nullptr, &m) != cudaSuccess || m < 2) return 0;
+  cudaGraphNode_t from[8];
+  cudaGraphEdgeData ed[8];
+  if (m > 8 || cudaGraphNodeGetDependencies_v2(node, from, ed, &m) != cudaSuccess) return -1;
+  int changed = 0;
+  for (size_t i = 1; i < m; ++i) {
+    if (ed[i].type != cudaGraphDependencyTypeProgrammatic) continue;
+    cudaGraphEdgeData full = {};
+    if (cudaGraphRemoveDependencies_v2(g, &from[i], &node, &ed[i], 1) != cudaSuccess ||
+        cudaGraphAddDependencies_v2(g, &from[i], &node, &full, 1) != cudaSuccess)
+      return -1;
+    ++changed;
+  }
+  return changed;
+}
+
 // Largest co-resident grid of the fused kernels (they spin on each other: every CTA of a launch must be resident).
 GX_API int gx_hips_max_grid() {
   int dev = 0, sms = 0, occ = 1 << 30;

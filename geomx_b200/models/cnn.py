@@ -13,7 +13,10 @@ into a CUDA graph and replayed per step.  At the reference's batch size (32 per 
   mlp_chain    da2 = dz3 · W0, one 16-CTA cluster (dense_tail_kernel, csrc/kernels/mlp_chain.cu).  With look-ahead the forward kernel stops
                at a3 and the cluster kernel runs the chain from a3 to da2.
   dense_wgrad  the three dense weight gradients and bias gradients, on a parallel branch: in the dense channel's step on the
-               high-priority stream when there is one, otherwise on the side stream, joined before the exchange   (csrc/kernels/mlp_chain.cu)
+               high-priority stream when there is one, otherwise on the side stream, joined before the exchange   (csrc/kernels/mlp_chain.cu).
+               When the forward kernel has computed dz3 it has stored everything this kernel reads, so its branch forks right after the
+               forward kernel, beside mlp_chain; the dense channel behind it also waits for mlp_chain, which reads the W0 it writes,
+               through a full graph edge (a programmatic one from mlp_chain made it wait for cnn_bwd_all too).
   cnn_bwd_all  conv1 data gradient + pool/ReLU routing + conv0 weight gradient ‖ conv1 weight gradient, one grid      (csrc/kernels/cnn_direct.cu)
   exchange     one LL kernel for all keys after the backward pass (several ranks), or key-group channels: the dense keys' exchange on
                a high-priority stream underneath cnn_bwd_all, the conv keys' one-hop exchange after it (one rank / GEOMX_STEP_OVERLAP=1)
@@ -544,7 +547,18 @@ class HipsCNNTrainStep:
         # programmatic edge separates the two)
         dense_kv = lambda: f.channel_step("dense", zero_grad=self.fused_zero_grad)
         if path.wgrad == "comm":
-            comm = [(DENSE_WGRAD + " + " + DENSE_KV, "comm", lambda: (wgrad(), dense_kv()))]
+            def wgrad_kv(tail=None):
+                # tail: the stream of the dense chain's data path, when the comm branch forked before it (see _body).  The exchange writes
+                # W0, which that path reads, so it waits for it; the weight gradients do not
+                wgrad()
+                if tail is not None:
+                    torch.cuda.current_stream().wait_stream(tail)
+                dense_kv()
+                if tail is not None:
+                    # in a captured graph the edge from the tail becomes a full one; only the edge from the weight gradients stays
+                    # programmatic (see gx_capture_demote_joined_edges)
+                    n.capture_demote_joined_edges()
+            comm = [(DENSE_WGRAD + " + " + DENSE_KV, "comm", wgrad_kv)]
         else:
             comm = [(DENSE_KV, "comm", dense_kv)] if path.overlap else []
 
@@ -605,20 +619,26 @@ class HipsCNNTrainStep:
         nf, join = self.path.n_fwd, self.path.lookahead_join
         rotated = steps[nf:] + [(name, join if where == "main" else where, fn) for name, where, fn in steps[:nf]]
         steps = {"all": steps, "fwd": steps[:nf], "rest": steps[nf:], "rotated": rotated}[part]
+        # from dz3, the forward launches store everything the dense weight gradients read (a2, a3, a4, dz4, dz3, dl) and the tail only
+        # turns dz3 into da2: the comm branch forks right after the forward launches, and its exchange joins the tail (see _steps)
+        early = part == "all" and self.path.wgrad == "comm" and self.path.dense == "dz3"
         for i, (name, where, fn) in enumerate(steps):
             if stop_after is not None and i >= stop_after:
                 break
+            if early and i == nf:
+                comm.wait_stream(main); comm_forked = True
             if where == "side":      # weight-gradient GEMMs leave the critical path: parallel branch of the captured graph
                 side.wait_stream(main)
                 with torch.cuda.stream(side):
                     fn()
                 forked = True
-            elif where == "comm":    # a key group's exchange: third branch, after everything issued so far on main and side
-                comm.wait_stream(main)
+            elif where == "comm":    # a key group's exchange: third branch, after everything issued so far on main and side (or `early`)
+                if not early:
+                    comm.wait_stream(main)
                 if forked:           # (a stream that has no work of this step yet must not be waited on: it is not part of a graph capture)
                     comm.wait_stream(side)
                 with torch.cuda.stream(comm):
-                    fn()
+                    fn(tail=main) if early else fn()
                 comm_forked = True
             else:
                 if where in ("join", "join_comm") and forked:

@@ -149,6 +149,16 @@ def dense_tail(a3, w0, w1, b1, w2, b2, label, loss, logits, dx, a4, dz4, dz3, dl
     return True
 
 
+def capture_demote_joined_edges():
+    """While the current stream is being captured into a CUDA graph: the launch just captured on it keeps its programmatic edge from the
+    launch before it on this stream, and waits for the streams it joined through full edges.  Returns the number of edges changed (0 when
+    the stream is not capturing)."""
+    rc = _lib().gx_capture_demote_joined_edges(_s())
+    if rc < 0:
+        raise RuntimeError("gx_capture_demote_joined_edges failed")
+    return rc
+
+
 def dense_wgrad(x, a3, a4, dz4, dz3, dl, dw0, db0, dw1, db1, dw2, db2):
     """The dense chain's weight and bias gradients (overwritten) from what :func:`mlp_chain_data` stored: dW0 = dz3ᵀ·x, dW1 = dz4ᵀ·a3,
     dW2 = dlᵀ·a4 and their column sums, one launch."""

@@ -77,6 +77,7 @@ SIGS = {
     "gx_hips_fsa_ll_step": [P, I, P],
     "gx_hips_fsa_direct_step": [P, I, P],
     "gx_hips_max_grid": [],
+    "gx_capture_demote_joined_edges": [P],
     "gx_hips_async_step": [P, P, P, P, I, I, I, P],
     "gx_hips_party_allreduce": [P, P, P, F, I, I, I, P],
     "gx_fabric_barrier": [P, I, I, I, P, P],
