@@ -7,20 +7,11 @@ import ctypes
 import pytest
 import torch
 
+from _cnn_ref import dev, nan, nat, rel_err, route  # noqa: F401  (nat: fixture)
+
 pytestmark = pytest.mark.gpu
 
 TAIL_SMS = 16        # the dense-chain cluster (dense_tail_kernel) that runs while the backward grid becomes resident: one CTA per SM
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
-def dev():
-    return torch.device("cuda", 0)
 
 
 def forward(nat, B, seed):
@@ -41,17 +32,8 @@ def forward(nat, B, seed):
 
 def wgrad1_ref(a1, a2, idx2, da2):
     """fp64 dW1 / db1 from the kernels' a1 and routing: the pooled gradient goes to the window's arg-max where a2 > 0."""
-    g = torch.where(a2 > 0, da2, torch.zeros_like(da2)).double()
-    B = g.shape[0]
-    dz = torch.zeros(B, 32, 8, 8, dtype=torch.float64, device=g.device)
-    for k in range(4):
-        dz[:, :, (k >> 1)::2, (k & 1)::2] = torch.where(idx2.long() == k, g, torch.zeros_like(g))
-    dw1 = torch.nn.grad.conv2d_weight(a1.double(), (32, 16, 5, 5), dz)
-    return dw1, dz.sum((0, 2, 3))
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
+    dz = route(torch.where(a2 > 0, da2, torch.zeros_like(da2)).double(), idx2)
+    return torch.nn.grad.conv2d_weight(a1.double(), (32, 16, 5, 5), dz), dz.sum((0, 2, 3))
 
 
 def test_grid_is_one_wave_beside_the_dense_chain(nat):
@@ -73,7 +55,6 @@ def test_split_wgrad1_matches_fp64(nat, B):
     x, w1, a1, idx1, a2, idx2, da2 = forward(nat, B, 100 + B)
     ref_w, ref_b = wgrad1_ref(a1, a2, idx2, da2)
     assert float(ref_w.abs().max()) > 0
-    nan = lambda *s: torch.full(s, float("nan"), device=dev())
     dw1, db1 = nan(32, 16, 5, 5), nan(32)
     assert nat.cnn_wgrad1(a1, a2, idx2, da2, dw1, db1)
     torch.cuda.synchronize()
@@ -92,7 +73,7 @@ def test_split_wgrad1_is_bitwise_repeatable(nat):
     outs = []
     for _ in range(3):
         dw0, db0 = torch.zeros(16, 1, 5, 5, device=dev()), torch.zeros(16, device=dev())
-        dw1, db1 = torch.full((32, 16, 5, 5), float("nan"), device=dev()), torch.full((32,), float("nan"), device=dev())
+        dw1, db1 = nan(32, 16, 5, 5), nan(32)
         nat.cnn_bwd_all(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1)
         torch.cuda.synchronize()
         outs.append((dw1, db1))

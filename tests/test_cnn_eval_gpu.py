@@ -4,30 +4,18 @@ slice never written, or a write past N, shows up.  Checked: the kernel against a
 batches (the last cluster's missing image) and the whole test-set size; launch-to-launch determinism; labels outside [0, 10); predict-only
 launches; the engine against fp64 and against the Gluon net re-homed onto it, in every update / graph / look-ahead mode and for every input
 kind; and that evaluation writes nothing the training step owns."""
-import gc
 import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import geomx_b200 as mx
+from _cnn_ref import conv_forward_ref, dense_chain_ref, engine, nat, rel_err  # noqa: F401  (nat, engine: fixtures)
 
 pytestmark = pytest.mark.gpu
 
 PAD = 64                    # sentinel elements after the N outputs of every buffer
 SENT = -7                   # int32 sentinel of pred / correct
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
 
 
 def _params(seed):
@@ -51,11 +39,9 @@ def _images(N, seed, zero_rows=()):
 
 def ref_forward(x, P):
     """fp64 forward of the demo CNN: (a2, a3, logits)."""
-    p = [t.double() for t in P]
-    h = F.max_pool2d(torch.relu(F.conv2d(x.double(), p[0], p[1])), 2)
-    a2 = F.max_pool2d(torch.relu(F.conv2d(h, p[2], p[3])), 2).reshape(x.shape[0], 512)
-    a3 = torch.relu(F.linear(a2, p[4], p[5]))
-    return a2, a3, F.linear(torch.relu(F.linear(a3, p[6], p[7])), p[8], p[9])
+    _, a2, _ = conv_forward_ref(x.double(), *[p.double() for p in P[:4]])
+    d = dense_chain_ref(P[4:], a2=a2)
+    return a2.flatten(1), d["a3"], d["logits"]
 
 
 def _outputs(N):
@@ -155,10 +141,8 @@ def test_cnn_eval_refuses_an_empty_batch(nat):
 
 
 # ---------------------------------------------------------------------------------------------------------------- engine
-def _engine(net=None, update="server", use_graph=True, lookahead=False):
-    from geomx_b200.parallel import Topology
-    return mx.models.HipsCNNTrainStep(net=net, batch_size=32, optimizer=mx.optimizer.Adam(learning_rate=0.01), topo=Topology(1, 0, 1, 1),
-                                      use_graph=use_graph, update=update, lookahead=lookahead)
+def _engine(engine, net=None, update="server", use_graph=True, lookahead=False):
+    return engine(32, mx.optimizer.Adam(learning_rate=0.01), net=net, use_graph=use_graph, update=update, lookahead=lookahead)
 
 
 def _train_batches(n, seed):
@@ -171,11 +155,6 @@ def _as_input(t, kind):
             "ndarray": lambda: mx.nd.array(t, ctx=mx.gpu(0))}[kind]()
 
 
-def _release():
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
 @pytest.mark.parametrize("update,use_graph,lookahead,x_kind,y_kind", [
     ("server", True, False, "pinned", "float"),
     ("server", False, False, "host", "int"),
@@ -184,48 +163,44 @@ def _release():
     ("local", True, False, "cuda", "float"),
     ("local", False, False, "ndarray", "int"),
 ])
-def test_engine_evaluate_and_predict_score_the_live_weights(nat, update, use_graph, lookahead, x_kind, y_kind):
+def test_engine_evaluate_and_predict_score_the_live_weights(nat, engine, update, use_graph, lookahead, x_kind, y_kind):
     torch.manual_seed(31)
     net = mx.models.build_cnn()
     net.initialize(init=mx.init.Xavier(), ctx=mx.gpu(0))
     net(mx.nd.array(torch.zeros(1, 1, 28, 28), ctx=mx.gpu(0)))          # deferred shapes -> parameters
-    eng = _engine(net, update, use_graph, lookahead)
-    try:
-        batches = _train_batches(20, 32)
-        for X, y in batches[:-1]:
-            eng.step(X, y)
-        N = 333
-        g = torch.Generator().manual_seed(33)
-        Xe, ye = torch.rand(N, 1, 28, 28, generator=g), torch.randint(0, 10, (N,), generator=g)
-        Xin = _as_input(Xe.reshape(N, 784) if x_kind == "host" else Xe, x_kind)     # both image layouts
-        yin = _as_input(ye.float() if y_kind == "float" else ye, x_kind)
-        # the last step and the evaluation are enqueued back to back: the evaluation must see that step's update (with look-ahead, the last
-        # completed one: the launch also ran the convolutions of the next batch, which change no weight)
-        eng.step_async(*batches[-1])
-        handle = eng.evaluate_async(Xin, yin)
-        logits = eng.predict(Xin)
-        mean_loss, acc = handle.item()
-        torch.cuda.synchronize()
-        P = [torch.from_numpy(p).cuda() for p in eng.params_numpy()]
-        _, _, ref = ref_forward(Xe.cuda(), P)
-        assert logits.shape == (N, 10) and logits.is_cuda
-        assert rel_err(logits, ref) <= 1e-5, rel_err(logits, ref)
-        ref_loss = -torch.log_softmax(ref, 1).gather(1, ye.cuda().view(-1, 1)).view(-1)
-        assert abs(mean_loss - float(ref_loss.mean())) <= 1e-4, (mean_loss, float(ref_loss.mean()))
-        top2 = ref.topk(2, dim=1).values
-        unclear = int(((top2[:, 0] - top2[:, 1]) <= 1e-3).sum())
-        ref_hits = int((ref.argmax(1).cpu() == ye).sum())
-        hits = round(acc * N)
-        assert abs(acc * N - hits) < 1e-6 and abs(hits - ref_hits) <= unclear, (acc, ref_hits, unclear)
-        # the Gluon net re-homed onto the engine reads the same live weights through the generic layer-by-layer path
-        gl = torch.from_numpy(net(mx.nd.array(Xe, ctx=mx.gpu(0))).asnumpy()).cuda()
-        assert rel_err(logits, gl) <= 1e-4, rel_err(logits, gl)
-        # same inputs, same bits
-        assert eng.evaluate(Xin, yin) == (mean_loss, acc)
-        assert torch.equal(eng.predict(Xin), logits)
-    finally:
-        del eng
-        _release()
+    eng = _engine(engine, net, update, use_graph, lookahead)
+    batches = _train_batches(20, 32)
+    for X, y in batches[:-1]:
+        eng.step(X, y)
+    N = 333
+    g = torch.Generator().manual_seed(33)
+    Xe, ye = torch.rand(N, 1, 28, 28, generator=g), torch.randint(0, 10, (N,), generator=g)
+    Xin = _as_input(Xe.reshape(N, 784) if x_kind == "host" else Xe, x_kind)     # both image layouts
+    yin = _as_input(ye.float() if y_kind == "float" else ye, x_kind)
+    # the last step and the evaluation are enqueued back to back: the evaluation must see that step's update (with look-ahead, the last
+    # completed one: the launch also ran the convolutions of the next batch, which change no weight)
+    eng.step_async(*batches[-1])
+    handle = eng.evaluate_async(Xin, yin)
+    logits = eng.predict(Xin)
+    mean_loss, acc = handle.item()
+    torch.cuda.synchronize()
+    P = [torch.from_numpy(p).cuda() for p in eng.params_numpy()]
+    _, _, ref = ref_forward(Xe.cuda(), P)
+    assert logits.shape == (N, 10) and logits.is_cuda
+    assert rel_err(logits, ref) <= 1e-5, rel_err(logits, ref)
+    ref_loss = -torch.log_softmax(ref, 1).gather(1, ye.cuda().view(-1, 1)).view(-1)
+    assert abs(mean_loss - float(ref_loss.mean())) <= 1e-4, (mean_loss, float(ref_loss.mean()))
+    top2 = ref.topk(2, dim=1).values
+    unclear = int(((top2[:, 0] - top2[:, 1]) <= 1e-3).sum())
+    ref_hits = int((ref.argmax(1).cpu() == ye).sum())
+    hits = round(acc * N)
+    assert abs(acc * N - hits) < 1e-6 and abs(hits - ref_hits) <= unclear, (acc, ref_hits, unclear)
+    # the Gluon net re-homed onto the engine reads the same live weights through the generic layer-by-layer path
+    gl = torch.from_numpy(net(mx.nd.array(Xe, ctx=mx.gpu(0))).asnumpy()).cuda()
+    assert rel_err(logits, gl) <= 1e-4, rel_err(logits, gl)
+    # same inputs, same bits
+    assert eng.evaluate(Xin, yin) == (mean_loss, acc)
+    assert torch.equal(eng.predict(Xin), logits)
 
 
 def _engine_tensors(eng):
@@ -249,42 +224,34 @@ def _bits(t):
 
 
 @pytest.mark.parametrize("update,lookahead", [("server", True), ("server", False), ("local", False)])
-def test_evaluation_leaves_training_alone(nat, update, lookahead):
+def test_evaluation_leaves_training_alone(nat, engine, update, lookahead):
     torch.manual_seed(41)
-    eng = _engine(None, update, True, lookahead)
-    try:
-        for X, y in _train_batches(5, 42):
-            eng.step(X, y)
-        torch.cuda.synchronize()
-        kps = eng.kernels_per_step
-        before = {k: _bits(v) for k, v in _engine_tensors(eng).items()}
-        g = torch.Generator().manual_seed(43)
-        Xe, ye = torch.rand(1001, 1, 28, 28, generator=g).cuda(), torch.randint(0, 10, (1001,), generator=g).float().cuda()
-        launches = nat.launch_count
-        for i in range(3):
-            eng.evaluate(Xe[:1001 - i], ye[:1001 - i])
-            assert nat.launch_count == launches + i + 1, "one native launch per evaluate"
-        eng.predict(Xe)
-        assert nat.launch_count == launches + 4
-        torch.cuda.synchronize()
-        for k, v in _engine_tensors(eng).items():
-            assert torch.equal(_bits(v), before[k]), (k, "written by evaluation")
-        assert eng.kernels_per_step == kps
-    finally:
-        del eng
-        _release()
+    eng = _engine(engine, None, update, True, lookahead)
+    for X, y in _train_batches(5, 42):
+        eng.step(X, y)
+    torch.cuda.synchronize()
+    kps = eng.kernels_per_step
+    before = {k: _bits(v) for k, v in _engine_tensors(eng).items()}
+    g = torch.Generator().manual_seed(43)
+    Xe, ye = torch.rand(1001, 1, 28, 28, generator=g).cuda(), torch.randint(0, 10, (1001,), generator=g).float().cuda()
+    launches = nat.launch_count
+    for i in range(3):
+        eng.evaluate(Xe[:1001 - i], ye[:1001 - i])
+        assert nat.launch_count == launches + i + 1, "one native launch per evaluate"
+    eng.predict(Xe)
+    assert nat.launch_count == launches + 4
+    torch.cuda.synchronize()
+    for k, v in _engine_tensors(eng).items():
+        assert torch.equal(_bits(v), before[k]), (k, "written by evaluation")
+    assert eng.kernels_per_step == kps
 
 
-def test_engine_evaluate_rejects_mismatched_inputs(nat):
-    eng = _engine(None, "server", False, False)
-    try:
-        with pytest.raises(ValueError):
-            eng.evaluate(torch.rand(4, 1, 28, 27), torch.zeros(4))
-        with pytest.raises(ValueError):
-            eng.evaluate(torch.rand(4, 784), torch.zeros(5))
-        with pytest.raises(ValueError):
-            eng.predict(torch.rand(0, 784))
-        assert math.isfinite(eng.evaluate(torch.rand(3, 784), torch.zeros(3))[0])
-    finally:
-        del eng
-        _release()
+def test_engine_evaluate_rejects_mismatched_inputs(nat, engine):
+    eng = _engine(engine, None, "server", False, False)
+    with pytest.raises(ValueError):
+        eng.evaluate(torch.rand(4, 1, 28, 27), torch.zeros(4))
+    with pytest.raises(ValueError):
+        eng.evaluate(torch.rand(4, 784), torch.zeros(5))
+    with pytest.raises(ValueError):
+        eng.predict(torch.rand(0, 784))
+    assert math.isfinite(eng.evaluate(torch.rand(3, 784), torch.zeros(3))[0])

@@ -3,25 +3,12 @@ batch rows: 1, 1, 2 and 8 clusters at the batch sizes below.  Against fp64 with 
 import pytest
 import torch
 
+from _cnn_ref import D0, D1, D2, dense_chain_ref, nan, nat, rel_err  # noqa: F401  (nat: fixture)
+
 pytestmark = pytest.mark.gpu
 
-D0, D1, D2, C = 512, 256, 128, 10
+C = 10
 BATCHES = [1, 2, 8, 32]
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
-
-
-def nan(*s):
-    return torch.full(s, float("nan"), device="cuda")
 
 
 def da2_from_dz3(nat, dz3, w0):
@@ -41,6 +28,6 @@ def test_da2_matches_fp64_and_repeats_bitwise(nat, B):
     w0 = (torch.randn(D1, D0, generator=g) * 0.05).cuda()
     outs = [da2_from_dz3(nat, dz3, w0) for _ in range(3)]
     assert not torch.isnan(outs[0]).any(), B
-    assert rel_err(outs[0], dz3.double() @ w0.double()) < 1e-6, B
+    assert rel_err(outs[0], dense_chain_ref([w0] + [None] * 5, dz3=dz3)["dx"]) < 1e-6, B
     for dx in outs[1:]:
         assert torch.equal(dx, outs[0]), (B, "da2 differs between launches")

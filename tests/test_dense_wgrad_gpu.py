@@ -2,28 +2,13 @@
 the step after the cluster kernel that computes the data path.  These tests check the kernel alone against fp64 with every output pre-filled
 with NaN, and that in a graph-captured step the dense keys' exchange applies the gradients this kernel writes: it runs on another stream
 than the cluster kernel, so an exchange ordered only behind the cluster kernel would read gradients that do not exist yet."""
-import gc
-
 import pytest
 import torch
 
 import geomx_b200 as mx
-from geomx_b200.models.cnn import STEP_SWITCHES
+from _cnn_ref import D0, D1, D2, engine, nan, nat, rel_err  # noqa: F401  (nat, engine: fixtures)
 
 pytestmark = pytest.mark.gpu
-
-D0, D1, D2 = 512, 256, 128
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
 
 
 @pytest.mark.parametrize("B", [1, 7, 31, 32])
@@ -35,7 +20,6 @@ def test_dense_wgrad_matches_fp64(nat, B):
     dz3, dz4 = r(B, D1) * (a3 > 0), r(B, D2) * (a4 > 0)
     dl = torch.zeros(B, 16, device="cuda")
     dl[:, :C] = r(B, C)
-    nan = lambda *s: torch.full(s, float("nan"), device="cuda")
     outs = [nan(D1, D0), nan(D1), nan(D2, D1), nan(D2), nan(C, D2), nan(C)]
     nat.dense_wgrad(x, a3, a4, dz4, dz3, dl, *outs)
     torch.cuda.synchronize()
@@ -47,40 +31,31 @@ def test_dense_wgrad_matches_fp64(nat, B):
 
 
 @pytest.mark.parametrize("B", [32, 20])
-def test_graph_step_applies_the_dense_weight_gradients(nat, monkeypatch, B):
+def test_graph_step_applies_the_dense_weight_gradients(nat, engine, B):
     """One rank, SGD at lr = 1 without momentum or weight decay: the dense parameters after one replay of the captured step must be exactly
     those an eager step gives from the same parameters and batch, and must have moved by the gradients that eager step left in the arena."""
-    from geomx_b200.parallel import Topology
-    for k in STEP_SWITCHES:
-        monkeypatch.delenv(k, raising=False)
     g = torch.Generator().manual_seed(400 + B)
     X, y = torch.rand(B, 1, 28, 28, generator=g).cuda(), torch.randint(0, 10, (B,), generator=g).float().cuda()
-    eng = mx.models.HipsCNNTrainStep(batch_size=B, optimizer=mx.optimizer.SGD(learning_rate=1.0, momentum=0.0, wd=0.0),
-                                     topo=Topology(1, 0, 1, 1), use_graph=True, fused_zero_grad=False)
-    try:
-        names = [n for n, _, _ in eng._steps()]
-        assert eng.fused_mlp and eng.overlap and any(n.startswith("dense weight gradients") for n in names), names
-        P0 = [p.clone() for p in eng.P]
+    eng = engine(B, mx.optimizer.SGD(learning_rate=1.0, momentum=0.0, wd=0.0), use_graph=True, fused_zero_grad=False)
+    names = [n for n, _, _ in eng._steps()]
+    assert eng.fused_mlp and eng.overlap and any(n.startswith("dense weight gradients") for n in names), names
+    P0 = [p.clone() for p in eng.P]
 
-        def start():
-            for p, v in zip(eng.P, P0):
-                p.copy_(v)
-            eng.fabric.load_master_from_param()
-            eng.x.copy_(X); eng.label.copy_(y)
-            torch.cuda.synchronize()
+    def start():
+        for p, v in zip(eng.P, P0):
+            p.copy_(v)
+        eng.fabric.load_master_from_param()
+        eng.x.copy_(X); eng.label.copy_(y)
+        torch.cuda.synchronize()
 
-        start()
-        eng._body(); torch.cuda.synchronize()
-        grads = [t.clone() for t in eng.G]
-        eager = [p.clone() for p in eng.P]
-        eng.capture()
-        start()
-        eng.graph.replay(); torch.cuda.synchronize()
-        for i in range(4, 10):
-            assert torch.equal(eng.P[i], eager[i]), "dense parameter %d differs between the captured and the eager step" % i
-            moved = P0[i] - eng.P[i]
-            assert rel_err(moved, grads[i] / B) < 1e-4, (i, rel_err(moved, grads[i] / B))   # (rounding of P0 - update)
-    finally:
-        del eng
-        gc.collect()
-        torch.cuda.empty_cache()
+    start()
+    eng._body(); torch.cuda.synchronize()
+    grads = [t.clone() for t in eng.G]
+    eager = [p.clone() for p in eng.P]
+    eng.capture()
+    start()
+    eng.graph.replay(); torch.cuda.synchronize()
+    for i in range(4, 10):
+        assert torch.equal(eng.P[i], eager[i]), "dense parameter %d differs between the captured and the eager step" % i
+        moved = P0[i] - eng.P[i]
+        assert rel_err(moved, grads[i] / B) < 1e-4, (i, rel_err(moved, grads[i] / B))   # (rounding of P0 - update)

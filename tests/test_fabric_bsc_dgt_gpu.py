@@ -13,67 +13,38 @@ Everything here runs the multi-rank LL packet kernel in loop-back (``HipsFabric(
 
 Measured errors are printed (``-s``).
 """
-import gc
-
 import numpy as np
 import pytest
 import torch
 
 import geomx_b200 as mx
-from geomx_b200.models.cnn import STEP_SWITCHES
 
 import _update_ref as R
-from test_update_paths_gpu import A_LOCAL, _batches, _clip_for, _opt, half_ulps
+from _cnn_ref import cleanup, dev, nat  # noqa: F401  (nat: fixture)
+from _update_harness import A_LOCAL, FAB_SPECS, KEY_MULTS, KEY_SIZES, PUSH_SCALE, SWITCHES, TOL, _batches, _clip_for, _opt, half_ulps
 
 pytestmark = pytest.mark.gpu
 
-SWITCHES = STEP_SWITCHES + ("GEOMX_FABRIC_PROTOCOL", "GEOMX_FABRIC_DIRECT", "GEOMX_PY_UPDATER", "GEOMX_WIRE_FP8", "ENABLE_DGT", "ENABLE_P3",
-                            "MXNET_KVSTORE_USE_HFA", "ADAPTIVE_K_FLAG", "DMLC_K", "DMLC_K_MIN", "DGT_CONTRIBUTION_ALPHA")
-
-TOL = R.DISP_TOL
+# the update paths' switches and the Bi-Sparse / DGT ones
+BSC_SWITCHES = SWITCHES + ("ADAPTIVE_K_FLAG", "DMLC_K", "DMLC_K_MIN", "DGT_CONTRIBUTION_ALPHA")
 # Relative slack of a kernel's Bi-Sparse selection against the reference's |v| at the K-th magnitude (see R.selection_slack): fp32 u / v
 # carry a few ulps of rounding per round (relative ~1e-7 after five rounds), so a real near-tie may fall either way; 1e-5 is far below
 # what a wrong rule (ties to the high index, a stale residual) produces on these tiles.
 SEL_SLACK = 1e-5
 
 
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
 @pytest.fixture
 def clean_env(monkeypatch):
-    for k in SWITCHES:
+    for k in BSC_SWITCHES:
         monkeypatch.delenv(k, raising=False)
     return monkeypatch
-
-
-def dev():
-    return torch.device("cuda", 0)
-
-
-def cleanup():
-    gc.collect()
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
 
 
 def bits(t):
     return t.detach().float().cpu().contiguous().view(torch.int32)
 
 
-KEY_SIZES = [1, 1000, 1024, 1025, 5000, 70000]
-KEY_MULTS = [(0.5, 2.0), (2.0, 0.0), (1.0, 1.5), (0.25, 1.0), (1.5, 0.5), (0.75, 3.0)]
 MIX_FMTS = ["fp32", "bsc", "fp16", "bsc", "fp8", "bsc"]
-PUSH_SCALE = 1.0 / 32
-SPECS = {
-    "sgd": dict(name="sgd", lr=0.1, wd=0.02, rescale_grad=2.0, clip_gradient=0.02, momentum=0.9),
-    "adam": dict(name="adam", lr=0.01, wd=0.02, rescale_grad=2.0, clip_gradient=0.02, beta1=0.9, beta2=0.999, epsilon=1e-8),
-    "dcasgd": dict(name="dcasgd", lr=0.1, wd=0.02, rescale_grad=2.0, clip_gradient=0.02, momentum=0.9, lamda=40.0),
-}
 
 
 def _fabric(sizes, fmts, spec, thr=0.01, mults=None, push_scale=PUSH_SCALE):
@@ -218,7 +189,7 @@ def test_bsc_mixed_rounds(nat, clean_env, kind):
     and the pulled aggregate (sparse for Bi-Sparse keys, halves for fp16 / fp8).  SGD / Adam / DCASGD: master weights and both state slots
     (displacement tolerance), dense pulls (fp32 and Bi-Sparse keys exact copies of the master weights, fp16 / fp8 keys fp16 of it).  Every
     round: ``bsc_u`` / ``bsc_v``, the step count, a valid selection."""
-    spec = SPECS.get(kind)
+    spec = FAB_SPECS.get(kind)
     f = _fabric(KEY_SIZES, MIX_FMTS, spec, mults=KEY_MULTS)
     try:
         gen = torch.Generator().manual_seed(5 + len(kind or ""))
@@ -268,7 +239,7 @@ def test_bsc_mixed_rounds(nat, clean_env, kind):
 def test_bsc_masked_rounds(nat, clean_env):
     """Masked rounds (``tile_active``) with Adam: the keys of the round follow the reference, every other key keeps w, s0, s1, the parameters
     and its Bi-Sparse u / v bit-identical.  The active sets only shrink (the fabric's Adam step count is per channel)."""
-    spec = SPECS["adam"]
+    spec = FAB_SPECS["adam"]
     f = _fabric(KEY_SIZES, MIX_FMTS, spec, mults=KEY_MULTS)
     try:
         gen = torch.Generator().manual_seed(77)
@@ -338,7 +309,7 @@ def test_bsc_channel_falls_back_to_ll(nat, clean_env, replicate):
     """A channel with Bi-Sparse tiles cannot take the direct protocol: it runs the LL kernel on its tiles, and its rounds equal
     ``fsa_step`` on a twin fabric bit for bit (weights, state, parameters, u / v); a replicated such channel cannot run in a compute kernel's
     tail (``channel_fused_args`` is None)."""
-    spec = SPECS["adam"]
+    spec = FAB_SPECS["adam"]
     fa = _fabric(KEY_SIZES, MIX_FMTS, spec, mults=KEY_MULTS)
     fb = _fabric(KEY_SIZES, MIX_FMTS, spec, mults=KEY_MULTS)
     try:
@@ -404,7 +375,7 @@ def test_dgt_rerank_and_rounds(nat, clean_env, adaptive):
         clean_env.setenv("DMLC_K_MIN", "0.05")
     # fixed: 5 % of the 79 tiles important; adaptive: the prefix with 60 % of the contribution, at least 5 % of the tiles.  The one-float
     # fp32 key and (at fixed K) the fp16 key rank below the dense fp8 key, so something is demoted
-    spec = SPECS["adam"]
+    spec = FAB_SPECS["adam"]
     k = 0.6 if adaptive else 0.05
     fa, fb = _dgt_fabric(spec, k), _dgt_fabric(spec, k)
     try:

@@ -17,7 +17,8 @@ import torch
 from geomx_b200 import lr_scheduler as S
 
 import _update_ref as R
-from test_update_paths_gpu import FAB_SPECS, KEY_MULTS, KEY_SIZES, PUSH_SCALE, _fab_grads, _fab_init, _fabric, cleanup, clean_env, dev, nat  # noqa: F401
+from _cnn_ref import cleanup, dev, nat  # noqa: F401  (nat: fixture)
+from _update_harness import FAB_SPECS, KEY_MULTS, KEY_SIZES, PUSH_SCALE, _fab_grads, _fab_init, _fabric, clean_env  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

@@ -3,37 +3,16 @@
 (csrc/kernels/mlp_chain.cu: da2 = dz3 W0 only).  These tests check the head against fp64, including confidently classified samples, the
 from-dz3 tail against fp64, the new pair against the pair that goes through a3, launch-to-launch determinism, and which pair the captured
 step runs with and without look-ahead.  Every output is pre-filled with NaN, so that an element never written shows up."""
-import gc
-
 import pytest
 import torch
-import torch.nn.functional as F
 
 import geomx_b200 as mx
-from geomx_b200.models.cnn import STEP_SWITCHES
+from _cnn_ref import D0, D1, D2, dense_chain_ref, engine, nan, nat, rel_err  # noqa: F401  (nat, engine: fixtures)
 
 pytestmark = pytest.mark.gpu
 
-D0, D1, D2, C = 512, 256, 128, 10
-SWITCHES = STEP_SWITCHES + ("GEOMX_MLP_CLUSTER",)
+C = 10
 HEAD_OUT = ("loss", "logits", "a4", "dz4", "dz3", "dl")
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    return native
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
-
-
-def nan(*s, dtype=torch.float32):
-    if dtype == torch.uint8:
-        return torch.full(s, 255, dtype=dtype, device="cuda")
-    return torch.full(s, float("nan"), dtype=dtype, device="cuda")
 
 
 def _inputs(B, seed, w2_scale=0.1):
@@ -65,20 +44,6 @@ def _run_head(nat, x, P, y):
     return out
 
 
-def _reference(a2, P, y):
-    """fp64 dense chain from a2 (a2 itself from the kernel, which the convolution tests check bit for bit against cnn_fwd)"""
-    w0, b0, w1, b1, w2, b2 = [t.double() for t in P[4:]]
-    B = a2.shape[0]
-    a3 = torch.relu(F.linear(a2.double().view(B, D0), w0, b0)).requires_grad_(True)
-    z4 = F.linear(a3, w1, b1); z4.retain_grad()
-    a4 = torch.relu(z4)
-    lg = F.linear(a4, w2, b2); lg.retain_grad()
-    loss = F.cross_entropy(lg, y.long(), reduction="none")
-    loss.sum().backward()
-    return {"a3": a3.detach(), "a4": a4.detach(), "loss": loss.detach(), "logits": lg.detach(), "dl": lg.grad, "dz4": z4.grad,
-            "dz3": a3.grad * (a3.detach() > 0)}
-
-
 @pytest.mark.parametrize("B", [2, 8, 32])
 @pytest.mark.parametrize("w2_scale", [0.1, 3.0], ids=["spread", "confident"])
 def test_fwd_head_matches_fp64(nat, B, w2_scale):
@@ -86,12 +51,13 @@ def test_fwd_head_matches_fp64(nat, B, w2_scale):
     got = _run_head(nat, x, P, y)
     assert torch.equal(got["dl"][:, C:], torch.zeros_like(got["dl"][:, C:])), (B, "dlogits beyond the classes")
     got["dl"] = got["dl"][:, :C]
-    ref = _reference(got["a2"], P, y)
+    # the dense chain from a2 (a2 itself from the kernel, which the convolution tests check bit for bit against cnn_fwd)
+    ref = dense_chain_ref(P[4:], y, a2=got["a2"])
     if w2_scale > 1:
         p_max = torch.softmax(ref["logits"], 1).max(1).values
         assert (p_max > 0.999).float().mean() > 0.5, "most samples must be classified confidently"
-    for name, want in ref.items():
-        g = got[name]
+    for name in ("a3", "a4", "loss", "logits", "dl", "dz4", "dz3"):
+        g, want = got[name], ref[name]
         assert not torch.isnan(g).any(), (B, name, "element never written")
         err = rel_err(g, want)
         assert err < (1e-6 if name == "a3" else 1e-5), (B, w2_scale, name, err)
@@ -120,7 +86,7 @@ def test_dense_tail_from_dz3_matches_fp64(nat, B):
     w0 = (torch.randn(D1, D0, generator=g) * 0.05).cuda()
     out = _run_tail(nat, dz3, w0, True)
     assert not torch.isnan(out["dx"]).any(), (B, "dx element never written")
-    assert rel_err(out["dx"], dz3.double() @ w0.double()) < 1e-6, B
+    assert rel_err(out["dx"], dense_chain_ref([w0] + [None] * 5, dz3=dz3)["dx"]) < 1e-6, B
     # nothing but dx is written in this mode
     for name in HEAD_OUT:
         if name != "dz3":
@@ -156,12 +122,9 @@ def test_head_and_tail_three_launches_bit_identical(nat):
 
 
 @pytest.mark.parametrize("lookahead", [False, True])
-def test_captured_step_pair(nat, monkeypatch, lookahead):
+def test_captured_step_pair(nat, engine, monkeypatch, lookahead):
     """B = 32: the classic step runs the forward kernel with its head and the tail from dz3; the look-ahead step keeps the pair through a3
     (its launch ends with the next batch's forward kernel, which would overwrite the loss and logits the host has not read yet)."""
-    from geomx_b200.parallel import Topology
-    for k in SWITCHES:
-        monkeypatch.delenv(k, raising=False)
     seen = {"fwd": [], "tail": []}
     fwd, tail = nat.cnn_fwd_dense0, nat.dense_tail
     monkeypatch.setattr(nat, "cnn_fwd_dense0", lambda *a, **k: (seen["fwd"].append(k.get("a4") is not None), fwd(*a, **k))[1])
@@ -169,20 +132,14 @@ def test_captured_step_pair(nat, monkeypatch, lookahead):
     B = 32
     g = torch.Generator().manual_seed(901)
     X, y = torch.rand(B, 1, 28, 28, generator=g), torch.randint(0, 10, (B,), generator=g).float()
-    eng = mx.models.HipsCNNTrainStep(batch_size=B, optimizer=mx.optimizer.Adam(learning_rate=0.01), topo=Topology(1, 0, 1, 1), use_graph=True,
-                                     lookahead=lookahead)
-    try:
-        l0 = eng.step(X.pin_memory(), y.pin_memory())
-        for _ in range(5):
-            l1 = eng.step(X.pin_memory(), y.pin_memory())
-        if lookahead:
-            l1 = eng.flush()
-        assert seen["fwd"] and seen["tail"], seen
-        assert set(seen["fwd"]) == {not lookahead} and set(seen["tail"]) == {not lookahead}, seen
-        if not lookahead:
-            assert eng.kernels_per_step == 6, eng.kernels_per_step
-            assert l0 == l0 and l1 < l0, (l0, l1)
-    finally:
-        del eng
-        gc.collect()
-        torch.cuda.empty_cache()
+    eng = engine(B, mx.optimizer.Adam(learning_rate=0.01), use_graph=True, lookahead=lookahead)
+    l0 = eng.step(X.pin_memory(), y.pin_memory())
+    for _ in range(5):
+        l1 = eng.step(X.pin_memory(), y.pin_memory())
+    if lookahead:
+        l1 = eng.flush()
+    assert seen["fwd"] and seen["tail"], seen
+    assert set(seen["fwd"]) == {not lookahead} and set(seen["tail"]) == {not lookahead}, seen
+    if not lookahead:
+        assert eng.kernels_per_step == 6, eng.kernels_per_step
+        assert l0 == l0 and l1 < l0, (l0, l1)

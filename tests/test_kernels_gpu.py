@@ -8,24 +8,9 @@ import torch
 import geomx_b200 as mx
 from geomx_b200.kvstore import compression as gc
 
+from _cnn_ref import dev, engine, nat, rel_err, step_reference  # noqa: F401  (nat, engine: fixtures)
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    return native
-
-
-def dev():
-    return torch.device("cuda", 0)
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-12))
 
 
 # ---------------------------------------------------------------------------------------------------------------- GEMM
@@ -50,77 +35,6 @@ def test_gemm_tf32_majors(nat, a_mn, b_mn, M, N, K):
     finally:
         nat.set_gemm_precision("3xtf32")
     assert 1e-5 < e1 < 2e-3, "plain tf32 mode rel err %g" % e1     # the fast mode really is the 10-bit-mantissa product
-
-
-def test_cnn_direct_kernels_match_torch(nat):
-    """conv0+conv1 forward (bias, ReLU, 2x2 max-pool fused) and the two backward kernels of csrc/kernels/cnn_direct.cu vs autograd on the same ops."""
-    import torch.nn.functional as F
-    torch.manual_seed(21)
-    for B in (32, 6):
-        x = torch.rand(B, 1, 28, 28, device=dev())
-        w0 = torch.randn(16, 1, 5, 5, device=dev()) * 0.2; b0 = torch.randn(16, device=dev()) * 0.1
-        w1 = torch.randn(32, 16, 5, 5, device=dev()) * 0.05; b1 = torch.randn(32, device=dev()) * 0.1
-        a1 = torch.empty(B, 16, 12, 12, device=dev()); idx1 = torch.empty(B, 16, 12, 12, dtype=torch.uint8, device=dev())
-        a2 = torch.empty(B, 32, 4, 4, device=dev()); idx2 = torch.empty(B, 32, 4, 4, dtype=torch.uint8, device=dev())
-        nat.cnn_fwd(x, w0, b0, w1, b1, a1, idx1, a2, idx2)
-        torch.cuda.synchronize()
-        # forward values against fp64
-        xd, w0d, b0d, w1d, b1d = (t.double() for t in (x, w0, b0, w1, b1))
-        h1 = F.max_pool2d(torch.relu(F.conv2d(xd, w0d, b0d)), 2)
-        h2 = F.max_pool2d(torch.relu(F.conv2d(a1.double(), w1d, b1d)), 2)          # second layer from the kernel's own a1
-        assert rel_err(a1, h1) < 1e-6 and rel_err(a2, h2) < 1e-6
-        # backward against fp64 with the kernel's OWN routing decisions (arg-max positions and ReLU masks are discrete: a reference that takes
-        # them in another precision differs by whole pixels on near-ties; cuDNN's fp32 algorithms are only good to ~1e-4 anyway)
-        def route(g, pooled, idx):                  # pooled gradient -> pre-pool map (2x upsampled), one non-zero per window
-            gm = torch.where(pooled > 0, g, torch.zeros_like(g)).double()
-            out = torch.zeros(g.shape[0], g.shape[1], 2 * g.shape[2], 2 * g.shape[3], dtype=torch.float64, device=g.device)
-            for k in range(4):
-                out[:, :, (k >> 1)::2, (k & 1)::2] = torch.where(idx == k, gm, torch.zeros_like(gm))
-            return out
-        da2 = torch.randn(B, 32, 4, 4, device=dev())
-        dz2 = route(da2, a2, idx2)
-        da1 = F.conv_transpose2d(dz2, w1d)
-        ref_dw1 = torch.nn.grad.conv2d_weight(a1.double(), w1.shape, dz2); ref_db1 = dz2.sum((0, 2, 3))
-        dz1 = route(da1, a1, idx1)
-        ref_dw0 = torch.nn.grad.conv2d_weight(xd, w0.shape, dz1); ref_db0 = dz1.sum((0, 2, 3))
-        dw0 = torch.zeros(16, 1, 5, 5, device=dev()); db0 = torch.zeros(16, device=dev())
-        dw1 = torch.full((32, 16, 5, 5), float("nan"), device=dev()); db1 = torch.full((32,), float("nan"), device=dev())
-        nat.cnn_bwd(x, w1, a1, idx1, a2, idx2, da2, dw0, db0)
-        assert nat.cnn_wgrad1(a1, a2, idx2, da2, dw1, db1)
-        torch.cuda.synchronize()
-        for got, ref, name in ((dw0, ref_dw0, "dw0"), (db0, ref_db0, "db0"), (dw1, ref_dw1, "dw1"), (db1, ref_db1, "db1")):
-            assert rel_err(got, ref) < 1e-5, (B, name, rel_err(got, ref))
-        # the one-launch form (heterogeneous grid) computes the same four gradients
-        dw0.zero_(); db0.zero_(); dw1.fill_(float("nan")); db1.fill_(float("nan"))
-        nat.cnn_bwd_all(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1)
-        torch.cuda.synchronize()
-        for got, ref, name in ((dw0, ref_dw0, "dw0"), (db0, ref_db0, "db0"), (dw1, ref_dw1, "dw1"), (db1, ref_db1, "db1")):
-            assert rel_err(got, ref) < 1e-5, (B, "one launch", name, rel_err(got, ref))
-
-
-def test_mlp_chain_matches_torch(nat):
-    """dense0 -> dense1 -> classifier -> softmax-CE fwd+bwd in one cluster launch vs autograd on the same fp32 ops."""
-    import torch.nn.functional as F
-    torch.manual_seed(11)
-    for B in (32, 20):
-        x = torch.randn(B, 512, device=dev()).relu()
-        w0 = (torch.randn(256, 512, device=dev()) * 0.05); b0 = torch.randn(256, device=dev()) * 0.1
-        w1 = (torch.randn(128, 256, device=dev()) * 0.08); b1 = torch.randn(128, device=dev()) * 0.1
-        w2 = (torch.randn(10, 128, device=dev()) * 0.1); b2 = torch.randn(10, device=dev()) * 0.1
-        y = torch.randint(0, 10, (B,), device=dev())
-        ps = [t.clone().requires_grad_(True) for t in (x, w0, b0, w1, b1, w2, b2)]
-        h = torch.relu(F.linear(ps[0], ps[1], ps[2])); h = torch.relu(F.linear(h, ps[3], ps[4])); lg = F.linear(h, ps[5], ps[6])
-        loss_ref = F.cross_entropy(lg, y, reduction="none")
-        loss_ref.sum().backward()
-        e = lambda *s: torch.full(s, float("nan"), device=dev())
-        loss, logits, dx = e(B), e(B, 10), e(B, 512)
-        g = [e(256, 512), e(256), e(128, 256), e(128), e(10, 128), e(10)]
-        assert nat.mlp_chain(x, w0, b0, w1, b1, w2, b2, y.float(), loss, logits, g[0], g[1], g[2], g[3], g[4], g[5], dx)
-        torch.cuda.synchronize()
-        assert rel_err(loss, loss_ref) < 1e-5 and rel_err(logits, lg.detach()) < 1e-5
-        assert rel_err(dx, ps[0].grad) < 1e-5
-        for got, ref in zip(g, [q.grad for q in ps[1:]]):
-            assert rel_err(got, ref) < 1e-5, (B, got.shape, rel_err(got, ref))
 
 
 def test_gemm_epilogues(nat):
@@ -377,34 +291,21 @@ def test_fp8_block_roundtrip(nat):
 
 
 # ---------------------------------------------------------------------------------------------------------------- flagship step
-def _torch_reference_step(P, x, y):
-    import torch.nn.functional as F
-    ps = [p.clone().requires_grad_(True) for p in P]
-    h = F.max_pool2d(torch.relu(F.conv2d(x, ps[0], ps[1])), 2)
-    h = F.max_pool2d(torch.relu(F.conv2d(h, ps[2], ps[3])), 2).flatten(1)
-    h = torch.relu(F.linear(h, ps[4], ps[5])); h = torch.relu(F.linear(h, ps[6], ps[7]))
-    logits = F.linear(h, ps[8], ps[9])
-    loss = F.cross_entropy(logits, y.long(), reduction="none")
-    loss.sum().backward()
-    return loss.detach(), [p.grad for p in ps]
-
-
-def test_fused_step_matches_torch(nat):
-    from geomx_b200.parallel import Topology
+def test_fused_step_matches_torch(nat, engine):
+    """The fused step's gradients against torch's fp64 autograd of the demo CNN (``step_reference``), then one Adam step."""
     torch.manual_seed(15)
-    eng = mx.models.HipsCNNTrainStep(batch_size=32, optimizer=mx.optimizer.Adam(learning_rate=0.01), topo=Topology(1, 0, 1, 1), use_graph=False,
-                                     fused_zero_grad=False)
+    eng = engine(32, mx.optimizer.Adam(learning_rate=0.01), use_graph=False, fused_zero_grad=False)
     X = torch.rand(32, 1, 28, 28, device=dev()); y = torch.randint(0, 10, (32,), device=dev()).float()
     P0 = [p.clone() for p in eng.P]
-    loss_ref, grads_ref = _torch_reference_step(P0, X, y)
     eng.x.copy_(X); eng.label.copy_(y)
     # run everything except the optimizer: call _body with lr = 0 so weights stay put, then inspect the gradient arena
     eng.fabric.set_optimizer(dict(mx.optimizer.SGD(learning_rate=0.0).spec()))
     eng._body(); torch.cuda.synchronize()
+    loss_ref, _, grads_ref, _ = step_reference(P0, X, y, eng.idx1, eng.idx2)
     assert rel_err(eng.loss, loss_ref) < 1e-5
     errs = [rel_err(g, gr) for g, gr in zip(eng.G, grads_ref)]
-    print("fused-step gradient rel errors vs fp32 torch:", ["%.2e" % e for e in errs])
-    # fp32-accurate everywhere (3xTF32 tensor-core products, fp32 FMA elsewhere): only summation order differs from torch
+    print("fused-step gradient rel errors vs fp64:", ["%.2e" % e for e in errs])
+    # fp32-accurate everywhere (3xTF32 tensor-core products, fp32 FMA elsewhere)
     assert max(errs) < 1e-4, errs
     # now one real Adam step on the same batch: w' = w - lr*m̂/(sqrt(v̂)+eps) with g/num_samples pushed; the expectation uses the gradient arena
     # produced by the first pass (identical inputs), so it checks scale + optimizer + broadcast exactly

@@ -1,6 +1,6 @@
 """Learning-rate schedules on the device, host side: ``LRScheduler.device_spec()`` (the one description of a schedule that the update kernels
-evaluate), what ``Optimizer.spec()`` carries, the ctypes packing, the engine's per-key multipliers, and that the update kernels that evaluate
-the schedule still compile without spills.  The device values themselves are checked in ``test_lr_schedule_gpu.py``."""
+evaluate), what ``Optimizer.spec()`` carries, the ctypes packing and the engine's per-key multipliers.  That the update kernels evaluating
+the schedule compile without spills is a row of ``test_kernel_budgets.py``; the device values are checked in ``test_lr_schedule_gpu.py``."""
 import ctypes
 
 import pytest
@@ -9,8 +9,6 @@ import geomx_b200 as mx
 from geomx_b200 import lr_scheduler as S
 from geomx_b200.models.cnn import _key_mults
 from geomx_b200.ops import _native_api as api
-
-from test_fwd_dense0_ptxas import _ptxas
 
 BASE = dict(warmup_steps=0, warmup_begin_lr=0.0, warmup_mode="linear", step=0, factor=1.0, stop_factor_lr=0.0, milestones=[], max_update=0,
             final_lr=0.0, pwr=1.0)
@@ -107,13 +105,3 @@ def test_engine_key_mults():
     m = _key_mults(opt, net)                                     # the net's Parameters win, as gluon.Trainer's param_dict does
     assert m[0] == (0.5, 1.0) and m[2] == (1.0, 1.0)
     assert all(m[i] == (1.0, 0.0) for i in range(1, 10, 2))
-
-
-def test_update_kernels_do_not_spill(tmp_path):
-    """Every update kernel has a constant-lr and a scheduled instance (step_lr<SCHED>): none of them, nor anything else in these files, may
-    spill."""
-    for name in ("optim", "hips_fabric", "cnn_direct"):
-        found = _ptxas(tmp_path, name)
-        assert found, name
-        for kernel, (regs, spills) in found.items():
-            assert not any(spills), (name, kernel, regs, spills)

@@ -17,12 +17,11 @@ import geomx_b200 as mx
 from geomx_b200 import lr_scheduler as S
 
 import _update_ref as R
-from test_update_paths_gpu import (ENGINE_CASES, FAB_PATHS, FAB_SPECS, KEY_MULTS, KEY_SIZES, MIXED_FMTS, PUSH_SCALE, _batches, _clip_for,
-                                   _engine_ref, _fab_grads, _fab_init, _fabric, _snapshot, cleanup, clean_env, dev, half_ulps, nat)
+from _cnn_ref import cleanup, dev, nat  # noqa: F401  (nat: fixture)
+from _update_harness import (ENGINE_CASES, FAB_PATHS, FAB_SPECS, KEY_MULTS, KEY_SIZES, MIXED_FMTS, PUSH_SCALE, TOL, _batches,  # noqa: F401
+                             _clip_for, _engine_ref, _fab_grads, _fab_init, _fabric, _snapshot, clean_env, half_ulps)
 
 pytestmark = pytest.mark.gpu
-
-TOL = R.DISP_TOL
 f32 = lambda x: float(np.float32(x))
 
 

@@ -4,14 +4,13 @@
   over several steps with rescale, clip, wd and momentum active, and with the reference's ``clip_gradient = 0`` quirk;
 * ``spec()`` packed by ``pack_hyper`` into the kernels' ``OptHyper``; the classes without a native kind give None;
 * the ctypes mirrors of ``OptHyper`` / ``FabricParams`` against the layout the C headers assert;
-* the TCP plane ships the pickled optimizer for kinds its C++ server does not run;
-* ptxas at the build's own flags: no update kernel spills, and the exchange kernels keep their register budgets.
+* the TCP plane ships the pickled optimizer for kinds its C++ server does not run.
+
+The update kernels' register and spill budgets are rows of ``test_kernel_budgets.py``.
 """
 import os
 import pickle
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -286,40 +285,3 @@ def test_dist_ps_ships_pickled_optimizer_for_kinds_the_host_server_lacks():
         assert [h for h, _ in sent] == [dist_ps.CMD_CONTROLLER], type(opt).__name__
     _, sent = _dist_ps_set(O.Adam(learning_rate=0.01))
     assert [h for h, _ in sent] == [dist_ps.CMD_OPT_SPEC] and sent[0][1].startswith("name=adam")
-
-
-# -------------------------------------------------------------------------------------------------------- register budgets
-def _ptxas(tmp_path, name):
-    if not (os.path.exists(build.NVCC) or shutil.which(build.NVCC)):
-        pytest.skip("nvcc not available")
-    src = os.path.join(build.CSRC, "kernels", name + ".cu")
-    r = subprocess.run([build.NVCC] + build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o", str(tmp_path / (name + ".o"))],
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout[-4000:]
-    found = {}
-    for block in r.stdout.split("Compiling entry function ")[1:]:
-        spills = [int(v) for v in re.findall(r"(\d+) bytes spill (?:stores|loads)", block)]
-        regs = int(re.search(r"Used (\d+) registers", block).group(1))
-        found[block.split("'")[1]] = (regs, spills)
-    return found
-
-
-@pytest.mark.parametrize("name", ["optim", "hips_fabric", "cnn_direct"])
-def test_update_kernels_do_not_spill(tmp_path, name):
-    found = _ptxas(tmp_path, name)
-    assert found
-    for k, (regs, spills) in found.items():
-        assert spills and not any(spills), (k, spills)
-    if name == "optim":
-        # one instance per kind: arena x {constant, scheduled lr}, multi-tensor, single-tensor
-        for kern, per_kind in (("arena_opt_kernel", 2), ("multi_tensor_opt_kernel", 1), ("single_opt_kernel", 1)):
-            assert sum(kern in k for k in found) == per_kind * len(api.OPT_KINDS), kern
-    if name == "hips_fabric":
-        for kern in ("hips_fsa_ll_kernel", "hips_fsa_direct_kernel"):
-            inst = {k: v for k, v in found.items() if kern in k}
-            # constant / scheduled lr, with / without the kinds after DCASGD; __launch_bounds__(256, 2)
-            assert len(inst) == 4 and all(r <= 128 for r, _ in inst.values()), inst
-    if name == "cnn_direct":
-        inst = {k: v for k, v in found.items() if "cnn_bwd_exchange_kernel" in k}
-        # two 288-thread CTAs per SM, which the kernel's ticket wait needs
-        assert len(inst) == 4 and all(r <= 112 for r, _ in inst.values()), inst

@@ -16,8 +16,9 @@ import geomx_b200 as mx
 from geomx_b200.models.cnn import LOCAL
 
 import _optim_ref as R
-from test_update_paths_gpu import (A, C, FAB_PATHS, KEY_MULTS, KEY_SIZES, ONE, PUSH_SCALE, TOL, _batches, _clip_for, _fab_grads,  # noqa: F401
-                                   _fab_init, _fabric, _padding_zero, _snapshot, cleanup, clean_env, dev, half_ulps, nat)
+from _cnn_ref import cleanup, dev, nat  # noqa: F401  (nat: fixture)
+from _update_harness import (A, C, FAB_PATHS, KEY_MULTS, KEY_SIZES, ONE, PUSH_SCALE, TOL, _batches, _clip_for, _fab_grads,  # noqa: F401
+                             _fab_init, _fabric, _padding_zero, _snapshot, clean_env, half_ulps)
 
 pytestmark = pytest.mark.gpu
 

@@ -8,7 +8,6 @@ path of ``test_step_paths_gpu.py``.
 Bitwise comparisons between two engines freeze the convolution keys (``lr_mult = 0``): conv0's weight gradient is summed with atomics, so
 two runs of the same step differ in its last bits, and through the next forward pass everywhere.  With the convolution weights fixed the
 rest of the step is deterministic, and a weighted step that should equal an unweighted one must equal it bit for bit."""
-import gc
 import os
 import subprocess
 import sys
@@ -16,28 +15,17 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import geomx_b200 as mx
-from geomx_b200.models.cnn import CNN_PARAM_NAMES, STEP_SWITCHES
+from geomx_b200.models.cnn import CNN_PARAM_NAMES
 from geomx_b200.parallel import Topology
 
 import _update_ref as U
-from test_step_paths_gpu import CASES, GRAD_NAMES, PATHS, conv_forward_ref, dev, images, nat, step_params  # noqa: F401  (nat: fixture)
+from _cnn_ref import CASE_IDS, CASES, GRAD_NAMES, PATHS, ROOT, dev, engine, images, nat, step_params, step_reference  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FROZEN_CONV = {0: 0.0, 1: 0.0, 2: 0.0, 3: 0.0}
-
-
-@pytest.fixture(autouse=True)
-def _clean_switches(monkeypatch):
-    for k in STEP_SWITCHES:
-        monkeypatch.delenv(k, raising=False)
-    yield
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 def coefficients(B, n, w):
@@ -46,15 +34,10 @@ def coefficients(B, n, w):
     return c
 
 
-def weighted_reference(P, x, y, c, idx1, idx2):
-    """fp64 autograd of sum_i c_i loss_i over the padded batch: the per-sample loss and the 10 gradients."""
-    ps = [p.detach().double().requires_grad_(True) for p in P]
-    _, a2, _ = conv_forward_ref(x.double(), ps[0], ps[1], ps[2], ps[3], idx1, idx2)
-    h = torch.relu(F.linear(a2.flatten(1), ps[4], ps[5]))
-    h = torch.relu(F.linear(h, ps[6], ps[7]))
-    loss = F.cross_entropy(F.linear(h, ps[8], ps[9]), y.long(), reduction="none")
-    (loss * c.to(loss.device)).sum().backward()
-    return loss.detach(), [p.grad for p in ps]
+def frozen(opt):
+    """``opt`` with the convolution keys frozen (lr_mult = 0)."""
+    opt.set_lr_mult(FROZEN_CONV)
+    return opt
 
 
 def variants(B):
@@ -63,14 +46,6 @@ def variants(B):
     even = next((k for k in range(B // 2, 0, -1) if k % 2 == 0 and k not in (1, B - 1)), None)
     out = [(k, k == odd) for k in sorted({1, B - 1} | {v for v in (odd, even) if v}) if 1 <= k < B]
     return out + [(B, True)]
-
-
-def engine(B, opt=None, frozen=False, **kw):
-    opt = opt or mx.optimizer.SGD(learning_rate=0.0)
-    if frozen:
-        opt.set_lr_mult(FROZEN_CONV)
-    kw.setdefault("topo", Topology(1, 0, 1, 1))
-    return mx.models.HipsCNNTrainStep(batch_size=B, optimizer=opt, **kw)
 
 
 def same_init(a, b):
@@ -105,15 +80,13 @@ def batch(g, n, kind="rand"):
 
 
 # ------------------------------------------------------------------------------------------------------------- 1. gradients vs fp64
-@pytest.mark.parametrize("path,B,env", CASES, ids=["%s-B%d" % (p, b) for p, b, _ in CASES])
-def test_partial_and_weighted_gradients_match_fp64(nat, monkeypatch, path, B, env):
+@pytest.mark.parametrize("path,B,env", CASES, ids=CASE_IDS)
+def test_partial_and_weighted_gradients_match_fp64(nat, engine, path, B, env):
     """Short batches (n = 1, odd, even, B - 1) and a weighted full batch on every kernel path: G = sum_i c_i grad_i and the per-sample loss
     against fp64 (2e-5 relative, as the full-batch path tests); the handle reports w_i * loss_i and its mean over n."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
     g = torch.Generator().manual_seed(500 + 3 * B + ord(path))
     P0 = step_params(g)
-    eng = engine(B, use_graph=False, fused_zero_grad=False)
+    eng = engine(B, env=env, use_graph=False, fused_zero_grad=False)
     for p, v in zip(eng.P, P0):
         p.copy_(v)
     eng.fabric.load_master_from_param()
@@ -127,7 +100,7 @@ def test_partial_and_weighted_gradients_match_fp64(nat, monkeypatch, path, B, en
         Xp = torch.zeros(B, 1, 28, 28); Xp[:n] = X
         yp = torch.zeros(B); yp[:n] = y
         c = coefficients(B, n, w)
-        loss_ref, grads_ref = weighted_reference(P0, Xp.to(dev()), yp.to(dev()), c, eng.idx1, eng.idx2)
+        loss_ref, _, grads_ref, _ = step_reference(P0, Xp.to(dev()), yp.to(dev()), eng.idx1, eng.idx2, coef=c)
         errs = {n_: U.rel(a, b) for n_, a, b in zip(GRAD_NAMES, eng.G, grads_ref)}
         lref = loss_ref[:n].cpu() * (1.0 if w is None else w.double())
         errs["loss"] = U.rel(lw, lref)
@@ -138,7 +111,6 @@ def test_partial_and_weighted_gradients_match_fp64(nat, monkeypatch, path, B, en
         assert not bad, (path, B, n, bad)
         for i, (p, p0) in enumerate(zip(eng.P, P0)):
             assert torch.equal(p, p0), "parameter %d changed by an lr = 0 step" % i
-    del eng
 
 
 # ------------------------------------------------------------------------------------------------------------- 2. ones are exact
@@ -153,12 +125,12 @@ MODES = {
 
 
 @pytest.mark.parametrize("mode", list(MODES))
-def test_unit_weights_are_bitwise_unweighted(nat, mode):
+def test_unit_weights_are_bitwise_unweighted(nat, engine, mode):
     """sample_weight = ones(B) replays the weighted graph, and its coefficient 1 must leave every bit as the unweighted step has it:
     parameters, optimizer state and the reported loss, over several steps (conv keys frozen, see the module docstring)."""
     B, opt, kw = MODES[mode]
     g = torch.Generator().manual_seed(11)
-    a, b = engine(B, opt(), frozen=True, **kw), engine(B, opt(), frozen=True, **kw)
+    a, b = engine(B, frozen(opt()), **kw), engine(B, frozen(opt()), **kw)
     same_init(a, b)
     la, lb = [], []
     for _ in range(4):
@@ -175,16 +147,15 @@ def test_unit_weights_are_bitwise_unweighted(nat, mode):
         assert abs(fa - fb) <= 1e-5 * abs(fa), (fa, fb)
     assert np.array_equal(np.array(la), np.array(lb), equal_nan=True), (la, lb)
     assert_same_state(a, b)
-    del a, b
 
 
 # ------------------------------------------------------------------------------------------------------------- 3. zero-weight rows
 @pytest.mark.parametrize("B", [32, 31, 48])
-def test_zero_weight_rows_are_inert(nat, B):
+def test_zero_weight_rows_are_inert(nat, engine, B):
     """Rows of weight 0 contribute exact zeros: other finite images and labels in them leave parameters and optimizer state bitwise equal."""
     g = torch.Generator().manual_seed(21 + B)
     opt = lambda: mx.optimizer.Adam(learning_rate=0.01)
-    a, b = engine(B, opt(), frozen=True), engine(B, opt(), frozen=True)
+    a, b = engine(B, frozen(opt())), engine(B, frozen(opt()))
     same_init(a, b)
     for _ in range(3):
         X, y = batch(g, B)
@@ -198,13 +169,12 @@ def test_zero_weight_rows_are_inert(nat, B):
         assert torch.equal(la, lb)
     torch.cuda.synchronize()
     assert_same_state(a, b)
-    del a, b
 
 
 # ------------------------------------------------------------------------------------------------------------- 4. a batch-n engine
 @pytest.mark.parametrize("B,n,kw", [(32, 12, {}), (48, 31, {}), (32, 7, {"lookahead": True, "loopback": True, "topo": Topology(1, 0, 1, 0)})],
                          ids=["A-n12", "D-n31", "lookahead-n7"])
-def test_short_batch_matches_batch_n_engine(nat, B, n, kw):
+def test_short_batch_matches_batch_n_engine(nat, engine, B, n, kw):
     """A short batch of n rows on a batch-B engine updates the weights as an engine built for batch n does on the same rows (SGD; fp32
     tolerance: the two run different kernel paths), for three steps."""
     g = torch.Generator().manual_seed(31 + n)
@@ -221,11 +191,10 @@ def test_short_batch_matches_batch_n_engine(nat, B, n, kw):
     errs = [U.rel(pb - p0, ps - p0) for pb, ps, p0 in zip(big.P, small.P, P0)]
     print("\n  B=%d n=%d: displacement rel err %s" % (B, n, " ".join("%.1e" % e for e in errs)))
     assert max(errs) < 1e-4, errs
-    del big, small
 
 
 # ------------------------------------------------------------------------------------------------------------- 5. graphs
-def test_weighted_graphs(nat):
+def test_weighted_graphs(nat, engine):
     """Weighted steps replay graphs of their own, one per input buffer, with the step's kernel count; a full unweighted step afterwards
     replays the original graph, captured once; set_learning_rate drops both kinds."""
     B = 32
@@ -247,18 +216,17 @@ def test_weighted_graphs(nat):
     assert eng.graph is None and not eng._graph_w
     eng.step(*batch(g, 3))
     assert eng._graph_w and eng.kernels_per_step == k
-    del eng
 
 
 # ------------------------------------------------------------------------------------------------------------- 6. look-ahead checkpoint
-def test_lookahead_short_batch_checkpoint(nat, tmp_path):
+def test_lookahead_short_batch_checkpoint(nat, engine, tmp_path):
     """A short, weighted batch primed last before flush(): a save_states / load_states round trip resumes it bitwise (conv keys frozen),
     the file holds batch:weight, and a file saved with a full unweighted primed batch does not."""
     B = 32
     g = torch.Generator().manual_seed(51)
     kw = dict(lookahead=True, loopback=True, topo=Topology(1, 0, 1, 0))
     opt = lambda: mx.optimizer.Adam(learning_rate=0.01)
-    a = engine(B, opt(), frozen=True, **kw)
+    a = engine(B, frozen(opt()), **kw)
     for _ in range(2):
         a.step(*batch(g, B))
     full = str(tmp_path / "full.params")
@@ -272,16 +240,15 @@ def test_lookahead_short_batch_checkpoint(nat, tmp_path):
     c = mx.nd.load(short)["batch:weight"].asnumpy()
     assert c.shape == (1, B) and np.array_equal(c[0, 13:], np.zeros(B - 13, np.float32))
     assert np.allclose(c[0, :13], w.numpy() * B / 13, rtol=1e-6)
-    b = engine(B, opt(), frozen=True, **kw)
+    b = engine(B, frozen(opt()), **kw)
     b.load_states(short)
     la, lb = a.flush(), b.flush()
     torch.cuda.synchronize()
     assert la == la and abs(la - lb) <= 1e-6 * abs(la), (la, lb)
     assert_same_state(a, b)
-    del a, b
 
 
-def test_lookahead_short_batch_before_flush_trains(nat):
+def test_lookahead_short_batch_before_flush_trains(nat, engine):
     """The last, short batch of a look-ahead run is trained by flush() with its own coefficients: the same weights (within fp32) as an
     engine without look-ahead after the same batches."""
     B = 32
@@ -298,11 +265,10 @@ def test_lookahead_short_batch_before_flush_trains(nat):
     torch.cuda.synchronize()
     errs = [U.rel(p - p0, q - p0) for p, q, p0 in zip(la.P, plain.P, P0)]
     assert max(errs) < 1e-4 and loss == loss, (errs, loss)
-    del la, plain
 
 
 # ------------------------------------------------------------------------------------------------------------- 7. errors
-def test_refusals_enqueue_nothing(nat):
+def test_refusals_enqueue_nothing(nat, engine):
     from geomx_b200.ops import native
     B = 8
     eng = engine(B, use_graph=False)
@@ -314,7 +280,6 @@ def test_refusals_enqueue_nothing(nat):
         with pytest.raises(ValueError):
             eng.step_async(*args)
     assert (native.launch_count, eng.steps_done, eng._pipeline()["n"]) == before
-    del eng
 
 
 # ------------------------------------------------------------------------------------------------------------- 8. several ranks

@@ -4,7 +4,8 @@ exchange variants at one and at several ranks.  Every check compares the whole r
 import pytest
 
 from geomx_b200.models.cnn import STEP_SWITCHES, StepPath, step_path
-from test_step_paths_gpu import CASES
+
+from _cnn_ref import CASE_IDS, CASES
 
 # path -> the fields that set it apart; the rest are those of one rank with default switches (see classic())
 PATHS = {
@@ -28,7 +29,7 @@ def classic(path, **fields):
     return StepPath(**rec)
 
 
-@pytest.mark.parametrize("path,B,env", CASES, ids=["%s-B%d" % (p, b) for p, b, _ in CASES])
+@pytest.mark.parametrize("path,B,env", CASES, ids=CASE_IDS)
 def test_paths_a_to_g(path, B, env):
     assert step_path(B, conv_tail_capable=True, env=env) == classic(path)
 

@@ -21,263 +21,83 @@ first position, like torch's max-pool.
 The file also tests the direct convolution kernels at their edges (list densities, batch limits, output contracts), the kernels of the GEMM
 paths that the step calls but no other test does, the loss of confidently classified samples, and the split-K GEMM epilogue contract.
 """
-import gc
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-import geomx_b200 as mx
-from geomx_b200.models.cnn import DENSE_KV, DENSE_WGRAD, DIRECT_FWD, EXCH, FUSED_BWD, GEMM_FWD, MLP, ONE_GRID, STEP_SWITCHES
+from _cnn_ref import (CASE_IDS, CASES, GRAD_NAMES, PATHS, check_routing, conv_forward_ref, conv_params, dev, engine, images, nan,  # noqa: F401
+                      nat, rel_err, route, step_params, step_reference, windows)
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def nat():
-    from geomx_b200.ops import native
-    native.require()
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    return native
-
-
-def dev():
-    return torch.device("cuda", 0)
-
-
-def rel_err(a, b):
-    return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-30))
-
-
-def nan_like(shape, dtype=torch.float32):
-    if dtype == torch.uint8:
-        return torch.full(shape, 255, dtype=dtype, device=dev())
-    return torch.full(shape, float("nan"), dtype=dtype, device=dev())
-
-
-# ---------------------------------------------------------------------------------------------------------------- fp64 reference pieces
-def windows(z):
-    """(B, C, H, W) -> (B, C, H/2, W/2, 4): the four candidates of every 2x2 pooling window, position k = 2*dy + dx (the kernels' idx)."""
-    B, C, H, W = z.shape
-    return z.reshape(B, C, H // 2, 2, W // 2, 2).permute(0, 1, 2, 4, 3, 5).reshape(B, C, H // 2, W // 2, 4)
-
-
-def pool_at(z, idx):
-    """Max-pool of ``z`` routed by the given arg-max positions (differentiable: the gradient goes to the chosen position only)."""
-    return windows(z).gather(-1, idx.long().unsqueeze(-1)).squeeze(-1)
-
-
-def route(g, idx):
-    """Pooled gradient (B, C, h, w) -> pre-pool map (B, C, 2h, 2w) with the value at the arg-max position of each window."""
-    B, C, h, w = g.shape
-    out = torch.zeros(B, C, 2 * h, 2 * w, dtype=g.dtype, device=g.device)
-    for k in range(4):
-        out[:, :, (k >> 1)::2, (k & 1)::2] = torch.where(idx == k, g, torch.zeros_like(g))
-    return out
-
-
-def check_routing(what, idx, z, zabs, bias):
-    """Compare a kernel's max-pool arg-max ``idx`` with the first maximum of the fp64 pre-bias map ``z`` (bias is per channel, so it does
-    not change the order).  ``zabs`` = the same convolution of |input| with |weights|: the scale of the fp32 rounding error of ``z``.
-
-    Windows whose pooled value is not clearly positive get no gradient whichever position is taken, and are skipped.  Windows whose top
-    candidates differ by more than fp64 rounding but by at most 1e-6 of the scale are near-ties: fp32 may order them either way; they are
-    skipped and counted.  Every other window must match, exact ties included (first position wins).  Returns (near-ties, exact ties)."""
-    cand = windows(z)
-    scale = windows(zabs).amax(-1) + bias.abs().view(1, -1, 1, 1)
-    top = cand.amax(-1)
-    gap = top.unsqueeze(-1) - cand
-    exact = gap <= 1e-12 * scale.unsqueeze(-1)                  # candidates equal to the maximum up to fp64 rounding
-    near = ((~exact) & (gap <= 1e-6 * scale.unsqueeze(-1))).any(-1)
-    first = torch.full(top.shape, 3, dtype=torch.long, device=z.device)
-    for k in (2, 1, 0):
-        first = torch.where(exact[..., k], torch.full_like(first, k), first)
-    live = (top + bias.view(1, -1, 1, 1)) > 1e-6 * scale
-    checked = live & ~near
-    bad = checked & (idx.long() != first)
-    assert not bool(bad.any()), "%s: %d of %d windows disagree with the fp64 first maximum (first at %s)" % (
-        what, int(bad.sum()), int(checked.sum()), bad.nonzero()[0].tolist())
-    n_near = int((live & near).sum())
-    assert n_near <= max(4, int(1e-4 * checked.numel())), "%s: %d near-tie windows" % (what, n_near)
-    return n_near, int((checked & (exact.sum(-1) > 1)).sum())
-
-
-def conv_forward_ref(x, w0, b0, w1, b1, idx1, idx2):
-    """fp64 conv0 -> ReLU -> pool -> conv1 -> ReLU -> pool, pooled at the kernels' arg-max positions; also checks those positions."""
-    z1 = F.conv2d(x, w0)
-    a1 = torch.relu(pool_at(z1, idx1) + b0.view(1, -1, 1, 1))
-    z2 = F.conv2d(a1, w1)
-    a2 = torch.relu(pool_at(z2, idx2) + b1.view(1, -1, 1, 1))
-    with torch.no_grad():
-        r1 = check_routing("idx1", idx1, z1, F.conv2d(x.abs(), w0.abs()), b0)
-        r2 = check_routing("idx2", idx2, z2, F.conv2d(a1.abs(), w1.abs()), b1)
-    return a1, a2, r1 + r2
-
-
-def step_reference(P, x, y, idx1, idx2):
-    """The whole step in fp64 autograd: per-sample loss, logits and the 10 parameter gradients (sums over the batch)."""
-    ps = [p.detach().double().requires_grad_(True) for p in P]
-    _, a2, ties = conv_forward_ref(x.double(), ps[0], ps[1], ps[2], ps[3], idx1, idx2)
-    h = torch.relu(F.linear(a2.flatten(1), ps[4], ps[5]))
-    h = torch.relu(F.linear(h, ps[6], ps[7]))
-    logits = F.linear(h, ps[8], ps[9])
-    loss = F.cross_entropy(logits, y.long(), reduction="none")
-    loss.sum().backward()
-    return loss.detach(), logits.detach(), [p.grad for p in ps], ties
-
-
-# ---------------------------------------------------------------------------------------------------------------- data
-def images(g, B, kind):
-    """'rand': uniform noise.  'patch': a zero background with a 12x12 random patch in the middle, like the demo's digits: every conv0
-    window in the background is an exact four-way tie."""
-    x = torch.rand(B, 1, 28, 28, generator=g)
-    if kind == "patch":
-        bg = torch.zeros_like(x)
-        bg[:, :, 8:20, 8:20] = x[:, :, 8:20, 8:20]
-        x = bg
-    return x.to(dev())
-
-
-def conv_params(g, regime="default"):
-    """conv0 / conv1 weights and biases.  'posbias': b0 > 0, so the background ties of 'patch' images have a positive pooled value and
-    carry gradient; 'full': b1 = +5 (a2 > 0 everywhere: every per-window list of the data-gradient kernel holds 32 entries); 'empty':
-    b1 = -5 (a2 = 0 everywhere, empty lists); 'dead0': b0 = -5 (a1 = 0 everywhere: every pixel skips its gradient sum)."""
-    w0 = torch.randn(16, 1, 5, 5, generator=g) * 0.2
-    b0 = torch.randn(16, generator=g) * 0.1
-    w1 = torch.randn(32, 16, 5, 5, generator=g) * 0.05
-    b1 = torch.randn(32, generator=g) * 0.1
-    if regime == "posbias":
-        b0 = 0.05 + 0.1 * torch.rand(16, generator=g)
-    elif regime == "full":
-        b1 = torch.full((32,), 5.0)
-    elif regime == "empty":
-        b1 = torch.full((32,), -5.0)
-    elif regime == "dead0":
-        b0 = torch.full((16,), -5.0)
-    return [t.to(dev()) for t in (w0, b0, w1, b1)]
-
-
-def step_params(g):
-    P = conv_params(g, "posbias")
-    for n_out, n_in in ((256, 512), (128, 256), (10, 128)):
-        P += [(torch.randn(n_out, n_in, generator=g) / math.sqrt(n_in)).to(dev()), (torch.randn(n_out, generator=g) * 0.1).to(dev())]
-    return P
-
-
 # ---------------------------------------------------------------------------------------------------------------- 1. the step, per path
-# the ordered (launch, stream) lists of the step on one rank (overlapped channels: the dense keys' exchange on the comm stream)
-WGRAD_KV = (DENSE_WGRAD + " + " + DENSE_KV, "comm")
-GEMM_CONV_FWD = [(GEMM_FWD[0], "main"), (GEMM_FWD[1], "main")]
-GEMM_CONV_BWD = [("pool+relu bwd -> rows", "main"), ("dWc1 gemm (split-K)", "side"), ("dcol1 gemm", "main"), ("conv0 wgrad + col2im", "main")]
-GEMM_HEAD = [("dense0 gemm", "main"), ("dense1 gemm", "main"), ("head fwd+bwd", "main"), ("dW1 gemm", "side"), ("dz3 gemm (mask,colsum)", "main"),
-             ("dW0 gemm", "side"), ("da2 gemm", "main")]
-
-# path -> (direct_conv, fused_mlp, fused_exchange, the step's (launch, stream) list)
-PATHS = {
-    "A": (True, True, False, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, (ONE_GRID, "main"), (EXCH, "join")]),
-    "B": (True, True, False, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, ("conv1 wgrad (direct, sparse)", "side"),
-                              ("conv1 dgrad + conv0 wgrad (direct)", "main"), (EXCH, "join")]),
-    "C": (True, True, True, [(DIRECT_FWD, "main"), (MLP, "main"), WGRAD_KV, (FUSED_BWD, "main")]),
-    "D": (True, False, False, [(DIRECT_FWD, "main")] + GEMM_HEAD + [(DENSE_KV, "comm"), (ONE_GRID, "main"), (EXCH, "join")]),
-    "E": (False, True, False, GEMM_CONV_FWD + [(MLP, "main"), WGRAD_KV] + GEMM_CONV_BWD + [(EXCH, "join")]),
-    "F": (False, True, False, GEMM_CONV_FWD + [(MLP, "main"), WGRAD_KV] + GEMM_CONV_BWD + [(EXCH, "join")]),
-    "G": (False, False, False, GEMM_CONV_FWD + GEMM_HEAD + [(DENSE_KV, "comm")] + GEMM_CONV_BWD + [(EXCH, "join")]),
-}
-CASES = [("A", 2, {}), ("A", 32, {}),
-         ("B", 32, {"GEOMX_CNN_BWD_ONE_LAUNCH": "0"}),
-         ("C", 32, {"GEOMX_FUSED_EXCHANGE": "1"}),
-         ("D", 48, {}), ("D", 64, {}), ("D", 32, {"GEOMX_FUSED_MLP": "0"}),
-         ("E", 1, {}), ("E", 31, {}), ("E", 32, {"GEOMX_DIRECT_CONV": "0"}),
-         ("F", 32, {"GEOMX_DIRECT_CONV": "0", "GEOMX_NO_POOL_FUSION": "1"}),
-         ("G", 33, {}), ("G", 96, {})]
-GRAD_NAMES = ["dw0", "db0", "dw1", "db1", "dW2", "db2", "dW3", "db3", "dW4", "db4"]
-
-
 @pytest.mark.parametrize("data", ["rand", "patch"])
-@pytest.mark.parametrize("path,B,env", CASES, ids=["%s-B%d" % (p, b) for p, b, _ in CASES])
-def test_step_path_matches_fp64(nat, monkeypatch, path, B, env, data):
+@pytest.mark.parametrize("path,B,env", CASES, ids=CASE_IDS)
+def test_step_path_matches_fp64(nat, engine, path, B, env, data):
     """One training step of every kernel path: per-sample loss, logits and all 10 gradients against fp64 autograd (2e-5 relative: the
     direct convolutions are exact fp32 FMA chains, the GEMMs 3xTF32 = fp32-accurate; measured errors are printed).  A second pass on the same
     batch must give the same gradients: accumulators (column sums, conv0 bias atomics) and the fused exchange's ticket / round counters
     have to re-arm themselves.  With SGD at lr = 0 the exchange must also hand back the parameters unchanged."""
-    from geomx_b200.parallel import Topology
-    for k in STEP_SWITCHES:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
     g = torch.Generator().manual_seed(1000 * B + (7 if data == "patch" else 0) + ord(path))
     P0 = step_params(g)
     X = images(g, B, data)
     y = torch.randint(0, 10, (B,), generator=g).float().to(dev())
-    eng = mx.models.HipsCNNTrainStep(batch_size=B, optimizer=mx.optimizer.SGD(learning_rate=0.0), topo=Topology(1, 0, 1, 1), use_graph=False,
-                                     fused_zero_grad=False)
-    try:
-        for p, v in zip(eng.P, P0):
-            p.copy_(v)
-        eng.fabric.load_master_from_param()
-        eng.x.copy_(X); eng.label.copy_(y)
-        eng.z2.fill_(float("nan"))
-        eng._body(); torch.cuda.synchronize()
-        # the intended kernels ran (otherwise a case would quietly test another path)
-        direct, fused_mlp, fused_exchange, want = PATHS[path]
-        steps = [(n, s) for n, s, _ in eng._steps()]
-        assert (eng.direct_conv, eng.fused_mlp, eng.fused_exchange) == (direct, fused_mlp, fused_exchange), (path, B, steps)
-        assert steps == want, (path, B, steps)
-        if not direct:        # the pooled conv1 GEMM leaves z2 untouched; the unfused form writes it and pools it separately
-            assert bool(torch.isnan(eng.z2).all()) == (path != "F"), path
-        loss, logits = eng.loss.clone(), eng.logits.clone()
-        grads = [t.clone() for t in eng.G]
-        loss_ref, logits_ref, grads_ref, ties = step_reference(P0, X, y, eng.idx1, eng.idx2)
-        errs = {"loss": rel_err(loss, loss_ref), "logits": rel_err(logits, logits_ref)}
-        errs.update({n: rel_err(a, b) for n, a, b in zip(GRAD_NAMES, grads, grads_ref)})
-        print("\n  path %s B=%-2d %-5s  near-ties conv0/conv1 %d/%d, exact ties %d/%d  |  %s" % (
-            path, B, data, ties[0], ties[2], ties[1], ties[3], "  ".join("%s %.1e" % kv for kv in errs.items())))
-        bad = {k: v for k, v in errs.items() if not v < 2e-5}
-        assert not bad, (path, B, data, bad)
-        # second pass on the same batch: same result, parameters untouched
-        eng._body(); torch.cuda.synchronize()
-        again = [rel_err(a, b) for a, b in zip(eng.G, grads)]
-        assert max(again) < 1e-6 and rel_err(eng.loss, loss) < 1e-6, (path, B, data, again)
-        for i, (p, p0) in enumerate(zip(eng.P, P0)):
-            assert torch.equal(p, p0), "parameter %d changed by an lr = 0 step (path %s)" % (i, path)
-    finally:
-        del eng
-        gc.collect()
-        torch.cuda.empty_cache()
+    eng = engine(B, env=env, use_graph=False, fused_zero_grad=False)
+    for p, v in zip(eng.P, P0):
+        p.copy_(v)
+    eng.fabric.load_master_from_param()
+    eng.x.copy_(X); eng.label.copy_(y)
+    eng.z2.fill_(float("nan"))
+    eng._body(); torch.cuda.synchronize()
+    # the intended kernels ran (otherwise a case would quietly test another path)
+    direct, fused_mlp, fused_exchange, want = PATHS[path]
+    steps = [(n, s) for n, s, _ in eng._steps()]
+    assert (eng.direct_conv, eng.fused_mlp, eng.fused_exchange) == (direct, fused_mlp, fused_exchange), (path, B, steps)
+    assert steps == want, (path, B, steps)
+    if not direct:        # the pooled conv1 GEMM leaves z2 untouched; the unfused form writes it and pools it separately
+        assert bool(torch.isnan(eng.z2).all()) == (path != "F"), path
+    loss, logits = eng.loss.clone(), eng.logits.clone()
+    grads = [t.clone() for t in eng.G]
+    loss_ref, logits_ref, grads_ref, ties = step_reference(P0, X, y, eng.idx1, eng.idx2)
+    errs = {"loss": rel_err(loss, loss_ref), "logits": rel_err(logits, logits_ref)}
+    errs.update({n: rel_err(a, b) for n, a, b in zip(GRAD_NAMES, grads, grads_ref)})
+    print("\n  path %s B=%-2d %-5s  near-ties conv0/conv1 %d/%d, exact ties %d/%d  |  %s" % (
+        path, B, data, ties[0], ties[2], ties[1], ties[3], "  ".join("%s %.1e" % kv for kv in errs.items())))
+    bad = {k: v for k, v in errs.items() if not v < 2e-5}
+    assert not bad, (path, B, data, bad)
+    # second pass on the same batch: same result, parameters untouched
+    eng._body(); torch.cuda.synchronize()
+    again = [rel_err(a, b) for a, b in zip(eng.G, grads)]
+    assert max(again) < 1e-6 and rel_err(eng.loss, loss) < 1e-6, (path, B, data, again)
+    for i, (p, p0) in enumerate(zip(eng.P, P0)):
+        assert torch.equal(p, p0), "parameter %d changed by an lr = 0 step (path %s)" % (i, path)
 
 
-def test_switches_are_read_at_construction(nat, monkeypatch):
+def test_switches_are_read_at_construction(nat, engine, monkeypatch):
     """The kernel path is chosen when the engine is constructed: step switches changed afterwards change neither the step's launches nor the
     graph that the host pipeline captures later on its second input buffer."""
-    from geomx_b200.parallel import Topology
-    for k in STEP_SWITCHES:
-        monkeypatch.delenv(k, raising=False)
     B = 32
-    eng = mx.models.HipsCNNTrainStep(batch_size=B, optimizer=mx.optimizer.SGD(learning_rate=0.0), topo=Topology(1, 0, 1, 1), use_graph=True)
-    try:
-        g = torch.Generator().manual_seed(77)
-        eng.x.copy_(images(g, B, "rand")); eng.label.copy_(torch.randint(0, 10, (B,), generator=g).float().to(dev()))
-        steps = [(n, s) for n, s, _ in eng._steps()]
-        assert steps == PATHS["A"][3], steps
-        eng.capture(); torch.cuda.synchronize()
-        assert eng.kernels_per_step == 6, eng.kernels_per_step
-        for k, v in (("GEOMX_CNN_BWD_ONE_LAUNCH", "0"), ("GEOMX_FUSED_EXCHANGE", "1"), ("GEOMX_DIRECT_CONV", "0"), ("GEOMX_FUSED_MLP", "0"),
-                     ("GEOMX_E2E_DIRECT_INPUT", "0")):
-            monkeypatch.setenv(k, v)
-        assert [(n, s) for n, s, _ in eng._steps()] == steps
-        eng._pipeline()
-        eng._alt_graph(); torch.cuda.synchronize()
-        assert eng.kernels_per_step == 6, eng.kernels_per_step
-    finally:
-        del eng
-        gc.collect()
-        torch.cuda.empty_cache()
+    eng = engine(B, use_graph=True)
+    g = torch.Generator().manual_seed(77)
+    eng.x.copy_(images(g, B, "rand")); eng.label.copy_(torch.randint(0, 10, (B,), generator=g).float().to(dev()))
+    steps = [(n, s) for n, s, _ in eng._steps()]
+    assert steps == PATHS["A"][3], steps
+    eng.capture(); torch.cuda.synchronize()
+    assert eng.kernels_per_step == 6, eng.kernels_per_step
+    for k, v in (("GEOMX_CNN_BWD_ONE_LAUNCH", "0"), ("GEOMX_FUSED_EXCHANGE", "1"), ("GEOMX_DIRECT_CONV", "0"), ("GEOMX_FUSED_MLP", "0"),
+                 ("GEOMX_E2E_DIRECT_INPUT", "0")):
+        monkeypatch.setenv(k, v)
+    assert [(n, s) for n, s, _ in eng._steps()] == steps
+    eng._pipeline()
+    eng._alt_graph(); torch.cuda.synchronize()
+    assert eng.kernels_per_step == 6, eng.kernels_per_step
 
 
 # ---------------------------------------------------------------------------------------------------------------- 2. cnn_direct.cu at its edges
-DIRECT_CASES = [(B, "rand", "default") for B in (1, 2, 3, 63, 64, 256)] + [(32, "patch", "posbias"), (6, "patch", "posbias")] + \
+DIRECT_CASES = [(B, "rand", "default") for B in (1, 2, 3, 6, 32, 63, 64, 256)] + [(32, "patch", "posbias"), (6, "patch", "posbias")] + \
                [(8, "rand", r) for r in ("full", "empty", "dead0")]
 
 
@@ -289,8 +109,8 @@ def test_cnn_direct_kernels_at_edges(nat, B, data, regime):
     x = images(g, B, data)
     w0, b0, w1, b1 = conv_params(g, regime)
     da2 = torch.randn(B, 32, 4, 4, generator=g).to(dev())
-    a1, idx1 = nan_like((B, 16, 12, 12)), nan_like((B, 16, 12, 12), torch.uint8)
-    a2, idx2 = nan_like((B, 32, 4, 4)), nan_like((B, 32, 4, 4), torch.uint8)
+    a1, idx1 = nan(B, 16, 12, 12), nan(B, 16, 12, 12, dtype=torch.uint8)
+    a2, idx2 = nan(B, 32, 4, 4), nan(B, 32, 4, 4, dtype=torch.uint8)
     nat.cnn_fwd(x, w0, b0, w1, b1, a1, idx1, a2, idx2)
     torch.cuda.synchronize()
     ps = [t.double().requires_grad_(True) for t in (w0, b0, w1, b1)]
@@ -340,13 +160,13 @@ def test_cnn_direct_kernels_at_edges(nat, B, data, regime):
     torch.cuda.synchronize()
     check_acc("dw0", dw0, s_dw0, 2); check_acc("db0", db0, s_db0, 2)
     if B % 2 == 0 and B <= 64:
-        dw1, db1 = nan_like((32, 16, 5, 5)), nan_like((32,))
+        dw1, db1 = nan(32, 16, 5, 5), nan(32)
         for _ in range(2):
             assert nat.cnn_wgrad1(a1, a2, idx2, da2, dw1, db1)
         torch.cuda.synchronize()
         check_over("dw1", dw1); check_over("db1", db1)
         dw0, db0 = s_dw0.clone(), s_db0.clone()
-        dw1, db1 = nan_like((32, 16, 5, 5)), nan_like((32,))
+        dw1, db1 = nan(32, 16, 5, 5), nan(32)
         for _ in range(2):
             nat.cnn_bwd_all(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1)
         torch.cuda.synchronize()
@@ -365,7 +185,7 @@ def test_cnn_direct_batch_refusals(nat, B):
     x, w1 = t(B, 1, 28, 28), t(32, 16, 5, 5)
     a1, idx1, a2, idx2 = t(B, 16, 12, 12), t(B, 16, 12, 12, dt=torch.uint8), t(B, 32, 4, 4), t(B, 32, 4, 4, dt=torch.uint8)
     da2, dw0, db0 = t(B, 32, 4, 4), t(16, 1, 5, 5), t(16)
-    dw1, db1 = nan_like((32, 16, 5, 5)), nan_like((32,))
+    dw1, db1 = nan(32, 16, 5, 5), nan(32)
     assert nat.cnn_wgrad1(a1, a2, idx2, da2, dw1, db1) is False
     with pytest.raises(RuntimeError):
         nat.cnn_bwd_all(x, w1, a1, idx1, a2, idx2, da2, dw0, db0, dw1, db1)
@@ -381,7 +201,7 @@ def test_conv_relu_pool_im2col_fwd(nat, B, data):
     g = torch.Generator().manual_seed(40 + B)
     x = images(g, B, data)
     w0, b0, _, _ = conv_params(g, "posbias" if data == "patch" else "default")
-    y, idx, col = nan_like((B, 16, 12, 12)), nan_like((B, 16, 12, 12), torch.uint8), nan_like((B * 64, 400))
+    y, idx, col = nan(B, 16, 12, 12), nan(B, 16, 12, 12, dtype=torch.uint8), nan(B * 64, 400)
     nat.conv_relu_pool_im2col_fwd(x, w0, b0, y, idx, col, 5, 5)
     torch.cuda.synchronize()
     xd, w0d, b0d = x.double(), w0.double(), b0.double()
@@ -399,7 +219,7 @@ def test_conv_relu_pool_wgrad_col2im(nat, B):
     g = torch.Generator().manual_seed(50 + B)
     x = images(g, B, "rand")
     w0, b0, _, _ = conv_params(g)
-    y, idx, col = nan_like((B, 16, 12, 12)), nan_like((B, 16, 12, 12), torch.uint8), nan_like((B * 64, 400))
+    y, idx, col = nan(B, 16, 12, 12), nan(B, 16, 12, 12, dtype=torch.uint8), nan(B * 64, 400)
     nat.conv_relu_pool_im2col_fwd(x, w0, b0, y, idx, col, 5, 5)
     dcol = torch.randn(B * 64, 400, generator=g).to(dev())
     da1 = F.fold(dcol.double().reshape(B, 64, 400).transpose(1, 2), (12, 12), 5)
@@ -424,7 +244,7 @@ def test_pool_relu_bwd_rows(nat, B):
     dp = torch.randn(B, 32, 4, 4, generator=g).to(dev())
     pooled = torch.relu(torch.randn(B, 32, 4, 4, generator=g)).to(dev())
     idx = torch.randint(0, 4, (B, 32, 4, 4), generator=g).to(torch.uint8).to(dev())
-    rows = nan_like((B * 64, 32))
+    rows = nan(B * 64, 32)
     s_db = torch.randn(32, generator=g).to(dev())
     db = s_db.clone()
     nat.pool_relu_bwd_rows(dp, pooled, idx, rows, db)
@@ -455,7 +275,7 @@ def test_head_fwd_bwd(nat, B, C):
     W = (torch.randn(C, K, generator=g) * 0.1).to(dev())
     bias = (torch.randn(C, generator=g) * 0.1).to(dev())
     label = torch.randint(0, C, (B,), generator=g).float().to(dev())
-    outs = [nan_like((B,)), nan_like((B, C)), nan_like((C, K)), nan_like((C,)), nan_like((B, K)), nan_like((K,))]
+    outs = [nan(B), nan(B, C), nan(C, K), nan(C), nan(B, K), nan(K)]
     nat.head_fwd_bwd(a, W, bias, label, *outs, True)
     torch.cuda.synchronize()
     refs = head_reference(a, W, bias, label)
@@ -468,7 +288,7 @@ def test_head_fwd_bwd_refusals(nat):
     """More than 32 classes (one warp holds a row's logits) and K not a multiple of 4 (128-bit staging loads) are refused."""
     for B, K, C in ((4, 128, 33), (4, 126, 10)):
         a, W, bias = torch.rand(B, K, device=dev()), torch.rand(C, K, device=dev()), torch.rand(C, device=dev())
-        outs = [nan_like((B,)), nan_like((B, C)), nan_like((C, K)), nan_like((C,)), nan_like((B, K)), nan_like((K,))]
+        outs = [nan(B), nan(B, C), nan(C, K), nan(C), nan(B, K), nan(K)]
         with pytest.raises(RuntimeError):
             nat.head_fwd_bwd(a, W, bias, torch.zeros(B, device=dev()), *outs, True)
 
@@ -513,7 +333,7 @@ def test_confident_loss(nat, kernel):
     g = torch.Generator().manual_seed(90)
     z, label, margin = confident_logits(g, B, C)
     lab = label.to(dev())
-    loss = nan_like((B,))
+    loss = nan(B)
     if kernel == "softmax_ce_fwd":
         logits = z.to(dev())
         nat.softmax_ce_fwd(logits, lab, loss)
@@ -522,16 +342,16 @@ def test_confident_loss(nat, kernel):
         K = 12
         a = torch.zeros(B, K, device=dev()); a[:, :C] = z.to(dev())
         W = torch.zeros(C, K, device=dev()); W[:, :C] = torch.eye(C, device=dev())
-        logits = nan_like((B, C))
-        nat.head_fwd_bwd(a, W, torch.zeros(C, device=dev()), lab, loss, logits, nan_like((C, K)), nan_like((C,)), nan_like((B, K)),
-                         nan_like((K,)), True)
+        logits = nan(B, C)
+        nat.head_fwd_bwd(a, W, torch.zeros(C, device=dev()), lab, loss, logits, nan(C, K), nan(C), nan(B, K),
+                         nan(K), True)
     else:
         # identity weights pass x[:, :10] (shifted to positive, so the ReLUs are transparent) through both hidden layers to the logits
         x = torch.zeros(B, 512, device=dev()); x[:, :C] = (z + 40).to(dev())
         eye = lambda n, k: torch.eye(n, k, device=dev())
         w = [eye(256, 512), torch.zeros(256, device=dev()), eye(128, 256), torch.zeros(128, device=dev()), eye(C, 128), torch.zeros(C, device=dev())]
-        logits = nan_like((B, C))
-        gr = [nan_like((256, 512)), nan_like((256,)), nan_like((128, 256)), nan_like((128,)), nan_like((C, 128)), nan_like((C,)), nan_like((B, 512))]
+        logits = nan(B, C)
+        gr = [nan(256, 512), nan(256), nan(128, 256), nan(128), nan(C, 128), nan(C), nan(B, 512)]
         assert nat.mlp_chain(x, *w, lab, loss, logits, *gr)
     torch.cuda.synchronize()
     exact = F.cross_entropy(logits.double(), lab.long(), reduction="none")
