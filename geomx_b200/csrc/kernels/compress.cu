@@ -4,8 +4,8 @@
 //   2bit  : src/kvstore/gradient_compression-inl.h:40-139 — one thread per 16-value word, byte-wise bit twiddling.
 //           Here: one thread packs 16 values from four 128-bit loads, identical bit layout.
 //   BSC   : src/kvstore/gradient_compression.cc:191-336 — single-threaded CPU lambdas (shuffle + heap + linear scans).
-//           Here: one CTA per tensor does momentum correction, sampled-threshold selection (bit-wise binary search for the
-//           k-th largest sample in smem) and *index-ordered* stream compaction with a block-wide scan, all in one launch;
+//           Here: one CTA per tensor does momentum correction, sampled-threshold selection (radix select of the k-th
+//           largest sample) and *index-ordered* stream compaction with a block-wide scan, all in one launch;
 //           several tensors are batched as blockIdx.x.
 //   fp8   : new on H100 — e4m3 payload + fp32 scale per 128 values, error feedback in `residual`.
 //   DGT   : 3rdparty/ps-lite/include/ps/kv_app.h:853-876 EvalMsgContribution — EMA of mean |g| per 4096-byte block.
@@ -101,9 +101,8 @@ __global__ void __launch_bounds__(BSC_THREADS, 1) bsc_kernel(const BscSeg* __res
   gx::pdl_launch();
   const BscSeg sg = segs[blockIdx.x];
   __shared__ int s_warp[33];
-  __shared__ float s_boundary;
-  __shared__ int s_cnt;
-  extern __shared__ float s_sample[];
+  __shared__ int s_hist[256];
+  __shared__ int s_sel[2];
   const long long n = sg.n;
   const float* src = MODE == 0 ? sg.v : sg.grad;
   float boundary = 0.f;
@@ -115,27 +114,30 @@ __global__ void __launch_bounds__(BSC_THREADS, 1) bsc_kernel(const BscSeg* __res
       sg.v[i] += u;
     }
     __syncthreads();
-    // 2) boundary = k_sample-th largest |v| over a strided sample (bit-wise binary search on the float pattern)
+    // 2) boundary = k_sample-th largest |v| over a strided sample: 8-bit radix select on the bit patterns of |v| (which order like the
+    //    values), four passes over the sample in global memory, so any sample size fits
     const int S = sg.sample;
     const long long stride = n / S > 0 ? n / S : 1;
-    for (int j = threadIdx.x; j < S; j += BSC_THREADS) s_sample[j] = fabsf(sg.v[(long long)j * stride]);
-    __syncthreads();
-    uint32_t lo = 0;  // largest bit pattern t with count(sample >= t) >= k_sample
-    for (int bit = 30; bit >= 0; --bit) {
-      const uint32_t cand = lo | (1u << bit);
-      if (threadIdx.x == 0) s_cnt = 0;
+    uint32_t prefix = 0, mask = 0;
+    int remaining = sg.k_sample < S ? sg.k_sample : S;  // k_sample > sample: the smallest sampled |v|, as the reference's heap gives
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      if (threadIdx.x < 256) s_hist[threadIdx.x] = 0;
       __syncthreads();
-      int c = 0;
-      for (int j = threadIdx.x; j < S; j += BSC_THREADS) c += (__float_as_uint(s_sample[j]) >= cand) ? 1 : 0;
-      c = (int)warp_sum((float)c);
-      if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_cnt, c);
+      for (int j = threadIdx.x; j < S; j += BSC_THREADS) {
+        const uint32_t key = __float_as_uint(sg.v[(long long)j * stride]) & 0x7fffffffu;
+        if ((key & mask) == prefix) atomicAdd(&s_hist[(key >> shift) & 255u], 1);
+      }
       __syncthreads();
-      if (s_cnt >= sg.k_sample) lo = cand;
+      const int h = threadIdx.x < 256 ? s_hist[255 - threadIdx.x] : 0;  // thread i owns bin 255-i: the scan counts the keys in higher bins
+      int total;
+      const int above = block_exclusive_scan(h, &total, s_warp);
+      if (threadIdx.x < 256 && above < remaining && above + h >= remaining) { s_sel[0] = 255 - (int)threadIdx.x; s_sel[1] = remaining - above; }
       __syncthreads();
+      prefix |= (uint32_t)s_sel[0] << shift;
+      mask |= 255u << shift;
+      remaining = s_sel[1];
     }
-    if (threadIdx.x == 0) s_boundary = __uint_as_float(lo);
-    __syncthreads();
-    boundary = s_boundary;
+    boundary = __uint_as_float(prefix);
   }
   // 3) index-ordered compaction, at most k entries
   const int k = sg.k;
@@ -255,16 +257,14 @@ GX_API int gx_dequantize_2bit(const void* in, float* out, long long n, float thr
   launch_pdl(dequantize_2bit_kernel, dim3(cgrid(n)), dim3(256), 0, s, reinterpret_cast<const uint32_t*>(in), out, n, thr, accumulate);
   return GX_CHECK_LAUNCH();
 }
-// segs: device array of BscSeg (see struct above), one CTA each.  max_sample: largest `sample` among them (smem sizing).
-GX_API int gx_bsc_compress_batch(const void* segs, int num_segs, int max_sample, float momentum, cudaStream_t s) {
-  if (max_sample > 48 * 1024) return -1;
-  const size_t smem = (size_t)max_sample * sizeof(float);
-  static bool set = false;
-  if (!set) { cudaFuncSetAttribute(bsc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 192 * 1024); set = true; }
-  launch_pdl(bsc_kernel<0>, dim3(num_segs), dim3(BSC_THREADS), smem, s, reinterpret_cast<const BscSeg*>(segs), momentum);
+// segs: device array of BscSeg (see struct above), one CTA each.
+GX_API int gx_bsc_compress_batch(const void* segs, int num_segs, float momentum, cudaStream_t s) {
+  if (num_segs == 0) return 0;
+  launch_pdl(bsc_kernel<0>, dim3(num_segs), dim3(BSC_THREADS), 0, s, reinterpret_cast<const BscSeg*>(segs), momentum);
   return GX_CHECK_LAUNCH();
 }
 GX_API int gx_bsc_pull_compress_batch(const void* segs, int num_segs, cudaStream_t s) {
+  if (num_segs == 0) return 0;
   launch_pdl(bsc_kernel<1>, dim3(num_segs), dim3(BSC_THREADS), 0, s, reinterpret_cast<const BscSeg*>(segs), 0.f);
   return GX_CHECK_LAUNCH();
 }
@@ -275,6 +275,7 @@ GX_API int gx_bsc_decompress(const float* zipped, float* out, long long n, int k
 }
 GX_API int gx_fp8_block_quantize(const float* x, float* residual, void* q, float* scale, long long n, cudaStream_t s) {
   const long long nb = (n + 127) / 128;
+  if (nb == 0) return 0;
   launch_pdl(fp8_block_quantize_kernel, dim3((unsigned)nb), dim3(128), 0, s, x, residual, reinterpret_cast<uint8_t*>(q), scale, n);
   return GX_CHECK_LAUNCH();
 }
@@ -284,6 +285,7 @@ GX_API int gx_fp8_block_dequantize(const void* q, const float* scale, float* out
 }
 GX_API int gx_dgt_contrib(const float* g, float* contrib, long long n, int block_elems, float alpha, int first, cudaStream_t s) {
   const long long nb = (n + block_elems - 1) / block_elems;
+  if (nb == 0) return 0;
   launch_pdl(dgt_contrib_kernel, dim3((unsigned)nb), dim3(256), 0, s, g, contrib, n, block_elems, alpha, first);
   return GX_CHECK_LAUNCH();
 }

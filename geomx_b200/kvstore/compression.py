@@ -34,8 +34,26 @@ __all__ = ["GradientCompression", "quantize_2bit", "dequantize_2bit", "bsc_compr
 BSC_PAD_VAL = -65530.0
 BSC_PAD_IDX = -1.0
 BSC_MOMENTUM = 0.9
+BSC_MAX_N = 1 << 24       # indices travel as float32, which holds every integer exactly only up to 2^24
 _POS = (0xC0, 0x30, 0x0C, 0x03)
 _NEG = (0x80, 0x20, 0x08, 0x02)
+
+
+def _flat(t):
+    """A read-only input as a contiguous float32 vector (fp16 / bf16 gradients are cast, as the reference's scripts cast them)."""
+    return t.reshape(-1).float().contiguous()
+
+
+def _state(t, what):
+    """A tensor the codec updates or fills in place: flattening a non-contiguous one would copy it, and the update would be lost."""
+    if t is not None and not t.is_contiguous():
+        raise MXNetError("%s must be contiguous" % what)
+
+
+def _bsc_check(n):
+    if n > BSC_MAX_N:
+        raise MXNetError("Bi-Sparse compression supports at most 2^24 = %d elements per tensor (indices are sent as float32), got %d"
+                         % (BSC_MAX_N, n))
 
 
 def _use_native(t):
@@ -56,12 +74,13 @@ def compressed_size_2bit(n: int) -> int:
 def quantize_2bit(grad: torch.Tensor, residual: torch.Tensor, threshold: float) -> torch.Tensor:
     """Returns ``ceil(N/16)`` packed words stored as float32 (the reference ships them as a float array)."""
     n = grad.numel()
+    _state(residual, "residual")
     if _use_native(grad):
         from ..ops import native
         out = torch.empty(compressed_size_2bit(n), dtype=torch.float32, device=grad.device)
-        native.quantize_2bit(grad.reshape(-1), residual.reshape(-1), out, float(threshold))
+        native.quantize_2bit(_flat(grad), residual.reshape(-1), out, float(threshold))
         return out
-    g = grad.reshape(-1).float(); r = residual.reshape(-1)
+    g = _flat(grad); r = residual.reshape(-1)
     r.add_(g)
     pos = r >= threshold
     neg = (r <= -threshold) & ~pos
@@ -78,6 +97,7 @@ def quantize_2bit(grad: torch.Tensor, residual: torch.Tensor, threshold: float) 
 def dequantize_2bit(packed: torch.Tensor, n: int, threshold: float, out: torch.Tensor | None = None) -> torch.Tensor:
     if out is None:
         out = torch.empty(n, dtype=torch.float32, device=packed.device)
+    _state(out, "out")
     if _use_native(packed):
         from ..ops import native
         native.dequantize_2bit(packed, out.reshape(-1), float(threshold))
@@ -99,7 +119,7 @@ def bsc_sizes(n: int, threshold: float):
     k = int(float(n) * threshold)
     sample = int(n * 0.005) if n * 0.005 * threshold >= 10 else int(10 / threshold)
     sample = max(1, min(sample, n))
-    k_sample = max(1, int(sample * threshold))
+    k_sample = min(sample, max(1, int(sample * threshold)))
     return k, sample, k_sample
 
 
@@ -115,17 +135,19 @@ def bsc_compress(grad: torch.Tensor, u: torch.Tensor, v: torch.Tensor, threshold
                  out: torch.Tensor | None = None) -> torch.Tensor:
     """Momentum-corrected sampled-threshold sparsifier.  Returns ``[vals(k) ‖ idx(k)]`` float32 (size 2k)."""
     n = grad.numel()
+    _bsc_check(n)
+    _state(u, "u"); _state(v, "v"); _state(out, "out")
     k, sample, k_sample = bsc_sizes(n, threshold)
     if out is None:
         out = torch.empty(2 * k, dtype=torch.float32, device=grad.device)
+    g = _flat(grad); u = u.reshape(-1); v = v.reshape(-1)
     if k == 0:
-        u.mul_(BSC_MOMENTUM).add_(grad.reshape(-1)); v.add_(u)
+        u.mul_(BSC_MOMENTUM).add_(g); v.add_(u)
         return out
     if _use_native(grad):
         from ..ops import native
-        native.bsc_compress(grad.reshape(-1), u.reshape(-1), v.reshape(-1), out, k, sample, k_sample, BSC_MOMENTUM)
+        native.bsc_compress(g, u, v, out, k, sample, k_sample, BSC_MOMENTUM)
         return out
-    g = grad.reshape(-1).float(); u = u.reshape(-1); v = v.reshape(-1)
     u.mul_(BSC_MOMENTUM).add_(g)
     v.add_(u)
     va = v.abs()
@@ -143,16 +165,18 @@ def bsc_compress(grad: torch.Tensor, u: torch.Tensor, v: torch.Tensor, threshold
 
 def bsc_pull_compress(dense: torch.Tensor, threshold: float, multiplier: int, out: torch.Tensor | None = None) -> torch.Tensor:
     n = dense.numel()
+    _bsc_check(n)
+    _state(out, "out")
     k = int(float(n) * threshold * multiplier)
     if out is None:
         out = torch.empty(2 * k, dtype=torch.float32, device=dense.device)
     if k == 0:
         return out
+    d = _flat(dense)
     if _use_native(dense):
         from ..ops import native
-        native.bsc_pull_compress(dense.reshape(-1), out, k)
+        native.bsc_pull_compress(d, out, k)
         return out
-    d = dense.reshape(-1).float()
     idx = torch.nonzero(d != 0).reshape(-1)[:k]
     m = idx.numel()
     out[:k] = BSC_PAD_VAL
@@ -167,6 +191,7 @@ def bsc_decompress(zipped: torch.Tensor, n: int, out: torch.Tensor | None = None
     if out is None:
         out = torch.zeros(n, dtype=torch.float32, device=zipped.device)
         accumulate = True
+    _state(out, "out")
     if _use_native(zipped):
         from ..ops import native
         native.bsc_decompress(zipped, out.reshape(-1), accumulate)
@@ -196,13 +221,14 @@ def fp8_block_quantize(x: torch.Tensor, residual: torch.Tensor | None = None):
     """x (+ residual) → (e4m3 payload uint8[N_pad], fp32 scales[N_pad/128]); residual receives the rounding error."""
     n = x.numel()
     nb = (n + FP8_BLOCK - 1) // FP8_BLOCK
+    _state(residual, "residual")
     if _use_native(x):
         from ..ops import native
         q = torch.empty(nb * FP8_BLOCK, dtype=torch.uint8, device=x.device)
         s = torch.empty(nb, dtype=torch.float32, device=x.device)
-        native.fp8_block_quantize(x.reshape(-1), residual.reshape(-1) if residual is not None else None, q, s)
+        native.fp8_block_quantize(_flat(x), residual.reshape(-1) if residual is not None else None, q, s)
         return q, s
-    xf = x.reshape(-1).float()
+    xf = _flat(x)
     if residual is not None:
         xf = xf + residual.reshape(-1)
     pad = nb * FP8_BLOCK - n
@@ -220,6 +246,7 @@ def fp8_block_quantize(x: torch.Tensor, residual: torch.Tensor | None = None):
 def fp8_block_dequantize(q: torch.Tensor, scale: torch.Tensor, n: int, out: torch.Tensor | None = None) -> torch.Tensor:
     if out is None:
         out = torch.empty(n, dtype=torch.float32, device=q.device)
+    _state(out, "out")
     if _use_native(q):
         from ..ops import native
         native.fp8_block_dequantize(q, scale, out.reshape(-1))

@@ -675,19 +675,23 @@ def bsc_segment(grad, u, v, out, k, sample, k_sample):
                    out.data_ptr(), (grad if grad is not None else v).numel(), k, sample, k_sample)
 
 
-def bsc_compress_batch(seg_table_dev, num, max_sample, momentum=0.9):
-    _ck(_lib().gx_bsc_compress_batch(_p(seg_table_dev), num, max_sample, momentum, _s()), "bsc_compress")
+def bsc_compress_batch(seg_table_dev, num, momentum=0.9):
+    _ck(_lib().gx_bsc_compress_batch(_p(seg_table_dev), num, momentum, _s()), "bsc_compress")
+
+
+def bsc_pull_compress_batch(seg_table_dev, num):
+    _ck(_lib().gx_bsc_pull_compress_batch(_p(seg_table_dev), num, _s()), "bsc_pull_compress")
 
 
 def bsc_compress(grad, u, v, out, k, sample, k_sample, momentum=0.9):
     tab = _segs_to_dev([bsc_segment(_f32c(grad), u, v, out, k, sample, k_sample)], grad.device)
-    bsc_compress_batch(tab, 1, sample, momentum)
+    bsc_compress_batch(tab, 1, momentum)
     return out
 
 
 def bsc_pull_compress(dense, out, k):
-    tab = _segs_to_dev([_BscSeg(dense.data_ptr(), 0, 0, out.data_ptr(), dense.numel(), k, 0, 0)], dense.device)
-    _ck(_lib().gx_bsc_pull_compress_batch(_p(tab), 1, _s()), "bsc_pull_compress")
+    tab = _segs_to_dev([bsc_segment(_f32c(dense), None, None, out, k, 0, 0)], dense.device)
+    bsc_pull_compress_batch(tab, 1)
     return out
 
 

@@ -60,7 +60,7 @@ SIGS = {
     # compress.cu
     "gx_quantize_2bit": [P, P, P, L, F, P],
     "gx_dequantize_2bit": [P, P, L, F, I, P],
-    "gx_bsc_compress_batch": [P, I, I, F, P],
+    "gx_bsc_compress_batch": [P, I, F, P],
     "gx_bsc_pull_compress_batch": [P, I, P],
     "gx_bsc_decompress": [P, P, L, I, I, P],
     "gx_fp8_block_quantize": [P, P, P, P, L, P],

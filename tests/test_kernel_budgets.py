@@ -42,6 +42,8 @@ BUDGETS = [
     ("optim", "", None, None, False),
     ("hips_fabric", "", None, None, False),
     ("cnn_direct", "", None, None, False),
+    # the gradient-compression kernels (bsc_kernel<0> at 1024 threads: at most 64 registers, enforced by its __launch_bounds__)
+    ("compress", "", None, None, False),
 ]
 
 

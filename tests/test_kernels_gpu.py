@@ -6,7 +6,6 @@ import pytest
 import torch
 
 import geomx_b200 as mx
-from geomx_b200.kvstore import compression as gc
 
 from _cnn_ref import dev, engine, nat, rel_err, step_reference  # noqa: F401  (nat, engine: fixtures)
 
@@ -244,50 +243,6 @@ def test_trainer_multi_tensor(nat):
         l.backward(); tr.step(32)
         vals.append(float(l.mean().asscalar()))
     assert vals[-1] < vals[0] * 0.7, vals      # memorising 32 random labels: the loss must fall clearly (the pace depends on the init draw)
-
-
-# ---------------------------------------------------------------------------------------------------------------- compression
-def test_2bit_matches_cpu_oracle(nat):
-    torch.manual_seed(12)
-    g = torch.randn(1000) * 0.6; r_cpu = torch.zeros(1000); r_gpu = torch.zeros(1000, device=dev())
-    for _ in range(3):
-        q_cpu = gc.quantize_2bit(g, r_cpu, 0.5)
-        q_gpu = gc.quantize_2bit(g.to(dev()), r_gpu, 0.5)
-        assert torch.equal(q_cpu.view(torch.int32), q_gpu.cpu().view(torch.int32))
-        assert torch.allclose(r_cpu, r_gpu.cpu())
-    d = gc.dequantize_2bit(q_gpu, 1000, 0.5)
-    assert torch.equal(d.cpu(), gc.dequantize_2bit(q_cpu, 1000, 0.5))
-
-
-def test_bsc_contract(nat):
-    torch.manual_seed(13)
-    n, thr = 131072, 0.01
-    g = torch.randn(n)
-    u_c, v_c = torch.zeros(n), torch.zeros(n)
-    u_g, v_g = torch.zeros(n, device=dev()), torch.zeros(n, device=dev())
-    for _ in range(2):
-        z_c = gc.bsc_compress(g, u_c, v_c, thr)
-        z_g = gc.bsc_compress(g.to(dev()), u_g, v_g, thr)
-        assert torch.allclose(z_c, z_g.cpu(), atol=1e-5), "GPU BSC differs from the CPU oracle"
-        assert torch.allclose(v_c, v_g.cpu(), atol=1e-5) and torch.allclose(u_c, u_g.cpu(), atol=1e-5)
-    k = z_g.numel() // 2
-    dense = gc.bsc_decompress(z_g, n)
-    assert int((dense != 0).sum()) <= k
-    z2 = gc.bsc_pull_compress(dense, thr, 2)
-    assert torch.allclose(gc.bsc_decompress(z2, n), dense)
-    assert torch.allclose(z2.cpu(), gc.bsc_pull_compress(dense.cpu(), thr, 2))
-
-
-def test_fp8_block_roundtrip(nat):
-    torch.manual_seed(14)
-    x = torch.randn(1000, device=dev()) * 3
-    res = torch.zeros(1000, device=dev())
-    q, s = gc.fp8_block_quantize(x, res)
-    y = gc.fp8_block_dequantize(q, s, 1000)
-    assert rel_err(y, x) < 0.05
-    assert torch.allclose(y + res, x, atol=1e-5)      # error feedback holds the exact remainder
-    qc, sc = gc.fp8_block_quantize(x.cpu(), torch.zeros(1000))
-    assert torch.allclose(gc.fp8_block_dequantize(qc, sc, 1000), y.cpu(), atol=1e-6)
 
 
 # ---------------------------------------------------------------------------------------------------------------- flagship step

@@ -93,6 +93,36 @@ def test_2bit_bit_layout_and_residual():
     assert gc.compressed_size_2bit(17) == 2 and gc.compressed_size_2bit(16) == 1
 
 
+def test_compress_reference_self_check():
+    """tests/_compress_ref.py, the GPU codec tests' reference: its 2-bit packer gives the bytes above, its e4m3 table is torch's for every
+    finite code, its rounding is torch's (nearest, ties to even) on values between the codes, and its fp32 FMA rounds once."""
+    import _compress_ref as CR
+    g = np.zeros(16, np.float32); g[0] = 1.0; g[1] = -1.0; g[5] = 0.7; g[15] = -0.2
+    words, r = CR.quantize_2bit(g, np.zeros(16, np.float32), 0.5)
+    assert words.view(np.uint8).tolist()[:4] == [0xC0 | 0x20, 0x30, 0, 0]
+    assert r.tolist() == np.array([0.5, -0.5, 0, 0, 0, np.float32(0.7) - np.float32(0.5)] + [0] * 9 + [-0.2], np.float32).tolist()
+    assert CR.dequantize_2bit(words, 16, 0.5).tolist() == [0.5, -0.5, 0, 0, 0, 0.5] + [0.0] * 10
+    for n in (1, 17, 1000):
+        x = (torch.randn(n) * 0.6).numpy()
+        rt = torch.zeros(n)
+        q = gc.quantize_2bit(torch.from_numpy(x), rt, 0.1)
+        w, rr = CR.quantize_2bit(x, np.zeros(n, np.float32), 0.1)
+        assert np.array_equal(q.view(torch.int32).numpy().view(np.uint32), w) and np.array_equal(rt.numpy(), rr)
+    table = CR.e4m3_table()
+    codes = torch.arange(256, dtype=torch.uint8)
+    finite = (codes & 0x7F) != 0x7F
+    assert np.array_equal(table[finite.numpy()], codes[finite].view(torch.float8_e4m3fn).double().numpy())
+    assert np.isnan(table[~finite.numpy()]).all()
+    mags = table[:127]
+    mids = ((mags[:-1] + mags[1:]) / 2).astype(np.float32)            # exact ties between neighbouring codes
+    x = np.concatenate([mids, -mids, np.nextafter(mids, 0), np.nextafter(mids, 1000), np.float32([0, -0.0, 448, 460, 1e-9, 2.0 ** -10, 3 * 2.0 ** -11]),
+                        (np.random.RandomState(0).randn(5000) * 50).astype(np.float32)]).astype(np.float32)
+    assert np.array_equal(CR.to_e4m3(x), torch.from_numpy(x).to(torch.float8_e4m3fn).view(torch.uint8).numpy())
+    assert CR.to_e4m3(np.float32([1e6, -1e6])).tolist() == [0x7E, 0xFE]     # saturates (torch's cast gives NaN there)
+    a, b, c = np.float32([1 + 2.0 ** -23]), np.float32([1 - 2.0 ** -23]), np.float32([-1.0])
+    assert CR.fma32(a, b, c)[0] == np.float32(-2.0 ** -46)                # one rounding; two roundings would give 0
+
+
 @needs_c
 def test_2bit_native_matches_python():
     C = runtime.C()
@@ -131,6 +161,34 @@ def test_bsc_contract():
     # pull side: capacity k * parties, non-zeros in index order
     z2 = gc.bsc_pull_compress(dense, thr, 2)
     assert z2.numel() == 2 * int(n * thr * 2) and torch.allclose(gc.bsc_decompress(z2, n), dense)
+
+
+def test_bsc_sizes_and_refusals():
+    """A threshold above 1 takes the smallest sampled |v| as the boundary (k_sample clamped to the sample, as the reference's heap does); more
+    than 2^24 elements, whose indices float32 cannot hold, is refused; state the codec updates in place must be contiguous."""
+    from geomx_b200.base import MXNetError
+    assert gc.bsc_sizes(1000, 2.0) == (2000, 5, 5)
+    g = torch.tensor([3.0, -1.0, 0.5, 2.0, -0.25]); u = torch.zeros(5); v = torch.zeros(5)
+    z = gc.bsc_compress(g, u, v, 2.0)                    # sample 5, k_sample 5 -> boundary = smallest |v| = 0.25: everything is sent
+    assert z[:5].tolist() == g.tolist() and z[5:10].tolist() == [-65530.0] * 5
+    assert z[10:15].tolist() == [0, 1, 2, 3, 4] and z[15:].tolist() == [-1.0] * 5
+    big = torch.zeros(1)
+    big_n = (1 << 24) + 1
+    with pytest.raises(MXNetError, match="2\\^24"):
+        gc.bsc_compress(big.expand(big_n), big.expand(big_n), big.expand(big_n), 0.01)
+    with pytest.raises(MXNetError, match="2\\^24"):
+        gc.bsc_pull_compress(big.expand(big_n), 0.01, 1)
+    g = torch.randn(64)
+    st = torch.zeros(64, 2)[:, 0]
+    for call in (lambda: gc.quantize_2bit(g, st, 0.5), lambda: gc.bsc_compress(g, st, torch.zeros(64), 0.5),
+                 lambda: gc.bsc_compress(g, torch.zeros(64), st, 0.5), lambda: gc.fp8_block_quantize(g, st),
+                 lambda: gc.dequantize_2bit(gc.quantize_2bit(g, torch.zeros(64), 0.5), 64, 0.5, out=st),
+                 lambda: gc.bsc_decompress(torch.zeros(4), 64, out=st), lambda: gc.fp8_block_dequantize(*gc.fp8_block_quantize(g), 64, out=st)):
+        with pytest.raises(MXNetError, match="contiguous"):
+            call()
+    assert torch.count_nonzero(st) == 0
+    r16, r32 = torch.zeros(64), torch.zeros(64)            # an fp16 gradient is cast, as the CUDA path does
+    assert torch.equal(gc.quantize_2bit(g.half(), r16, 0.5), gc.quantize_2bit(g.half().float(), r32, 0.5)) and torch.equal(r16, r32)
 
 
 @needs_c
