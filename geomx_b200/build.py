@@ -99,7 +99,7 @@ def build_runtime(force=False, verbose=False):
     if jobs or not os.path.exists(out):
         # link the SHARED libstdc++ explicitly: some toolchains (e.g. a relocated g++ that only ships libstdc++.a) would otherwise embed a
         # second, static copy next to the one torch already loaded — two iostream/locale runtimes in one process crash on first use
-        _run([CXX, "-shared", "-o", out] + objs + ["-pthread", "-l:libstdc++.so.6"] + (["-fsanitize=" + _SAN] if _SAN else []))
+        _run([CXX, "-shared", "-o", out] + objs + ["-pthread", "-l:libstdc++.so.6", "-ldl"] + (["-fsanitize=" + _SAN] if _SAN else []))
     return out
 
 
@@ -130,7 +130,8 @@ def build_capi(force=False, verbose=False):
             if verbose and o.strip():
                 print(o)
     if jobs or not os.path.exists(out):
-        _run([CXX, "-shared", "-o", out] + objs + ["-pthread", "-l:libstdc++.so.6", "-Wl,--no-undefined"] + (["-fsanitize=" + _SAN] if _SAN else []))
+        # no CUDA here: the device predictor (runtime/predict_device.h) dlopens libgeomx_kernels.so when dev_type 2 is asked for
+        _run([CXX, "-shared", "-o", out] + objs + ["-pthread", "-l:libstdc++.so.6", "-ldl", "-Wl,--no-undefined"] + (["-fsanitize=" + _SAN] if _SAN else []))
     return out
 
 

@@ -22,6 +22,8 @@
 // fp32 = one 128-byte swizzle atom per row.  Out-of-bounds rows/cols/k are zero-filled by TMA, masked in the epilogue.
 #include <cuda.h>
 
+#include <atomic>
+
 #include "common.cuh"
 
 namespace gx {
@@ -418,12 +420,16 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, di
   if (env_stages > 0 && env_stages < stages) stages = env_stages;
   if (stages < 1) stages = 1;
   p.stages = stages;
-  static bool attr_set = false;
+  // the dynamic shared-memory limit is an attribute of the function in each device's context: set once per device, not once per process
+  static std::atomic<unsigned long long> attr_set{0};
   auto kern = gemm_tf32_kernel<BLOCK_N, A_MN, B_MN, SPLIT>;
-  if (!attr_set) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+  if (bit == 0 || !(attr_set.load(std::memory_order_acquire) & bit)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::bytes(L::STAGES));
     if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    attr_set.fetch_or(bit, std::memory_order_release);
   }
   launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), L::bytes(stages), stream, ta, tb, p);
   return (int)cudaGetLastError();
@@ -462,7 +468,7 @@ GX_API int gx_gemm_set_debug(unsigned long long* p) { g_gemm_dbg = p; return 0; 
 static int gemm_tf32_impl(const float* A, long long lda, int a_mn, const float* B, long long ldb, int b_mn, int M, int N, int K, float* D,
                           long long ldd, const float* bias, const float* mask, long long ldmask, float* colsum, int relu, int accumulate,
                           int store_mode, int hw, float alpha, int split_k,
-                          int pool_w, unsigned char* pool_idx, cudaStream_t stream) {
+                          int pool_w, unsigned char* pool_idx, int precision, cudaStream_t stream) {
   using namespace gx;
   if (relu && split_k > 1) return -2;
   if (M <= 0 || N <= 0) return 0;
@@ -513,7 +519,7 @@ static int gemm_tf32_impl(const float* A, long long lda, int a_mn, const float* 
   p.a_bytes = a_mn ? p.a_boxes * MN_BOX_BYTES : a_rows * BLOCK_K * 4;
   p.b_bytes = b_mn ? p.b_boxes * MN_BOX_BYTES : b_rows * BLOCK_K * 4;
   p.tx_bytes = p.a_bytes + p.b_bytes;
-  const bool split = gemm_precision() == 3;
+  const bool split = precision == 3;
   dim3 grid((unsigned)ceil_div(N, block_n), (unsigned)mt, (unsigned)split_k);
   switch (block_n) {
     case 16: return dispatch_major<16>(split, a_mn, b_mn, ta, tb, p, grid, stream);
@@ -527,7 +533,15 @@ GX_API int gx_gemm_tf32(const float* A, long long lda, int a_mn, const float* B,
                         long long ldd, const float* bias, const float* mask, long long ldmask, float* colsum, int relu, int accumulate,
                         int store_mode, int hw, float alpha, int split_k, cudaStream_t stream) {
   return gemm_tf32_impl(A, lda, a_mn, B, ldb, b_mn, M, N, K, D, ldd, bias, mask, ldmask, colsum, relu, accumulate, store_mode == 2 ? 1 : store_mode, hw,
-                        alpha, split_k, 0, nullptr, stream);
+                        alpha, split_k, 0, nullptr, gemm_precision(), stream);
+}
+// gx_gemm_tf32 at an explicit precision (3 = 3xTF32, 1 = TF32) that leaves the process-wide setting alone: for callers whose results must
+// not depend on it (the device predictor, predict_dev.cu)
+GX_API int gx_gemm_tf32_prec(const float* A, long long lda, int a_mn, const float* B, long long ldb, int b_mn, int M, int N, int K, float* D,
+                             long long ldd, const float* bias, const float* mask, long long ldmask, float* colsum, int relu, int accumulate,
+                             int store_mode, int hw, float alpha, int split_k, int precision, cudaStream_t stream) {
+  return gemm_tf32_impl(A, lda, a_mn, B, ldb, b_mn, M, N, K, D, ldd, bias, mask, ldmask, colsum, relu, accumulate, store_mode == 2 ? 1 : store_mode, hw,
+                        alpha, split_k, 0, nullptr, precision == 1 ? 1 : 3, stream);
 }
 // Convolution-as-GEMM with the 2x2/2 max-pool fused into the epilogue: rows of A are (image, oh, ow) with ow fastest and `hw` = OH*OW,
 // `pool_w` = OW.  D receives the POOLED NCHW map [images][N][OH/2][OW/2], `pool_idx` the arg-max position of every pooled element.
@@ -535,7 +549,7 @@ GX_API int gx_gemm_tf32(const float* A, long long lda, int a_mn, const float* B,
 GX_API int gx_gemm_tf32_pool(const float* A, long long lda, int a_mn, const float* B, long long ldb, int b_mn, int M, int N, int K, float* D,
                              const float* bias, int relu, int hw, int pool_w, unsigned char* pool_idx, float alpha, cudaStream_t stream) {
   return gemm_tf32_impl(A, lda, a_mn, B, ldb, b_mn, M, N, K, D, N, bias, nullptr, 0, nullptr, relu, 0, 2, hw, alpha, 1, pool_w,
-                        pool_idx, stream);
+                        pool_idx, gemm_precision(), stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -7,7 +7,8 @@
 // that symbol.py builds structurally + the elementwise family), its own memory planner (role of src/executor/graph_executor.cc
 // InitDataEntryMemory / nnvm PlanMemory).  Both graph dialects load: this framework's `geomx_b200-symbol-1` and the reference's nnvm JSON
 // (string-valued attrs, `[node, index, version]` input triples, BatchNorm statistics as inputs 3/4), so `-symbol.json` + `.params`
-// checkpoints written by either side can be served.  GPU inference is the Python Executor's job (device tensors belong to PyTorch).
+// checkpoints written by either side can be served.  The same plan also runs on an H100 (predict_device.h: the arena and the parameters in
+// device memory, the operators as sm_90a kernels); the Python Executor serves device tensors that belong to PyTorch.
 #pragma once
 #include <algorithm>
 #include <cctype>
@@ -274,6 +275,7 @@ struct Node {
 struct Storage {
   bool external = false;             // parameter / input buffer owned outside the arena
   int block = -1;
+  int64_t offset = 0;                // first float of the block in the arena
   int64_t size = 0;
   int ref = 0;
   float* ptr = nullptr;
@@ -282,7 +284,7 @@ struct Storage {
 class Predictor {
  public:
   Predictor(const std::string& json, const char* params, size_t param_size, const std::vector<std::string>& input_keys,
-            const std::vector<Shape>& input_shapes, const std::vector<std::string>& output_keys) {
+            const std::vector<Shape>& input_shapes, const std::vector<std::string>& output_keys, bool host_arena = true) : host_arena_(host_arena) {
     doc_ = std::make_shared<JValue>(JParser(json.data(), json.size()).Parse());
     BuildGraph(output_keys);
     LoadParams(params, param_size);
@@ -320,11 +322,14 @@ class Predictor {
     if (size != static_cast<size_t>(Numel(n.shape))) throw std::runtime_error("GetOutput: output " + std::to_string(i) + " has " + std::to_string(Numel(n.shape)) + " values, buffer holds " + std::to_string(size));
     memcpy(out, storages_[n.storage].ptr, size * sizeof(float));
   }
-  size_t ArenaBytes() const { return arena_.size() * sizeof(float); }
+  size_t ArenaBytes() const { return static_cast<size_t>(arena_floats_) * sizeof(float); }
   size_t NumOps() const { return order_.size(); }
 
  private:
+  friend class DevicePredictor;        // runs this plan on the GPU: reads the graph, the order and the storages
   Predictor(const Predictor&) = default;
+  bool host_arena_ = true;             // false: the arena lives on the device, only its size is planned here
+  int64_t arena_floats_ = 0;
   std::shared_ptr<JValue> doc_;
   std::vector<Node> nodes_;
   std::vector<Entry> heads_;
@@ -496,8 +501,9 @@ class Predictor {
     std::vector<int64_t> offset(block_size.size(), 0);
     int64_t total = 0;
     for (size_t b = 0; b < block_size.size(); ++b) { offset[b] = total; total += (block_size[b] + 15) / 16 * 16; }
-    arena_.assign(static_cast<size_t>(total), 0.f);
-    for (auto& s : storages_) if (!s.external) s.ptr = arena_.data() + offset[s.block];
+    arena_floats_ = total;
+    arena_.assign(host_arena_ ? static_cast<size_t>(total) : 0, 0.f);
+    for (auto& s : storages_) if (!s.external) { s.offset = offset[s.block]; s.ptr = host_arena_ ? arena_.data() + s.offset : nullptr; }
     for (auto& h : heads_) if (!nodes_[h.node].known) throw std::runtime_error("output " + nodes_[h.node].name + " has no shape");
   }
 

@@ -222,6 +222,7 @@ int GXStorageAlloc(size_t nbytes, void** out);
 int GXStorageFree(void* p);
 
 /* ---- predict API (include/mxnet/c_predict_api.h) --------------------------------------------------------------------------------------- */
+/* dev_type 1 runs the graph on the host; dev_type 2 on CUDA device dev_id (an H100, sm_90a), with the planned predictor's operators only. */
 int GXPredCreate(const char* symbol_json, const void* param_bytes, int param_size, int dev_type, int dev_id, uint32_t num_input_nodes, const char** input_keys,
                  const uint32_t* input_shape_indptr, const uint32_t* input_shape_data, PredictorHandle* out);
 int GXPredCreatePartialOut(const char* symbol_json, const void* param_bytes, int param_size, int dev_type, int dev_id, uint32_t num_input_nodes,
@@ -238,7 +239,8 @@ int GXPredForward(PredictorHandle handle);
 int GXPredPartialForward(PredictorHandle handle, int step, int* step_left);
 int GXPredGetOutput(PredictorHandle handle, uint32_t index, float* data, uint32_t size);
 int GXPredGetPlan(PredictorHandle handle, uint64_t* arena_bytes, uint32_t* num_ops);
-int GXPredGetEngine(PredictorHandle handle, int* out);        /* 1 planned predictor, 2 general executor (operators outside the planned set) */
+int GXPredGetEngine(PredictorHandle handle, int* out);        /* 1 planned predictor, 2 general executor (operators outside the planned set),
+                                                                 3 planned predictor on the GPU (dev_type 2) */
 int GXPredFree(PredictorHandle handle);
 int GXNDListCreate(const char* nd_file_bytes, int nd_file_size, NDListHandle* out, uint32_t* out_length);
 int GXNDListGet(NDListHandle handle, uint32_t index, const char** out_key, const float** out_data, const uint32_t** out_shape, uint32_t* out_ndim);
