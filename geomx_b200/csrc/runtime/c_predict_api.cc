@@ -4,8 +4,8 @@
 //   MXPredCreate :78, MXPredCreatePartialOut :111, MXPredCreateMultiThread :144, MXPredReshape :170, MXPredGetOutputShape :185,
 //   MXPredSetInput :198, MXPredForward :207, MXPredPartialForward :224, MXPredGetOutput :233, MXPredFree :242, MXNDList{Create,Get,Free} :252-277.
 // dev_type 1 (cpu) runs the plan on the host; dev_type 2 (gpu) runs the same plan on CUDA device dev_id (predict_device.h, sm_90a kernels
-// reached through dlopen, so this library links no CUDA).  A graph outside the planned operator set runs on the host's general executor,
-// and is refused on the device.
+// reached through dlopen, so this library links no CUDA).  A graph outside the planned operator set runs on the host's general executor;
+// on the device, the planner takes the general executor's other operators as well (predict_device.h, the device-only set).
 // Errors: -1 + GXRTGetLastError() (shared with c_api_runtime.cc, thread-local).
 #include <cstdint>
 #include <map>
@@ -181,7 +181,8 @@ void MakeHost(Handle* h, const char* json, const void* params, int param_size, u
     catch (const std::exception& e2) { throw std::runtime_error(msg + "; the general executor could not run the graph either: " + e2.what()); }
   }
 }
-// dev_type 2: the planned predictor on device dev_id.  Whatever stops it, the message names the ways that remain.
+// dev_type 2: the planned predictor, with the device-only operator set, on device dev_id.  Whatever stops it, the message names the ways
+// that remain.
 void MakeDevice(Handle* h, const char* json, const void* params, int param_size, int dev_id, uint32_t n_in, const char** keys,
                 const uint32_t* indptr, const uint32_t* shape_data, uint32_t n_out, const char** out_keys) {
   try {
@@ -194,10 +195,11 @@ void MakeDevice(Handle* h, const char* json, const void* params, int param_size,
     const auto shapes = Shapes(n_in, indptr, shape_data);
     std::unique_ptr<Predictor> plan;
     try {
-      plan = std::make_unique<Predictor>(std::string(json), static_cast<const char*>(params), static_cast<size_t>(param_size), ik, shapes, ok, false);
+      plan = std::make_unique<Predictor>(std::string(json), static_cast<const char*>(params), static_cast<size_t>(param_size), ik, shapes, ok, false,
+                                         gxrt::predict::extended::Ops());
     } catch (const std::runtime_error& e) {
       if (!Unsupported(e.what())) throw;
-      throw std::runtime_error(std::string(e.what()) + "; the device runs the planned predictor's operators only");
+      throw std::runtime_error(std::string(e.what()) + "; the device runs the operators of the planned predictor and of the general executor only");
     }
     h->dev = DevicePredictor::Create(std::move(plan), dev_id);
   } catch (const std::exception& e) {
@@ -286,7 +288,7 @@ GX_CAPI int GXPredGetOutput(void* handle, uint32_t index, float* data, uint32_t 
   return Guard([&] { Handle* h = H(handle); if (h->pred) h->pred->GetOutput(index, data, size); else if (h->dev) h->dev->GetOutput(index, data, size); else h->gen->GetOutput(index, data, size); });
 }
 // 1: the planned predictor (predict.h) runs this graph on the host, 2: the general executor (train_exec.h) does, 3: the planned predictor
-// runs it on a GPU (predict_device.h)
+// runs it on a GPU, with the general executor's other operators as device kernels (predict_device.h)
 GX_CAPI int GXPredGetEngine(void* handle, int* out) { return Guard([&] { Handle* h = H(handle); *out = h->pred ? 1 : h->dev ? 3 : 2; }); }
 // planner statistics: bytes of the activation arena and the number of operators that run
 GX_CAPI int GXPredGetPlan(void* handle, uint64_t* arena_bytes, uint32_t* num_ops) {

@@ -149,6 +149,7 @@ class Attrs {
  public:
   Attrs() = default;
   explicit Attrs(const JValue* o) : o_(o) {}
+  const JValue* Object() const { return o_; }
   const JValue* Raw(const std::string& k) const { const JValue* v = o_ ? o_->Find(k) : nullptr; return (v && v->kind != JValue::kNull && !(v->kind == JValue::kStr && v->str == "None")) ? v : nullptr; }
   bool Has(const std::string& k) const { return Raw(k) != nullptr; }
   double Float(const std::string& k, double def) const {
@@ -267,9 +268,15 @@ struct Node {
   Attrs attrs;
   std::vector<Entry> inputs;
   bool nnvm = false;                 // dialect: decides the defaults of absent attributes (Pooling stride, BatchNorm fix_gamma / eps)
-  Shape shape;                       // output 0 (every supported op has one visible output)
+  Shape shape;                       // output 0; every output of a multi-output node (SliceChannel) has this shape
   int storage = -1;
   bool known = false;                // shape inferred
+  // the device's operators beyond the planned set (predict_device.h): canonical operator name, the attributes in the general executor's
+  // string form, the output count and the storages of outputs 1..
+  bool extended = false;
+  std::map<std::string, std::string> sattrs;
+  int num_out = 1;
+  std::vector<int> more_storage;
 };
 
 struct Storage {
@@ -281,10 +288,20 @@ struct Storage {
   float* ptr = nullptr;
 };
 
+// The device-only operator set (predict_device.h), handed to the planner by the device predictor only: whether it has an operator the
+// planned set lacks, a node's output count from its attributes, and `infer`, which gives such a node its canonical name, string attributes,
+// output count and shape from its inputs' shapes.
+struct ExtendedOps {
+  bool (*has)(const std::string& op);
+  int (*num_outputs)(const Node& nd);
+  void (*infer)(Node& nd, const std::vector<const Node*>& in);
+};
+
 class Predictor {
  public:
   Predictor(const std::string& json, const char* params, size_t param_size, const std::vector<std::string>& input_keys,
-            const std::vector<Shape>& input_shapes, const std::vector<std::string>& output_keys, bool host_arena = true) : host_arena_(host_arena) {
+            const std::vector<Shape>& input_shapes, const std::vector<std::string>& output_keys, bool host_arena = true,
+            const ExtendedOps* extended = nullptr) : host_arena_(host_arena), extended_(extended) {
     doc_ = std::make_shared<JValue>(JParser(json.data(), json.size()).Parse());
     BuildGraph(output_keys);
     LoadParams(params, param_size);
@@ -320,7 +337,7 @@ class Predictor {
   void GetOutput(size_t i, float* out, size_t size) const {
     const Node& n = nodes_[Head(i)];
     if (size != static_cast<size_t>(Numel(n.shape))) throw std::runtime_error("GetOutput: output " + std::to_string(i) + " has " + std::to_string(Numel(n.shape)) + " values, buffer holds " + std::to_string(size));
-    memcpy(out, storages_[n.storage].ptr, size * sizeof(float));
+    memcpy(out, storages_[StorageOf(heads_[i])].ptr, size * sizeof(float));
   }
   size_t ArenaBytes() const { return static_cast<size_t>(arena_floats_) * sizeof(float); }
   size_t NumOps() const { return order_.size(); }
@@ -329,6 +346,7 @@ class Predictor {
   friend class DevicePredictor;        // runs this plan on the GPU: reads the graph, the order and the storages
   Predictor(const Predictor&) = default;
   bool host_arena_ = true;             // false: the arena lives on the device, only its size is planned here
+  const ExtendedOps* extended_ = nullptr;
   int64_t arena_floats_ = 0;
   std::shared_ptr<JValue> doc_;
   std::vector<Node> nodes_;
@@ -341,6 +359,7 @@ class Predictor {
   std::vector<float> arena_;
 
   int Head(size_t i) const { if (i >= heads_.size()) throw std::runtime_error("output index out of range"); return heads_[i].node; }
+  int StorageOf(const Entry& e) const { const Node& n = nodes_[e.node]; return e.index == 0 ? n.storage : n.more_storage.at(e.index - 1); }
 
   // ---- graph construction (both dialects)
   void BuildGraph(const std::vector<std::string>& output_keys) {
@@ -388,12 +407,18 @@ class Predictor {
       heads_.clear();
       for (auto& k : output_keys) {
         int found = -1;
-        for (int i = 0; i < n; ++i) if (nodes_[i].name == k || nodes_[i].name + "_output" == k) found = i;
+        int index = 0;
+        for (int i = 0; i < n; ++i) {
+          if (nodes_[i].name == k || nodes_[i].name + "_output" == k) { found = i; index = 0; }
+          // the device's set: output j of a multi-output node by the general executor's name, "<name>_output<j>"
+          else if (extended_)
+            for (int j = 0, m = extended_->num_outputs(nodes_[i]); m > 1 && j < m; ++j) if (k == nodes_[i].name + "_output" + std::to_string(j)) { found = i; index = j; }
+        }
         if (found < 0) throw std::runtime_error("output " + k + " is not a node of the graph");
-        heads_.push_back(Entry{found, 0});
+        heads_.push_back(Entry{found, index});
       }
     }
-    for (auto& h : heads_) if (h.index != 0) throw std::runtime_error("secondary operator outputs cannot be predictor outputs");
+    if (!extended_) for (auto& h : heads_) if (h.index != 0) throw std::runtime_error("secondary operator outputs cannot be predictor outputs");
   }
 
   void LoadParams(const char* blob, size_t size) {
@@ -421,6 +446,10 @@ class Predictor {
     return op == "Flatten" || op == "flatten" || op == "Reshape" || op == "reshape" || op == "Dropout" || op == "identity" || op == "_copy" ||
            op == "BlockGrad" || op == "stop_gradient" || op == "LinearRegressionOutput" || op == "MAERegressionOutput" || op == "expand_dims";
   }
+  // a view of its input: the planned set's, and the device set's squeeze / Cast / MakeLoss
+  static bool IsView(const Node& nd) {
+    return nd.extended ? (nd.op == "squeeze" || nd.op == "Cast" || nd.op == "MakeLoss") : IsView(nd.op);
+  }
   static bool IsInplace(const std::string& op) {
     static const char* k[] = {"Activation", "LeakyReLU", "relu", "sigmoid", "tanh", "exp", "log", "sqrt", "abs", "negative", "square", "softsign",
                               "clip", "_plus_scalar", "_minus_scalar", "_mul_scalar", "_div_scalar", "_rminus_scalar", "_rdiv_scalar",
@@ -436,12 +465,13 @@ class Predictor {
     std::vector<int> stack;
     for (auto& h : heads_) stack.push_back(h.node);
     while (!stack.empty()) { const int i = stack.back(); stack.pop_back(); if (need[i]) continue; need[i] = 1; for (auto& e : nodes_[i].inputs) stack.push_back(e.node); }
-    std::vector<int> consumers(n, 0);
-    for (int i = 0; i < n; ++i) if (need[i]) for (auto& e : nodes_[i].inputs) ++consumers[e.node];
-    for (auto& h : heads_) consumers[h.node] += 1 << 20;          // outputs stay alive
+    std::map<std::pair<int, int>, int> uses;                       // readers of every (node, output)
+    for (int i = 0; i < n; ++i) if (need[i]) for (auto& e : nodes_[i].inputs) ++uses[{e.node, e.index}];
+    for (auto& h : heads_) uses[{h.node, h.index}] += 1 << 20;    // outputs stay alive
+    auto consumers = [&](int i, int j) { auto it = uses.find({i, j}); return it == uses.end() ? 0 : it->second; };
 
     storages_.clear(); order_.clear(); inputs_.clear();
-    for (auto& nd : nodes_) { nd.known = false; nd.storage = -1; nd.shape.clear(); }
+    for (auto& nd : nodes_) { nd.known = false; nd.storage = -1; nd.shape.clear(); nd.more_storage.clear(); }
     std::vector<int64_t> block_size;
     std::vector<int> free_blocks;
     auto release = [&](int sid) {
@@ -452,7 +482,7 @@ class Predictor {
       if (!need[i]) continue;
       Node& nd = nodes_[i];
       if (nd.op == "null") {
-        Storage s; s.external = true; s.ref = consumers[i];
+        Storage s; s.external = true; s.ref = consumers(i, 0);
         auto in = input_shapes_.find(nd.name);
         if (in != input_shapes_.end()) {
           nd.shape = in->second; nd.known = true;
@@ -468,17 +498,14 @@ class Predictor {
         nd.storage = static_cast<int>(storages_.size()); storages_.push_back(s);
         continue;
       }
-      for (auto& e : nd.inputs) if (e.index != 0) throw std::runtime_error(nd.name + ": reads a secondary output, which the native predictor does not produce");
+      if (!extended_) for (auto& e : nd.inputs) if (e.index != 0) throw std::runtime_error(nd.name + ": reads a secondary output, which the native predictor does not produce");
+      for (auto& e : nd.inputs) CheckOutput(e, nd.name);
       InferShape(nd);
       const int64_t numel = Numel(nd.shape);
       const Node* src = nd.inputs.empty() ? nullptr : &nodes_[nd.inputs[0].node];
-      if (IsView(nd.op) && src->known) {
-        nd.storage = src->storage;
-        storages_[nd.storage].ref += consumers[i];
-      } else if (IsInplace(nd.op) && !storages_[src->storage].external && storages_[src->storage].ref == 1 && consumers[i] > 0) {
-        nd.storage = src->storage;
-        storages_[nd.storage].ref += consumers[i];
-      } else {
+      const int src_storage = src ? StorageOf(nd.inputs[0]) : -1;
+      // a fresh block of the arena for output j, best fit among the free ones
+      auto alloc = [&](int j) {
         int best = -1;
         for (size_t f = 0; f < free_blocks.size(); ++f) {
           const int b = free_blocks[f];
@@ -491,12 +518,23 @@ class Predictor {
           for (size_t f = 1; f < free_blocks.size(); ++f) if (block_size[free_blocks[f]] > block_size[free_blocks[g]]) g = f;
           blk = free_blocks[g]; free_blocks.erase(free_blocks.begin() + g); block_size[blk] = numel;
         } else { blk = static_cast<int>(block_size.size()); block_size.push_back(numel); }
-        Storage s; s.block = blk; s.size = numel; s.ref = std::max(consumers[i], 1);
-        nd.storage = static_cast<int>(storages_.size()); storages_.push_back(s);
-        if (consumers[i] == 0) release(nd.storage);
+        Storage s; s.block = blk; s.size = numel; s.ref = std::max(consumers(i, j), 1);
+        const int sid = static_cast<int>(storages_.size()); storages_.push_back(s);
+        if (consumers(i, j) == 0) release(sid);
+        return sid;
+      };
+      if (IsView(nd) && src->known) {
+        nd.storage = src_storage;
+        storages_[nd.storage].ref += consumers(i, 0);
+      } else if (!nd.extended && IsInplace(nd.op) && !storages_[src_storage].external && storages_[src_storage].ref == 1 && consumers(i, 0) > 0) {
+        nd.storage = src_storage;
+        storages_[nd.storage].ref += consumers(i, 0);
+      } else {
+        nd.storage = alloc(0);
+        for (int j = 1; j < nd.num_out; ++j) nd.more_storage.push_back(alloc(j));
       }
       order_.push_back(i);
-      for (auto& e : nd.inputs) if (nodes_[e.node].storage >= 0) release(nodes_[e.node].storage);
+      for (auto& e : nd.inputs) if (nodes_[e.node].storage >= 0) release(StorageOf(e));
     }
     std::vector<int64_t> offset(block_size.size(), 0);
     int64_t total = 0;
@@ -505,6 +543,13 @@ class Predictor {
     arena_.assign(host_arena_ ? static_cast<size_t>(total) : 0, 0.f);
     for (auto& s : storages_) if (!s.external) { s.offset = offset[s.block]; s.ptr = host_arena_ ? arena_.data() + s.offset : nullptr; }
     for (auto& h : heads_) if (!nodes_[h.node].known) throw std::runtime_error("output " + nodes_[h.node].name + " has no shape");
+    for (auto& h : heads_) CheckOutput(h, "the graph's outputs");
+  }
+  // an entry names an output its node has (the producer is planned first: its output count is known)
+  void CheckOutput(const Entry& e, const std::string& who) const {
+    const Node& src = nodes_[e.node];
+    if (e.index < 0 || e.index >= src.num_out)
+      throw std::runtime_error(who + ": reads output " + std::to_string(e.index) + " of " + src.name + ", which has " + std::to_string(src.num_out) + " output(s)");
   }
 
   const Node& In(const Node& nd, size_t i) const {
@@ -685,7 +730,10 @@ class Predictor {
                op == "_copy" || op == "BlockGrad" || op == "stop_gradient" || op == "clip" || ScalarKind(op) >= 0 || UnaryKind(op) >= 0) {
       nd.shape = InShape(nd, 0);
     } else {
-      throw std::runtime_error("operator " + op + " (node " + nd.name + ") is not supported by the native predictor");
+      if (extended_ == nullptr || !extended_->has(op)) throw std::runtime_error("operator " + op + " (node " + nd.name + ") is not supported by the native predictor");
+      std::vector<const Node*> in;
+      for (size_t i = 0; i < nd.inputs.size(); ++i) { InShape(nd, i); in.push_back(&In(nd, i)); }
+      extended_->infer(nd, in);
     }
     nd.known = true;
   }

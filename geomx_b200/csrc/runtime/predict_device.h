@@ -1,5 +1,6 @@
 // The planned predictor on an H100 (GXPredCreate* with dev_type 2): predict.h's graph, shape inference and liveness-planned arena, run as
-// sm_90a kernels (kernels/predict_dev.cu).
+// sm_90a kernels (kernels/predict_dev.cu).  On the device the planner also takes the general executor's other operators (namespace
+// extended below), so every graph the host serves, on either engine, runs here.
 //
 // libgeomx_capi.so links no CUDA: the kernels library is dlopen'ed from the directory this library was loaded from, on the first device
 // request, and reached through its `gx_pred_*` entry points only.  Parameters go to the device once, at create, together with what is
@@ -15,6 +16,7 @@
 #include <mutex>
 #include <type_traits>
 
+#include "graph.h"
 #include "predict.h"
 
 namespace gxrt {
@@ -52,6 +54,19 @@ struct DeviceApi {
   long long (*conv_workspace)(int, int, int, int, int, int, int, int);
   int (*conv)(const float*, const float*, long long, const float*, float*, float*, long long, int, int, int, int, int, int, int, int, int, int, int, int,
               int, int, int, int, void*);
+  int (*gather)(const float*, float*, long long, int, const long long*, int, float, void*);
+  int (*take)(const float*, const float*, float*, long long, long long, long long, long long, void*);
+  int (*one_hot)(const float*, float*, long long, long long, float, float, void*);
+  int (*where)(const float*, const float*, const float*, float*, long long, void*);
+  int (*arg)(const float*, float*, long long, long long, long long, int, void*);
+  int (*reduce)(int, const float*, float*, long long, int, const long long*, int, const long long*, float, void*);
+  int (*norm)(int, const float*, const float*, const float*, float*, long long, long long, long long, float, void*);
+  int (*lrn)(const float*, float*, long long, long long, long long, long long, float, float, float, void*);
+  int (*softmax_ce)(const float*, const float*, float*, long long, long long, void*);
+  int (*dot)(const float*, const float*, float*, int, int, int, int, int, void*);
+  long long (*deconv_workspace)(int, int, int, int, int, int, int, int);
+  int (*deconv)(const float*, const float*, const float*, float*, float*, long long, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
+                int, int, void*);
 
   void Check(int rc, const std::string& what) const { if (rc != 0) throw std::runtime_error(what + " failed: " + error_string(rc)); }
 
@@ -89,11 +104,92 @@ struct DeviceApi {
     sym(a->map, "gx_pred_map"); sym(a->pointwise, "gx_pred_pointwise"); sym(a->affine, "gx_pred_affine"); sym(a->binary, "gx_pred_binary");
     sym(a->transpose, "gx_pred_transpose"); sym(a->add_n, "gx_pred_add_n"); sym(a->concat_part, "gx_pred_concat_part"); sym(a->softmax, "gx_pred_softmax");
     sym(a->embedding, "gx_pred_embedding"); sym(a->pool, "gx_pred_pool"); sym(a->fc, "gx_pred_fc"); sym(a->conv_workspace, "gx_pred_conv_workspace");
-    sym(a->conv, "gx_pred_conv");
+    sym(a->conv, "gx_pred_conv"); sym(a->gather, "gx_pred_gather"); sym(a->take, "gx_pred_take"); sym(a->one_hot, "gx_pred_one_hot");
+    sym(a->where, "gx_pred_where"); sym(a->arg, "gx_pred_arg"); sym(a->reduce, "gx_pred_reduce"); sym(a->norm, "gx_pred_norm"); sym(a->lrn, "gx_pred_lrn");
+    sym(a->softmax_ce, "gx_pred_softmax_ce"); sym(a->dot, "gx_pred_dot"); sym(a->deconv_workspace, "gx_pred_deconv_workspace");
+    sym(a->deconv, "gx_pred_deconv");
     if (!missing.empty()) return path + " has no entry point " + missing + " (an older build?)";
     return "";
   }
 };
+
+// ------------------------------------------------------------------------------------------------ the device-only operator set
+// Every operator of the general executor (train_exec.h Executor::Run) that the planned set lacks.  Its nodes are planned with the general
+// executor's canonical names, string attributes and shape rules (graph.h), so the device reads a graph exactly as the general executor does.
+namespace extended {
+
+// the node as the general executor's graph sees it; inputs carry only their names (InferNode's messages)
+inline graph::Node GraphNode(const Node& nd, const std::vector<const Node*>& in = {}) {
+  graph::Node g;
+  g.op = graph::CanonicalOp(nd.op); g.name = nd.name; g.attrs = nd.sattrs;
+  for (const Node* i : in) { auto v = std::make_shared<graph::Node>(); v->name = i->name; g.inputs.push_back(graph::Entry{v, 0}); }
+  return g;
+}
+inline std::map<std::string, std::string> StringAttrs(const Node& nd) {
+  std::map<std::string, std::string> m;
+  const JValue* o = nd.attrs.Object();
+  if (o == nullptr || o->kind != JValue::kObj) return m;
+  for (auto& kv : o->obj) {
+    if (kv.first == "__attr__" && kv.second.kind == JValue::kObj) { for (auto& u : kv.second.obj) m[u.first] = graph::JAttrToString(u.second); continue; }
+    if (kv.second.kind != JValue::kNull) m[kv.first] = graph::JAttrToString(kv.second);
+  }
+  return m;
+}
+inline int NumOutputs(const Node& nd) {
+  if (graph::CanonicalOp(nd.op) != "SliceChannel") return 1;
+  Node t = nd; t.sattrs = StringAttrs(nd);
+  return graph::NumOutputs(GraphNode(t));
+}
+inline bool Has(const std::string& op) { return graph::FindOp(op) != nullptr; }
+// graph.h FromJSON's checks first: a variadic operator's count attribute defaults to its inputs, and the input count must be the operator's
+inline void Infer(Node& nd, const std::vector<const Node*>& in) {
+  nd.sattrs = StringAttrs(nd);
+  const graph::OpDef& d = graph::GetOp(nd.op);
+  if (*d.key_var_num_args && !graph::AttrView(nd.sattrs).Has(d.key_var_num_args)) nd.sattrs[d.key_var_num_args] = std::to_string(in.size());
+  const size_t want = d.inputs(graph::AttrView(nd.sattrs)).size();
+  if (in.size() != want)
+    throw std::runtime_error(nd.name + " (" + d.name + "): " + std::to_string(in.size()) + " inputs in the file, the operator takes " + std::to_string(want));
+  const graph::Node g = GraphNode(nd, in);
+  std::vector<const Shape*> shapes;
+  for (const Node* i : in) shapes.push_back(&i->shape);
+  Shape out;
+  if (!graph::InferNode(g, shapes, [](size_t, const Shape&) {}, &out)) throw std::runtime_error(nd.name + " (" + g.op + "): the output shape cannot be inferred");
+  nd.op = g.op; nd.extended = true; nd.num_out = graph::NumOutputs(g); nd.shape = out;
+}
+inline const ExtendedOps* Ops() { static const ExtendedOps ops{&Has, &NumOutputs, &Infer}; return &ops; }
+
+// the general executor's unary kinds that the planned set lacks, in the order of train_exec.h Un() (device kinds 11..30)
+inline int UnaryKind(const std::string& op) {
+  static const char* names[] = {"sin", "cos", "tan", "arcsin", "arccos", "arctan", "sinh", "cosh", "log1p", "expm1", "log2", "log10", "rsqrt", "reciprocal",
+                                "cbrt", "erf", "floor", "ceil", "round", "sign"};
+  for (int i = 0; i < 20; ++i) if (op == names[i]) return 11 + i;
+  return -1;
+}
+// binary power and comparisons (device kinds 6..12), scalar power / max / min (pointwise modes 9..12)
+inline int BinaryKind(const std::string& op) {
+  static const char* names[] = {"broadcast_power", "broadcast_equal", "broadcast_not_equal", "broadcast_greater", "broadcast_greater_equal", "broadcast_lesser",
+                                "broadcast_lesser_equal"};
+  for (int i = 0; i < 7; ++i) if (op == names[i]) return 6 + i;
+  return -1;
+}
+inline int ScalarMode(const std::string& op) {
+  static const char* names[] = {"_power_scalar", "_rpower_scalar", "_maximum_scalar", "_minimum_scalar"};
+  for (int i = 0; i < 4; ++i) if (op == names[i]) return 9 + i;
+  return -1;
+}
+inline bool IsGather(const std::string& op) {
+  static const char* names[] = {"slice_axis", "slice", "SwapAxis", "tile", "repeat", "Pad", "reverse", "broadcast_to", "broadcast_axis", "UpSampling", "SliceChannel"};
+  for (auto n : names) if (op == n) return true;
+  return false;
+}
+inline bool IsReduce(const std::string& op) { return op == "sum" || op == "mean" || op == "max" || op == "min" || op == "prod" || op == "norm"; }
+inline void SplitAxis(const Shape& s, int64_t ax, int64_t* outer, int64_t* c, int64_t* inner) {
+  *outer = 1; *inner = 1; *c = s[ax];
+  for (int64_t i = 0; i < ax; ++i) *outer *= s[i];
+  for (size_t i = ax + 1; i < s.size(); ++i) *inner *= s[i];
+}
+
+}  // namespace extended
 
 // makes `dev` current for its lifetime and gives the caller's device back.  A thread that had no current CUDA context keeps `dev`:
 // "restoring" the device 0 that cudaGetDevice reports for such a thread would create a context on a GPU the caller never used.
@@ -208,7 +304,7 @@ class DevicePredictor {
     const Node& n = plan_->nodes_[plan_->Head(i)];
     if (size != static_cast<size_t>(Numel(n.shape))) throw std::runtime_error("GetOutput: output " + std::to_string(i) + " has " + std::to_string(Numel(n.shape)) + " values, buffer holds " + std::to_string(size));
     DeviceGuard g(api_, dev_);
-    api_.Check(api_.d2h(out, ptr_[n.storage], size * sizeof(float), stream_), "GetOutput: device-to-host copy");
+    api_.Check(api_.d2h(out, ptr_[plan_->StorageOf(plan_->heads_[i])], size * sizeof(float), stream_), "GetOutput: device-to-host copy");
     api_.Check(api_.stream_sync(stream_), "GetOutput: stream synchronisation");
   }
   size_t ArenaBytes() const { return plan_->ArenaBytes(); }
@@ -232,7 +328,7 @@ class DevicePredictor {
 
   const Node& In(const Node& nd, size_t i) const { return plan_->In(nd, i); }
   float* Ptr(const Node& nd) const { return ptr_[nd.storage]; }
-  const float* InPtr(const Node& nd, size_t i) const { return ptr_[In(nd, i).storage]; }
+  const float* InPtr(const Node& nd, size_t i) const { In(nd, i); return ptr_[plan_->StorageOf(nd.inputs[i])]; }
   bool IsParam(const Node& nd, size_t i) const {
     const Node& s = In(nd, i);
     return s.op == "null" && !plan_->input_shapes_.count(s.name) && plan_->params_->count(s.name);
@@ -248,7 +344,8 @@ class DevicePredictor {
     for (int id : p.order_) {
       const Node& nd = p.nodes_[id];
       const std::string& op = nd.op;
-      if (Predictor::IsView(op)) continue;
+      if (Predictor::IsView(nd)) continue;
+      if (nd.extended) { ValidateExtended(nd); continue; }
       const Attrs& a = nd.attrs;
       if (op == "Activation") {
         const std::string t = a.Str("act_type", "relu");
@@ -338,7 +435,14 @@ class DevicePredictor {
     ws_floats_ = 0;
     for (int id : p.order_) {
       const Node& nd = p.nodes_[id];
-      if (nd.op != "Convolution") continue;
+      if (nd.extended && nd.op == "Deconvolution") {
+        const graph::detail::Win w = graph::detail::Window(extended::GraphNode(nd), false, In(nd, 0).shape);
+        const Shape& xs = In(nd, 0).shape;
+        const int64_t G = graph::AttrView(nd.sattrs).Int("num_group", 1);
+        ws_floats_ = std::max(ws_floats_, api_.deconv_workspace((int)xs[0], (int)xs[1], (int)xs[2], (int)xs[3], (int)(nd.shape[1] / G), (int)w.kh, (int)w.kw, (int)G));
+        continue;
+      }
+      if (nd.op != "Convolution" || nd.extended) continue;
       const Predictor::Conv c = p.ConvAttrs(nd);
       const Shape& xs = In(nd, 0).shape;
       const bool pointwise = c.kh == 1 && c.kw == 1 && c.sh == 1 && c.sw == 1 && c.ph == 0 && c.pw == 0;
@@ -374,7 +478,8 @@ class DevicePredictor {
     const Predictor& p = *plan_;
     const Node& nd = p.nodes_[id];
     const std::string& op = nd.op;
-    if (Predictor::IsView(op)) return;
+    if (Predictor::IsView(nd)) return;
+    if (nd.extended) { EnqueueExtended(nd); return; }
     const Attrs& a = nd.attrs;
     void* s = stream_;
     float* y = Ptr(nd);
@@ -444,16 +549,7 @@ class DevicePredictor {
       const Shape& w = In(nd, 1).shape;
       Check(api_.embedding(x, InPtr(nd, 1), y, Numel(xs), w[0], w[1], s), nd);
     } else if ((k = Predictor::BinaryKind(op)) >= 0) {
-      const Shape& ps = In(nd, 0).shape; const Shape& qs = In(nd, 1).shape;
-      if (ps == qs) { Check(api_.binary(k, x, InPtr(nd, 1), y, n, 0, nullptr, nullptr, nullptr, s), nd); return; }
-      const size_t r = nd.shape.size();
-      std::vector<long long> sp(r, 0), sq(r, 0), shape(nd.shape.begin(), nd.shape.end());
-      auto strides = [&](const Shape& sh, std::vector<long long>& out) {
-        long long st = 1;
-        for (int i = static_cast<int>(sh.size()) - 1; i >= 0; --i) { out[i + r - sh.size()] = sh[i] == 1 ? 0 : st; st *= sh[i]; }
-      };
-      strides(ps, sp); strides(qs, sq);
-      Check(api_.binary(k, x, InPtr(nd, 1), y, n, static_cast<int>(r), shape.data(), sp.data(), sq.data(), s), nd);
+      Binary(nd, k);
     } else if ((k = Predictor::ScalarKind(op)) >= 0) {
       Check(api_.pointwise(3 + k, x, y, n, static_cast<float>(a.Float("scalar", 0.0)), 0.f, s), nd);
     } else if (op == "add_n" || op == "ElementWiseSum") {
@@ -463,6 +559,182 @@ class DevicePredictor {
     } else {
       throw std::runtime_error("operator " + op + " has no device kernel");
     }
+  }
+
+  // predict.h RunBinary: operands broadcast over the output's axes
+  void Binary(const Node& nd, int k) {
+    const float* x = InPtr(nd, 0); float* y = Ptr(nd);
+    const long long n = Numel(nd.shape);
+    const Shape& ps = In(nd, 0).shape; const Shape& qs = In(nd, 1).shape;
+    if (ps == qs) { Check(api_.binary(k, x, InPtr(nd, 1), y, n, 0, nullptr, nullptr, nullptr, stream_), nd); return; }
+    const size_t r = nd.shape.size();
+    std::vector<long long> sp(r, 0), sq(r, 0), shape(nd.shape.begin(), nd.shape.end());
+    auto strides = [&](const Shape& sh, std::vector<long long>& out) {
+      long long st = 1;
+      for (int i = static_cast<int>(sh.size()) - 1; i >= 0; --i) { out[i + r - sh.size()] = sh[i] == 1 ? 0 : st; st *= sh[i]; }
+    };
+    strides(ps, sp); strides(qs, sq);
+    Check(api_.binary(k, x, InPtr(nd, 1), y, n, static_cast<int>(r), shape.data(), sp.data(), sq.data(), stream_), nd);
+  }
+
+  // ---- the device-only set: train_exec.h Run's forward branches
+
+  // the kernels take at most 8 axes and extents in 32 bits; Deconvolution indexes its furthest output row / column and its products in 32 bits
+  void ValidateExtended(const Node& nd) const {
+    const std::string& op = nd.op;
+    std::vector<const Shape*> shapes{&nd.shape};
+    for (size_t i = 0; i < nd.inputs.size(); ++i) shapes.push_back(&In(nd, i).shape);
+    for (const Shape* sh : shapes) {
+      if (sh->size() > 8) throw std::runtime_error(nd.name + ": the device kernels take at most 8 axes, got " + ShapeStr(*sh));
+      for (int64_t d : *sh) Int(d, nd);
+    }
+    if (op == "Deconvolution") {
+      const graph::detail::Win w = graph::detail::Window(extended::GraphNode(nd), false, In(nd, 0).shape);
+      const Shape& xs = In(nd, 0).shape;
+      const int64_t G = graph::AttrView(nd.sattrs).Int("num_group", 1);
+      for (int64_t v : {w.kh, w.kw, w.sh, w.sw, w.ph, w.pw, w.dh, w.dw, G}) Int(v, nd);
+      Int(nd.shape[2] + w.ph, nd); Int(nd.shape[3] + w.pw, nd);
+      Int((w.kh - 1) * w.dh, nd); Int((w.kw - 1) * w.dw, nd);
+      Int(xs[2] * xs[3], nd); Int(nd.shape[1] / G * w.kh * w.kw, nd);
+    } else if (!(extended::IsGather(op) || extended::IsReduce(op) || extended::UnaryKind(op) >= 0 || extended::BinaryKind(op) >= 0 ||
+                 extended::ScalarMode(op) >= 0 || op == "take" || op == "pick" || op == "one_hot" || op == "where" || op == "argmax" || op == "argmin" ||
+                 op == "LayerNorm" || op == "InstanceNorm" || op == "L2Normalization" || op == "LRN" || op == "dot" || op == "smooth_l1" ||
+                 op == "softmax_cross_entropy")) {
+      throw std::runtime_error("operator " + op + " (node " + nd.name + ") has no device kernel");
+    }
+  }
+
+  void EnqueueExtended(const Node& nd) {
+    namespace D = graph::detail;
+    const graph::AttrView a(nd.sattrs);
+    const std::string& op = nd.op;
+    void* s = stream_;
+    float* y = Ptr(nd);
+    const long long n = Numel(nd.shape);
+    const float* x = InPtr(nd, 0);
+    const Shape& xs = In(nd, 0).shape;
+    int k;
+    int64_t outer, C, inner;
+    if (op == "SliceChannel") {
+      for (int j = 0; j < nd.num_out; ++j) Gather(nd, j, j == 0 ? y : ptr_[nd.more_storage[j - 1]]);
+    } else if (extended::IsGather(op)) {
+      Gather(nd, 0, y);
+    } else if (op == "take" || op == "pick") {
+      extended::SplitAxis(xs, D::AxisOf(a.Int("axis", op == "take" ? 0 : -1), xs.size(), nd.name), &outer, &C, &inner);
+      Check(api_.take(x, InPtr(nd, 1), y, outer, C, inner, op == "take" ? Numel(In(nd, 1).shape) : 0, s), nd);
+    } else if (op == "one_hot") {
+      Check(api_.one_hot(x, y, n, nd.shape.back(), static_cast<float>(a.Float("on_value", 1)), static_cast<float>(a.Float("off_value", 0)), s), nd);
+    } else if (op == "where") {
+      Check(api_.where(x, InPtr(nd, 1), InPtr(nd, 2), y, n, s), nd);
+    } else if (op == "argmax" || op == "argmin") {
+      extended::SplitAxis(xs, D::AxisOf(a.Int("axis", 0), xs.size(), nd.name), &outer, &C, &inner);
+      Check(api_.arg(x, y, outer, C, inner, op == "argmax", s), nd);
+    } else if (extended::IsReduce(op)) {
+      const auto axes = a.Tuple("axis", {});
+      std::vector<char> red(xs.size(), axes.empty());
+      for (auto ax : axes) red[D::AxisOf(ax, xs.size(), nd.name)] = 1;
+      std::vector<long long> kd, ks, rd, rs;
+      long long st = 1;
+      for (int i = static_cast<int>(xs.size()) - 1; i >= 0; --i) {
+        (red[i] ? rd : kd).insert((red[i] ? rd : kd).begin(), xs[i]);
+        (red[i] ? rs : ks).insert((red[i] ? rs : ks).begin(), st);
+        st *= xs[i];
+      }
+      kd.insert(kd.end(), ks.begin(), ks.end()); rd.insert(rd.end(), rs.begin(), rs.end());
+      const int kind = op == "max" ? 1 : op == "min" ? 2 : op == "prod" ? 3 : op == "norm" ? 4 : 0;
+      const float div = op == "mean" ? static_cast<float>(Numel(xs) / n) : 1.f;
+      Check(api_.reduce(kind, x, y, n, static_cast<int>(ks.size()), kd.data(), static_cast<int>(rs.size()), rd.data(), div, s), nd);
+    } else if (op == "LayerNorm" || op == "InstanceNorm" || op == "L2Normalization") {
+      int mode = 2;
+      float eps = static_cast<float>(a.Float("eps", 1e-10));
+      if (op == "LayerNorm") { mode = 0; eps = static_cast<float>(a.Float("eps", 1e-5)); extended::SplitAxis(xs, D::AxisOf(a.Int("axis", -1), xs.size(), nd.name), &outer, &C, &inner); }
+      else if (op == "InstanceNorm") { mode = 1; eps = static_cast<float>(a.Float("eps", 1e-3)); outer = xs[0]; C = xs[1]; inner = Numel(xs) / (xs[0] * xs[1]); }
+      else {                            // train_exec.h NormGroups
+        const std::string m = a.Str("mode", "instance");
+        const int64_t total = Numel(xs);
+        if (m == "instance") { outer = xs[0]; C = total / xs[0]; inner = 1; }
+        else if (m == "channel" && xs.size() >= 2) { outer = xs[0]; C = xs[1]; inner = total / (xs[0] * xs[1]); }
+        else if (m == "spatial" && xs.size() >= 3) { outer = xs[0] * xs[1]; C = total / (xs[0] * xs[1]); inner = 1; }
+        else throw std::runtime_error(nd.name + ": L2Normalization mode " + m + " is not supported for a tensor of shape " + ShapeStr(xs));
+      }
+      Check(api_.norm(mode, x, mode == 2 ? nullptr : InPtr(nd, 1), mode == 2 ? nullptr : InPtr(nd, 2), y, outer, C, inner, eps, s), nd);
+    } else if (op == "LRN") {
+      const int64_t ns = a.Int("nsize", 1);
+      Check(api_.lrn(x, y, xs[0], xs[1], xs[2] * xs[3], ns / 2, static_cast<float>(a.Float("alpha", 1e-4)) / static_cast<float>(ns),
+                     static_cast<float>(a.Float("beta", 0.75)), static_cast<float>(a.Float("knorm", 2)), s), nd);
+    } else if (op == "Deconvolution") {
+      const D::Win w = D::Window(extended::GraphNode(nd), false, xs);
+      Check(api_.deconv(x, InPtr(nd, 1), nd.inputs.size() > 2 ? InPtr(nd, 2) : nullptr, y, ws_, ws_floats_, (int)xs[0], (int)xs[1], (int)xs[2], (int)xs[3],
+                        (int)nd.shape[1], (int)nd.shape[2], (int)nd.shape[3], (int)w.kh, (int)w.kw, (int)w.sh, (int)w.sw, (int)w.ph, (int)w.pw, (int)w.dh,
+                        (int)w.dw, (int)a.Int("num_group", 1), s), nd);
+    } else if (op == "dot") {
+      const bool ta = a.Bool("transpose_a", false), tb = a.Bool("transpose_b", false);
+      Check(api_.dot(x, InPtr(nd, 1), y, (int)nd.shape[0], (int)nd.shape[1], (int)(ta ? xs[0] : xs[1]), ta, tb, s), nd);
+    } else if (op == "smooth_l1") {
+      const float sg = static_cast<float>(a.Float("scalar", 1));
+      Check(api_.pointwise(13, x, y, n, sg * sg, 0.f, s), nd);
+    } else if (op == "softmax_cross_entropy") {
+      Check(api_.softmax_ce(x, InPtr(nd, 1), y, xs[0], xs[1], s), nd);
+    } else if ((k = extended::UnaryKind(op)) >= 0) {
+      Check(api_.map(k, x, y, n, s), nd);
+    } else if ((k = extended::BinaryKind(op)) >= 0) {
+      Binary(nd, k);
+    } else if ((k = extended::ScalarMode(op)) >= 0) {
+      Check(api_.pointwise(k, x, y, n, static_cast<float>(a.Float("scalar", 0)), 0.f, s), nd);
+    } else {
+      throw std::runtime_error("operator " + op + " has no device kernel");
+    }
+  }
+
+  // train_exec.h BuildMap's per-axis rules as one gather launch; `part` is SliceChannel's output (its slice along the axis)
+  void Gather(const Node& nd, int part, float* y) {
+    namespace D = graph::detail;
+    const graph::AttrView a(nd.sattrs);
+    const std::string& op = nd.op;
+    const Shape& xs = In(nd, 0).shape;
+    Shape os = nd.shape;
+    int64_t split_ax = -1;
+    if (op == "SliceChannel") { split_ax = D::AxisOf(a.Int("axis", 1), xs.size(), nd.name); os = xs; os[split_ax] = xs[split_ax] / nd.num_out; }   // before squeeze_axis
+    const size_t r = os.size();
+    Shape in = xs; while (in.size() < r) in.insert(in.begin(), 1);
+    std::vector<long long> stride(r, 1), off(r, 0), div(r, 1), before(r, 0), flags(r, 0), perm(r);
+    for (int i = static_cast<int>(r) - 2; i >= 0; --i) stride[i] = stride[i + 1] * in[i + 1];
+    for (size_t i = 0; i < r; ++i) perm[i] = static_cast<long long>(i);
+    int pad_mode = -1;
+    float fill = 0.f;
+    if (op == "SliceChannel") {
+      off[split_ax] = part * os[split_ax];
+    } else if (op == "slice_axis") {
+      const int64_t ax = D::AxisOf(a.Int("axis", 0), r, nd.name);
+      int64_t lo, hi; D::SliceRange(a.Has("begin"), a.Int("begin", 0), a.Has("end"), a.Int("end", 0), in[ax], nd.name, &lo, &hi);
+      off[ax] = lo;
+    } else if (op == "slice") {
+      const auto b = D::TupleOpt(a, "begin"), e = D::TupleOpt(a, "end");
+      for (size_t i = 0; i < b.size(); ++i) { int64_t lo, hi; D::SliceRange(b[i].first, b[i].second, e[i].first, e[i].second, in[i], nd.name, &lo, &hi); off[i] = lo; }
+    } else if (op == "SwapAxis") {
+      std::swap(perm[D::AxisOf(a.Int("dim1", 0), r, nd.name)], perm[D::AxisOf(a.Int("dim2", 0), r, nd.name)]);
+    } else if (op == "tile") {
+      for (size_t i = 0; i < r; ++i) flags[i] = 1;
+    } else if (op == "repeat") {
+      div[D::AxisOf(a.Int("axis", 0), r, nd.name)] = a.Int("repeats", 1);
+    } else if (op == "UpSampling") {
+      div[2] = div[3] = a.Int("scale", 1);
+    } else if (op == "reverse") {
+      for (auto ax : a.Tuple("axis", {})) flags[D::AxisOf(ax, r, nd.name)] = 2;
+    } else if (op == "broadcast_to" || op == "broadcast_axis") {
+      for (size_t i = 0; i < r; ++i) flags[i] = in[i] == 1 && os[i] != 1 ? 4 : 0;
+    } else if (op == "Pad") {
+      const auto pw = a.Tuple("pad_width", {});
+      for (size_t i = 0; i < r; ++i) before[i] = pw[2 * i];
+      const std::string mode = a.Str("mode", "constant");
+      pad_mode = mode == "constant" ? 0 : mode == "edge" ? 1 : 2;
+      fill = static_cast<float>(a.Float("constant_value", 0));
+    }
+    std::vector<long long> rule;
+    for (auto* row : {&os, &in}) rule.insert(rule.end(), row->begin(), row->end());
+    for (size_t i = 0; i < r; ++i) rule.push_back(stride[perm[i]]);
+    for (auto* row : {&before, &div, &off, &flags}) rule.insert(rule.end(), row->begin(), row->end());
+    Check(api_.gather(InPtr(nd, 0), y, Numel(os), static_cast<int>(r), rule.data(), pad_mode, fill, stream_), nd);
   }
 
   // predict.h Softmax: (outer, C, inner) around `axis` of `shape`
