@@ -89,9 +89,13 @@ class HybridConcurrent(HybridSequential):
         super().__init__(prefix=prefix, params=params); self.axis = axis
 
     def forward(self, x):
+        from ...symbol import Symbol
+        if isinstance(x, Symbol):                     # export traces hybrid_forward
+            return HybridBlock.forward(self, x)
         return NDArray(torch.cat([blk(x)._t for blk in self._children.values()], dim=self.axis))
 
-    hybrid_forward = None
+    def hybrid_forward(self, F, x):
+        return F.concat(*[blk(x) for blk in self._children.values()], dim=self.axis)
 
 
 class Identity(HybridBlock):

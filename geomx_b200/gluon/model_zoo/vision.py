@@ -208,9 +208,8 @@ class _Fire(HybridBlock):
             self.e3 = nn.Conv2D(e3, 3, padding=1, activation="relu")
 
     def hybrid_forward(self, F, x):
-        from ... import ndarray as nd
         s = self.squeeze(x)
-        return nd.concat(self.e1(s), self.e3(s), dim=1)
+        return F.concat(self.e1(s), self.e3(s), dim=1)
 
 
 class SqueezeNet(HybridBlock):
@@ -268,8 +267,7 @@ class _DenseLayer(HybridBlock):
                 b.add(nn.Dropout(dropout))
 
     def hybrid_forward(self, F, x):
-        from ... import ndarray as nd
-        return nd.concat(x, self.body(x), dim=1)
+        return F.concat(x, self.body(x), dim=1)
 
 
 class DenseNet(HybridBlock):
@@ -312,8 +310,7 @@ class _Branches(HybridBlock):
             setattr(self, "b%d" % i, b)
 
     def hybrid_forward(self, F, x):
-        from ... import ndarray as nd
-        return nd.concat(*[getattr(self, "b%d" % i)(x) for i in range(self._n)], dim=1)
+        return F.concat(*[getattr(self, "b%d" % i)(x) for i in range(self._n)], dim=1)
 
 
 def _seq(*blocks):

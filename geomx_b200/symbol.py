@@ -635,6 +635,25 @@ def _nd_param_shape(a, pname, in_shape):
     return None
 
 
+def _bind_positional(qual, args, kwargs):
+    """Bind the positional arguments from the first non-Symbol one on to the imperative function's parameter names, so that
+    ``mx.sym.clip(x, 0, 6)``, ``x.clip(0, 6)`` and ``F.clip(x, 0, 6)`` in a traced block mean ``clip(x, a_min=0, a_max=6)`` as in the
+    reference's generated ``mx.sym`` functions.  Returns the leading Symbols (still positional) and the keyword arguments."""
+    import inspect
+    first = next(i for i, x in enumerate(args) if not isinstance(x, Symbol))
+    refuse = MXNetError("mx.sym.%s: positional arguments must be Symbols, pass attributes by keyword" % qual)
+    try:
+        params = list(inspect.signature(_resolve_nd(qual)).parameters.values())
+    except (AttributeError, TypeError, ValueError):
+        raise refuse from None
+    kwargs = dict(kwargs)
+    for i in range(first, len(args)):
+        if i >= len(params) or any(p.kind != p.POSITIONAL_OR_KEYWORD for p in params[:i + 1]) or params[i].name in kwargs:
+            raise refuse
+        kwargs[params[i].name] = args[i]
+    return list(args[:first]), kwargs
+
+
 def _nd_op(qual):
     def build(*args, name=None, **kwargs):
         auto = _AUTO_PARAMS.get(qual)
@@ -647,7 +666,7 @@ def _nd_op(qual):
                     kwargs[pn] = Variable("%s_%s" % (name, pn))
         pos = [x for x in args if isinstance(x, Symbol)]
         if len(pos) != len(args):
-            raise MXNetError("mx.sym.%s: positional arguments must be Symbols, pass attributes by keyword" % qual)
+            pos, kwargs = _bind_positional(qual, args, kwargs)
         skw = [k for k, v in kwargs.items() if isinstance(v, Symbol)]
         attrs = {"fn": qual, "npos": len(pos), "sym_kwargs": skw,
                  "kwargs": {k: (list(v) if isinstance(v, tuple) else v) for k, v in kwargs.items() if k not in skw}}

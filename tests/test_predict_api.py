@@ -266,3 +266,74 @@ def test_hybridblock_export_traces_a_graph(tmp_path):
             return mx.nd.NDArray(x._t * 2)
     with pytest.raises(MXNetError, match="no symbolic rule"):
         Opaque().export(str(tmp_path / "op"))
+
+
+def _zoo_names():
+    from geomx_b200.gluon.model_zoo import vision
+    return sorted(vision._models)
+
+
+@pytest.mark.parametrize("name", _zoo_names())
+def test_model_zoo_exports_and_serves(tmp_path, name):
+    """Every network of get_model's table at the smallest input its family accepts: it exports in both JSON dialects, and the host
+    predictor's output matches the imperative forward and the fp64 evaluation of the exported graph, with the same bytes from both."""
+    from test_predict_gpu import ZOO_SIZE, export_net, fp32_tol, ref_eval, rel_err, zoo_net
+    net, x = zoo_net(name, 2, ZOO_SIZE.get(name, 32))
+    with mx.autograd.predict_mode():
+        want = net(mx.nd.array(x)).asnumpy()
+    outs = []
+    for nnvm in (False, True):
+        text, blob, params = export_net(net, str(tmp_path / name), nnvm=nnvm)
+        assert ("arg_nodes" in json.loads(text)) == nnvm
+        p = predictor.Predictor(text, blob, {"data": x.shape})
+        engine = ctypes.c_int()
+        assert predictor._lib().GXPredGetEngine(p._h, ctypes.byref(engine)) == 0 and engine.value == 1     # the planned interpreter
+        p.forward(data=x)
+        outs.append(p.get_output(0))
+        ref = ref_eval(text, params, {"data": x})
+        tol = fp32_tol(net, x, ref)[0]
+        assert rel_err(outs[-1], ref) <= tol, (nnvm, rel_err(outs[-1], ref))
+    assert outs[0].shape == want.shape == (2, 7)
+    assert rel_err(outs[0], want.astype(np.float64)) <= tol, rel_err(outs[0], want.astype(np.float64))
+    assert outs[0].tobytes() == outs[1].tobytes()
+
+
+def test_user_blocks_with_concurrent_branches_and_clip_export(tmp_path):
+    """HybridConcurrent (an Identity branch beside a layer) and ReLU6 written as F.clip(x, 0, 6) / mx.sym.clip(x, 0, 6) export and serve."""
+    from geomx_b200 import gluon
+    from geomx_b200.gluon import nn
+    from geomx_b200.gluon.contrib.nn import HybridConcurrent, Identity
+
+    class ReLU6(gluon.HybridBlock):
+        def hybrid_forward(self, F, x):
+            return F.clip(x, 0, 6)
+
+    net = nn.HybridSequential()
+    cat = HybridConcurrent(axis=1)
+    cat.add(Identity(), nn.Conv2D(3, 3, padding=1))
+    net.add(nn.Conv2D(4, 1), cat, ReLU6(), nn.Dense(5))
+    net.initialize(mx.init.Xavier())
+    x = np.random.RandomState(0).randn(2, 2, 6, 6).astype(np.float32) * 8
+    with mx.autograd.predict_mode():
+        want = net(mx.nd.array(x)).asnumpy()
+    for nnvm in (False, True):
+        net.export(str(tmp_path / "blk"), nnvm=nnvm)
+        text = open(str(tmp_path / "blk-symbol.json")).read()
+        assert text.count('"concat"') == 1 and text.count('"clip"') == 1, text
+        p = predictor.Predictor(text, open(str(tmp_path / "blk-0000.params"), "rb").read(), {"data": x.shape})
+        p.forward(data=x)
+        np.testing.assert_allclose(p.get_output(0), want, rtol=1e-5, atol=1e-5)
+    # positional attributes bind to mx.nd.clip's parameter names, from mx.sym and from Symbol.clip
+    data = sym.Variable("data")
+    xs = np.linspace(-9, 9, 12, dtype=np.float32).reshape(3, 4)
+    for s in (sym.clip(data, 0, 6), data.clip(0, 6), sym.clip(data, 0, a_max=6)):
+        assert s.attrs["kwargs"] == {"a_min": 0, "a_max": 6}
+        p = predictor.Predictor(s.tojson(nnvm=True), b"", {"data": xs.shape})
+        p.forward(data=xs)
+        np.testing.assert_array_equal(p.get_output(0), np.clip(xs, 0, 6))
+    with pytest.raises(MXNetError, match="positional arguments must be Symbols"):
+        sym.clip(data, 0, 6, 7)                                  # more values than clip has parameters
+    with pytest.raises(MXNetError, match="positional arguments must be Symbols"):
+        sym.clip(data, 0, a_min=1)                               # a_min twice
+    with pytest.raises(MXNetError, match="positional arguments must be Symbols"):
+        sym.concat(data, 1)                                      # concat's arrays are variadic
